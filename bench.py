@@ -1,11 +1,12 @@
 #!/usr/bin/env python
 """bench.py -- BASELINE.json metric: 1024x1024 tiles/s for embedding precompute + AMG (vit_b, 32x32 point grid, batch of 16
-synthetic LM tiles = BASELINE.json configs[1]) on N B200s, plus the ViT-H encoder forward as a fraction of the bf16
+synthetic LM tiles = BASELINE.json configs[1]) on N H100s, plus the ViT-H encoder forward as a fraction of the bf16
 tensor-core roofline.
 
   python bench.py --gpus N --steps K --warmup W            # ours (torchrun for N > 1, one rank per GPU, weak scaling)
   python bench.py --impl reference --gpus N --steps K ...  # the reference algorithm's CPU path (oracle port) on host cores
   python bench.py --config cfg1|cfg3|cfg4|cfg5 ...                   # the other BASELINE.json GPU configurations (extra JSON lines)
+  python bench.py ... --dump-outputs DIR                   # also write what the last timed step computed, as DIR/<name>.npy
 
 One "step" = one pass of the hot path over one batch of 16 tiles per GPU.  BOTH arms run the same workload
 (`workload_config`): same tiles, same seeded weights, same point grid and the same generate() thresholds, chosen so that
@@ -15,7 +16,7 @@ the thresholds-0.0 worst case (every mask reaches the NMS) is timed as an extra 
   e2e   : tiles/s through the reference-facing API (precompute_image_embeddings + AutomaticMaskGenerator.initialize /
           generate) from HOST uint16 tiles to HOST uint32 label images; H2D / D2H inside the timed region.
 Timing: CUDA events on the launching stream, barrier + synchronize on both sides, max over ranks.  Every step streams
-multi-GB decoder activations (>> 126 MB L2), so no extra L2 flush is needed ("l2": "working_set_exceeds_l2").
+multi-GB decoder activations (>> 50 MB L2), so no extra L2 flush is needed ("l2": "working_set_exceeds_l2").
 """
 import argparse
 import json
@@ -63,7 +64,8 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16; no sustained rate has been measured
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "datasheet"
 
 
 class ClockSampler:
@@ -188,8 +190,7 @@ def run_reference(args):
 # ---------------------------------------------------------------------------------------------------- our arm
 def vit_h_roofline(device, steps=3):
     """ViT-H encoder forward: ms/tile and fraction of the bf16 tensor roofline.  Measured at batch 4 and 8 tiles (distinct
-    uint8 tiles each step, so nothing is cached): at batch 4 the fp32 residual stream (84 MB) stays in the 126 MB L2,
-    at batch 8 it does not -- the better of the two is reported together with its batch."""
+    uint8 tiles each step, so nothing is cached); the better of the two is reported together with its batch."""
     from oracle import sam_ref  # weights only (seeded generator); nothing of the oracle is timed here
     from micro_sam_b200 import _lib
     from micro_sam_b200.sam import B200Sam
@@ -222,7 +223,7 @@ def vit_h_roofline(device, steps=3):
     return best, [dict(r, ms_per_tile=r["ms"] / best[1]) for r in rep]
 
 
-def kernel_table(rep, steps, pk, dev_ms_per_step, traffic):
+def kernel_table(rep, steps, pk, dev_ms_per_step):
     """Per-kernel rows from the library's CUDA-event records: time share, achieved algorithmic TFLOP/s and GB/s against the
     two rooflines; `bound` = the roofline that gives the larger lower bound on the kernel's time."""
     rows = []
@@ -234,11 +235,26 @@ def kernel_table(rep, steps, pk, dev_ms_per_step, traffic):
         f_t, f_h = tf / pk["bf16_tflops_sustained"], gbs / pk["hbm_gbs"]
         row = {"kernel": r["name"], "ms_per_step": ms, "launches_per_step": n, "share_of_step": ms / dev_ms_per_step,
                "tflops": tf, "gbs": gbs, "frac_tensor": f_t, "frac_hbm": f_h, "bound": "tensor" if f_t >= f_h else "hbm"}
-        t = traffic.get(r["name"])
-        if t:
-            row["dram_bytes_per_launch_ncu"] = t["bytes_per_launch"]
         rows.append(row)
     return rows
+
+
+def dump_outputs(path, last):
+    """Writes what the last timed step returned to its caller, as float32 .npy files (~25 MB in all): `iou_preds` [16, 3072]
+    (every tile), and fixed seeded samples of the larger outputs -- `labels` [16, 262144] (the same pixels of every tile's
+    label image) and `features` [2097152] (elements of the [16, 256, 64, 64] image embeddings)."""
+    os.makedirs(path, exist_ok=True)
+    rng = np.random.default_rng(1234)
+    pix = torch.from_numpy(np.sort(rng.choice(TILE * TILE, 262144, replace=False)))
+    feat = last["features"].reshape(-1)
+    idx = torch.from_numpy(np.sort(rng.choice(feat.numel(), 2097152, replace=False)))
+    arrays = {
+        "labels": torch.stack([l.reshape(-1)[pix.to(l.device)] for l in last["labels"]]).float(),
+        "iou_preds": torch.stack([v.reshape(-1) for v in last["iou_preds"]]).float(),
+        "features": feat[idx.to(feat.device)].float(),
+    }
+    for name, a in arrays.items():
+        np.save(os.path.join(path, f"{name}.npy"), a.cpu().numpy().astype(np.float32))
 
 
 def run_ours(args):
@@ -253,10 +269,6 @@ def run_ours(args):
     from oracle import sam_ref  # seeded weight generator only
     from micro_sam_b200 import _lib, instance_segmentation as iseg, sam as sam_mod, util
     pk, pk_src = peaks()
-    traffic = {}
-    tp = os.path.join(ROOT, "profiles", "r2_dram_traffic.json")
-    if os.path.exists(tp):
-        traffic = json.load(open(tp))
 
     sd = sam_ref.seeded_state_dict(args.model, seed=0)
     pred = util.get_sam_model(args.model, device=device, state_dict=sd, max_batch=args.enc_batch, max_prompts=args.max_prompts)
@@ -268,16 +280,23 @@ def run_ours(args):
                   box_nms_thresh=args.box_nms_thresh)
     worst_kw = dict(pred_iou_thresh=0.0, stability_score_thresh=0.0, box_nms_thresh=args.box_nms_thresh)
     survivors = []
+    last = {}   # what the last timed step computed (--dump-outputs; the label buffer is reused per tile, so it is copied)
 
-    def step_device(kw=gen_kw, count=False):
+    def step_device(kw=gen_kw, count=False, capture=False):
         feats = sam.encode_u8(tiles_u8)
         out = None
+        labels, ious = [], []
         for t in range(N_TILES):
             emb = {"features": feats[t:t + 1], "input_size": (TILE, TILE), "original_size": (TILE, TILE)}
             amg.initialize(tiles[t], image_embeddings=emb)
             out = amg.generate_device(**kw)
+            if capture:   # `_crop_list`, not `crop_list`: the property would materialise the lazily skipped statistics
+                labels.append(out.clone())
+                ious.append(amg._crop_list[0]["iou_preds"].clone())
             if count:
                 survivors.append(amg._n_keep_dev.clone())
+        if capture:
+            last.update(features=feats, labels=labels, iou_preds=ious)
         return out
 
     def step_e2e():
@@ -318,9 +337,17 @@ def run_ours(args):
     for _ in range(args.warmup):
         step_device()
     l0 = _lib.launch_count()
-    dev_ms, _ = timed(step_device, args.steps, 0)
+    n_timed = [0]
+
+    def timed_step():
+        n_timed[0] += 1
+        return step_device(capture=bool(args.dump_outputs) and n_timed[0] == args.steps)
+
+    dev_ms, _ = timed(timed_step, args.steps, 0)
     launches = (_lib.launch_count() - l0) / args.steps
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
     value = world * N_TILES * args.steps / (dev_ms / 1e3)
     # ---- end to end through the reference-facing API (host in, host out)
     e2e_ms, e2e_wall = timed(step_e2e, args.steps, max(1, args.warmup // 2))
@@ -341,7 +368,7 @@ def run_ours(args):
     rep = _lib.profile_report()
     L.msam_profile(0)
     prof_ms = sum(r["ms"] for r in rep)
-    table = kernel_table(rep, 1, pk, dev_ms / args.steps, traffic)
+    table = kernel_table(rep, 1, pk, dev_ms / args.steps)
 
     stage = {}
 
@@ -394,7 +421,6 @@ def run_ours(args):
             "peak": pk["bf16_tflops_sustained"] if bound == "tensor" else pk["hbm_gbs"],
             "unit": "TFLOP/s" if bound == "tensor" else "GB/s",
             "frac": dom["frac_tensor"] if bound == "tensor" else dom["frac_hbm"],
-            "traffic": dom.get("dram_bytes_per_launch_ncu"),
             "peak_source": f"{pk_src} " + ("bf16_tflops_sustained" if bound == "tensor" else "hbm_gbs"),
             "launches_per_step": dom["launches_per_step"], "share_of_step": dom["share_of_step"],
             "avg_launch_ms": dom["ms_per_step"] / max(dom["launches_per_step"], 1),
@@ -454,6 +480,8 @@ def main():
     ap.add_argument("--box-nms-thresh", type=float, default=BENCH_THRESH["box_nms_thresh"])
     ap.add_argument("--no-vith", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step computed to DIR/<name>.npy (float32, fixed seeded samples)")
     args = ap.parse_args()
     if args.model is None:
         args.model = {"cfg1": "vit_t", "cfg2": "vit_b", "cfg3": "vit_l", "cfg4": "vit_h", "cfg5": "vit_b"}[args.config]
@@ -464,7 +492,7 @@ def main():
         run_reference(args)
     else:
         if not torch.cuda.is_available():
-            raise SystemExit("bench.py: no CUDA device (the B200 path has no CPU fallback; use --impl reference)")
+            raise SystemExit("bench.py: no CUDA device (the GPU path has no CPU fallback; use --impl reference)")
         run_ours(args)
 
 

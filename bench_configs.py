@@ -458,5 +458,5 @@ def main(args):
     if args.impl == "reference":
         return run_reference(args)
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device (the B200 path has no CPU fallback; use --impl reference)")
+        raise SystemExit("bench.py: no CUDA device (the GPU path has no CPU fallback; use --impl reference)")
     return {"cfg1": run_cfg1, "cfg3": run_cfg3, "cfg4": run_cfg4, "cfg5": run_cfg5}[args.config](args)

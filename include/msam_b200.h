@@ -1,4 +1,4 @@
-/* msam_b200.h -- C ABI of libmsam_b200.so: the B200 (sm_100a) SAM inference core behind micro-sam's predictor seam.
+/* msam_b200.h -- C ABI of libmsam_b200.so: the sm_90a (H100) SAM inference core behind micro-sam's predictor seam.
  *
  * The reference (micro-sam) has no FFI; its seam is the Python `SamPredictor`/`Sam` duck type returned by
  * micro_sam/util.py:318 (get_sam_model).  Each entry point below names the reference call it replaces.

@@ -1,5 +1,5 @@
 """ctypes binding of libmsam_b200.so (include/msam_b200.h).  There is NO CPU fallback: if the library is missing or
-no sm_100 device is present, calls raise."""
+no sm_90 device is present, calls raise."""
 from __future__ import annotations
 
 import ctypes

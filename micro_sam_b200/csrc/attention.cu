@@ -1,370 +1,14 @@
-// Windowed ViT-encoder attention for sm_100a (14x14 windows, 196 keys incl. the zero-pad tokens, which stay in the key set
-// with q=k=v=qkv.bias exactly like the reference): softmax(scale * Q K^T + rel_h[q,kh] + rel_w[q,kw]) V, one CTA per
-// (128-query tile, head, window).  Restates segment_anything's Attention.forward + add_decomposed_rel_pos
-// (oracle/sam_ref.py:Attention).  The global (64x64) blocks live in attention_global.cu.
-// Warp roles: warps 0-3 softmax/epilogue (thread r <-> query row r <-> TMEM lane r), warp 4 TMA producer,
-// warp 5 TMEM allocator + MMA issuer.
+// ViT-encoder attention dispatch (restates segment_anything's Attention.forward + add_decomposed_rel_pos,
+// oracle/sam_ref.py:Attention): the windowed blocks (14x14 windows, 196 keys incl. the zero-pad tokens, which stay in the key
+// set with q=k=v=qkv.bias exactly like the reference) run attention_win2.cu, the global (64x64) blocks attention_global.cu.
 #include "kernels.h"
-#include "ptx.cuh"
-#include "tensormap.h"
-#include <stdlib.h>
-#include <type_traits>
 
 namespace msam {
 
-constexpr int ATT_THREADS = 192;
-constexpr int ATT_BOX_BYTES = 128 * 128;  // 128 rows x 64 bf16
-
-struct AttParams {
-  __nv_bfloat16* out;
-  int d_model;   // heads * D
-  int grid;      // 64
-  float scale_log2;
-  unsigned long long* trace;
-};
-
-#define ATT_TRACE(slot) do { if (tr) { unsigned long long t_; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_)); tr[slot] = t_; } } while (0)
-
-__device__ __forceinline__ float ex2f(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
-// x[i] <- x[i + sh] for a per-lane shift sh in [0, 2^NBITS), using static indices only.
-template <int N, int NBITS>
-__device__ __forceinline__ void lane_shift(float (&x)[N], int sh) {
-#pragma unroll
-  for (int b = NBITS - 1; b >= 0; --b) {
-    const int step = 1 << b;
-    const bool on = (sh & step) != 0;
-#pragma unroll
-    for (int i = 0; i + step < N; ++i) x[i] = on ? x[i + step] : x[i];
-  }
-}
-
-// =================================================================================================================
-// Windowed attention (14x14 windows, 196 keys incl. pad tokens): one CTA per (128-query tile, head, window).
-// All 196 keys fit one N=208 MMA tile, so S = Q K^T is computed ONCE and kept in TMEM for both softmax passes
-// (max, then exp), P (128 x 208, bf16) goes to shared memory over the dead Q/K tiles and O = P V accumulates over
-// the dead S columns: 256 TMEM columns and < 113 KB shared memory for head_dim 64 -> two CTAs per SM overlap each
-// other's serial phases.  Warp roles as in attn_kernel.
-constexpr int WIN_NK = 208;                      // keys padded to a multiple of 16
-constexpr int WIN_KBOX = WIN_NK * 128;           // bytes of one 64-column K/V box (208 rows)
-
-template <int D>
-struct WinCfg {
-  static constexpr int NB = (D + 63) / 64;
-  static constexpr int KSTEPS = D / 16;
-  static constexpr int Q_BYTES = NB * ATT_BOX_BYTES;
-  static constexpr int K_BYTES = NB * WIN_KBOX;
-  static constexpr int RT_BOX = 64 * 128;
-  // COMPACT (head_dim 80, two 64-column boxes per operand): 152 KB in the plain layout = one CTA per SM, i.e. the serial
-  // load -> T -> S -> softmax -> P.V chain of a window runs unoverlapped.  Compact layout: P covers only keys [0,192) =
-  // 3 boxes = exactly Q|RT (48 KB); the last 4 real keys (192..195) are added on the CUDA cores in the epilogue; V is
-  // loaded over the dead K tile once S has been computed.  100 KB -> two CTAs per SM.
-  static constexpr bool COMPACT = (D == 80);
-  static constexpr int PV_KSTEPS = COMPACT ? 12 : WIN_NK / 16;
-  static constexpr int P_BYTES = (COMPACT ? 3 : 4) * ATT_BOX_BYTES;   // blocks of 64 keys
-  static constexpr int R0_BYTES = (Q_BYTES + K_BYTES) > P_BYTES ? (Q_BYTES + K_BYTES) : P_BYTES;  // Q|K aliased by P
-  static constexpr int OFF_K = COMPACT ? (Q_BYTES + NB * RT_BOX) : Q_BYTES;
-  static constexpr int OFF_V = COMPACT ? OFF_K : R0_BYTES;
-  static constexpr int OFF_RT = COMPACT ? Q_BYTES : OFF_V + K_BYTES;
-  static constexpr int OFF_BAR = COMPACT ? (OFF_K + K_BYTES) : (OFF_RT + NB * RT_BOX);
-  static constexpr int SMEM_BYTES = OFF_BAR + 128 + 1024;
-  static_assert(!COMPACT || P_BYTES <= Q_BYTES + NB * RT_BOX, "compact layout: P must fit over Q|RT");
-};
-
-template <int D>
-__global__ void __launch_bounds__(ATT_THREADS, 2)
-attn_window_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
-                   const __grid_constant__ CUtensorMap tmRT, const AttParams p) {
-  using C = WinCfg<D>;
-  constexpr int S = 14, G = 196;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;
-  uint8_t* sK = smem + C::OFF_K;
-  uint8_t* sP = smem;  // aliases Q|K (compact: Q|RT) once S has been computed
-  uint8_t* sV = smem + C::OFF_V;
-  uint8_t* sRT = smem + C::OFF_RT;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
-  uint64_t *ld_full = bars, *v_full = bars + 1, *t_full = bars + 2, *t_done = bars + 3, *s_full = bars + 4,
-           *p_full = bars + 5, *o_full = bars + 6;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 7);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int qt = blockIdx.x, head = blockIdx.y, group = blockIdx.z;
-  unsigned long long* tr = nullptr;
-  if (p.trace && threadIdx.x == 0 && qt == 0 && head == 0 && group < 64) tr = p.trace + group * 16;
-  ATT_TRACE(0);
-
-  if (warp == 4 && lane == 0) {
-    prefetch_tmap(&tmQ);
-    prefetch_tmap(&tmKV);
-    prefetch_tmap(&tmRT);
-    mbar_init(ld_full, 1);
-    mbar_init(v_full, 1);
-    mbar_init(t_full, 1);
-    mbar_init(t_done, 128);
-    mbar_init(s_full, 1);
-    mbar_init(p_full, 128);
-    mbar_init(o_full, 1);
-    fence_barrier_init();
-  }
-  if (warp == 5) tmem_alloc(tmem_slot, 256);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  const int row0 = group * G;
-  ATT_TRACE(1);
-
-  if (warp == 4) {
-    if (lane == 0) {
-      const int qcol = head * D, kcol = p.d_model + head * D, vcol = 2 * p.d_model + head * D;
-      mbar_expect_tx(ld_full, C::Q_BYTES + C::K_BYTES + C::NB * C::RT_BOX);
-      for (int b = 0; b < C::NB; ++b) {
-        tma_load_2d(sQ + b * ATT_BOX_BYTES, &tmQ, ld_full, qcol + b * 64, row0 + qt * 128);
-        tma_load_2d(sK + b * WIN_KBOX, &tmKV, ld_full, kcol + b * 64, row0);
-        tma_load_2d(sRT + b * C::RT_BOX, &tmRT, ld_full, b * 64, 0);
-      }
-      if (C::COMPACT) mbar_wait(s_full, 0, 44);  // S = Q K^T has been computed: V goes over the dead K tile
-      mbar_expect_tx(v_full, C::K_BYTES);
-      for (int b = 0; b < C::NB; ++b) tma_load_2d(sV + b * WIN_KBOX, &tmKV, v_full, vcol + b * 64, row0);
-    }
-  } else if (warp == 5) {
-    // MMA issuer: warp-uniform control flow, one elected lane issues (see ptx.cuh:elect_one)
-    constexpr uint32_t idescT = make_idesc_bf16(128, 64);
-    constexpr uint32_t idescS = make_idesc_bf16(128, WIN_NK);
-    constexpr uint32_t idescO = make_idesc_bf16(128, D, 1);
-    const uint32_t aQ = smem_u32(sQ), aK = smem_u32(sK), aV = smem_u32(sV), aP = smem_u32(sP), aRT = smem_u32(sRT);
-    auto kdesc = [](uint32_t base, uint32_t box_bytes, int ks) {
-      return make_desc_sw128(base + (uint32_t)(ks >> 2) * box_bytes + (uint32_t)(ks & 3) * 32u, 0, 1024);
-    };
-    mbar_wait(ld_full, 0, 40);
-    tc_fence_after();
-    if (elect_one()) {
-#pragma unroll
-      for (int ks = 0; ks < C::KSTEPS; ++ks)
-        umma_bf16(tmem, kdesc(aQ, ATT_BOX_BYTES, ks), kdesc(aRT, C::RT_BOX, ks), idescT, ks > 0);
-      umma_commit(t_full);
-    }
-    __syncwarp();
-    mbar_wait(t_done, 0, 41);  // T (columns [0,64)) is in registers: S may overwrite it
-    tc_fence_after();
-    if (elect_one()) {
-#pragma unroll
-      for (int ks = 0; ks < C::KSTEPS; ++ks)
-        umma_bf16(tmem, kdesc(aQ, ATT_BOX_BYTES, ks), kdesc(aK, WIN_KBOX, ks), idescS, ks > 0);
-      umma_commit(s_full);
-    }
-    __syncwarp();
-    mbar_wait(p_full, 0, 42);  // P written (over Q|K) and S fully consumed
-    mbar_wait(v_full, 0, 43);
-    tc_fence_after();
-    if (elect_one()) {
-#pragma unroll
-      for (int ks = 0; ks < C::PV_KSTEPS; ++ks) {
-        const uint64_t da = make_desc_sw128(aP + (uint32_t)(ks >> 2) * ATT_BOX_BYTES + (uint32_t)(ks & 3) * 32u, 0, 1024);
-        const uint64_t db = make_desc_sw128(aV + (uint32_t)ks * 2048u, WIN_KBOX, 1024);
-        umma_bf16(tmem, da, db, idescO, ks > 0);   // O over the dead S columns [0, D)
-      }
-      umma_commit(o_full);
-    }
-    __syncwarp();
-  } else {
-    const int r = threadIdx.x;
-    const uint32_t tlane = tmem + ((uint32_t)(warp * 32) << 16);
-    const int qi = qt * 128 + r;
-    constexpr float LOG2E = 1.4426950408889634f;
-    float yh[S], yw[S];
-    mbar_wait(t_full, 0, 50);
-    tc_fence_after();
-    ATT_TRACE(2);
-    {
-      int qh = qi / S;
-      const int qw = qi % S;
-      if (qh > S - 1) qh = S - 1;
-      float x[32];
-      uint32_t v[32];
-      tmem_ld32(tlane + 0, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 32; ++i) x[i] = __uint_as_float(v[i]);
-      lane_shift<32, 4>(x, qh);
-#pragma unroll
-      for (int kh = 0; kh < S; ++kh) yh[kh] = x[S - 1 - kh] * LOG2E;
-      tmem_ld32(tlane + 32, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 32; ++i) x[i] = __uint_as_float(v[i]);
-      lane_shift<32, 4>(x, qw);
-#pragma unroll
-      for (int kw = 0; kw < S; ++kw) yw[kw] = x[S - 1 - kw] * LOG2E;
-    }
-    tc_fence_before();
-    mbar_arrive(t_done);
-    ATT_TRACE(3);
-
-    const float sl2 = p.scale_log2;
-    mbar_wait(s_full, 0, 51);
-    tc_fence_after();
-    ATT_TRACE(4);
-    // pass A: row max over the 196 valid keys (S stays in TMEM)
-    float m = -INFINITY;
-#pragma unroll
-    for (int c = 0; c < 7; ++c) {
-      uint32_t v[32];
-      if (c < 6) tmem_ld32(tlane + c * 32, v);
-      else { uint32_t w[16]; tmem_ld16(tlane + 192, w);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] = w[i]; }
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        const int key = c * 32 + i;
-        if (key < G) m = fmaxf(m, fmaf(__uint_as_float(v[i]), sl2, yh[key / S] + yw[key % S]));
-      }
-    }
-    ATT_TRACE(5);
-    // pass B: p = exp2(s - m) -> bf16 P tile (K-major SW128 blocks of 64 keys) over the dead Q|K buffers
-    float l = 0.f;
-    float ptail[4] = {0.f, 0.f, 0.f, 0.f};  // compact layout: probabilities of keys 192..195
-#pragma unroll
-    for (int c = 0; c < 7; ++c) {
-      uint32_t v[32];
-      if (c < 6) tmem_ld32(tlane + c * 32, v);
-      else { uint32_t w[16]; tmem_ld16(tlane + 192, w);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] = w[i]; }
-      tmem_ld_wait();
-      uint32_t pk[16];
-#pragma unroll
-      for (int i = 0; i < 32; i += 2) {
-        const int key = c * 32 + i;
-        float p0 = 0.f, p1 = 0.f;
-        if (key < G) p0 = ex2f(fmaf(__uint_as_float(v[i]), sl2, yh[key / S] + yw[key % S]) - m);
-        if (key + 1 < G) p1 = ex2f(fmaf(__uint_as_float(v[i + 1]), sl2, yh[(key + 1) / S] + yw[(key + 1) % S]) - m);
-        l += p0 + p1;
-        pk[i >> 1] = pack_bf16(p0, p1);
-        if (C::COMPACT && c == 6 && i < 4) { ptail[i] = p0; ptail[i + 1] = p1; }
-      }
-      if (C::COMPACT && c == 6) continue;  // keys 192.. are added in the epilogue
-      uint8_t* prow = sP + (c >> 1) * ATT_BOX_BYTES + r * 128;
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        if (c == 6 && q >= 2) break;  // keys 208.. do not exist
-        const int ch = (c & 1) * 4 + q;
-        *reinterpret_cast<uint4*>(prow + ((ch ^ (r & 7)) << 4)) = make_uint4(pk[q * 4], pk[q * 4 + 1], pk[q * 4 + 2], pk[q * 4 + 3]);
-      }
-    }
-    ATT_TRACE(6);
-    tc_fence_before();
-    fence_proxy_async_smem();
-    mbar_arrive(p_full);
-    ATT_TRACE(7);
-
-    mbar_wait(o_full, 0, 52);
-    tc_fence_after();
-    ATT_TRACE(8);
-    const float inv = 1.0f / l;
-    long out_row = -1;
-    {
-      const int wpr = (p.grid + S - 1) / S;
-      const int b = group / (wpr * wpr), wy = (group / wpr) % wpr, wx = group % wpr;
-      const int y = wy * S + qi / S, x = wx * S + qi % S;
-      if (qi < G && y < p.grid && x < p.grid) out_row = (long)b * p.grid * p.grid + y * p.grid + x;
-    }
-    __nv_bfloat16* orow = p.out + (out_row < 0 ? 0 : out_row) * p.d_model + head * D;
-#pragma unroll
-    for (int c = 0; c < D / 16; ++c) {
-      uint32_t v[16];
-      tmem_ld16(tlane + c * 16, v);
-      tmem_ld_wait();
-      if constexpr (C::COMPACT) {  // O += p[192..195] V[192..195]  (V tile: SW128 boxes of 64 dims, 208 rows of 128 B)
-        const uint32_t vb = smem_u32(sV) + (uint32_t)((c * 16) >> 6) * WIN_KBOX;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const int row = 192 + k;
-#pragma unroll
-          for (int hx = 0; hx < 2; ++hx) {
-            const int ch = (((c * 16) & 63) >> 3) + hx;
-            const uint4 w4 = ld_shared_v4(vb + row * 128 + ((ch ^ (row & 7)) << 4));
-            const uint32_t ws[4] = {w4.x, w4.y, w4.z, w4.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              v[hx * 8 + 2 * e] = __float_as_uint(fmaf(ptail[k], __uint_as_float(ws[e] << 16), __uint_as_float(v[hx * 8 + 2 * e])));
-              v[hx * 8 + 2 * e + 1] = __float_as_uint(fmaf(ptail[k], __uint_as_float(ws[e] & 0xffff0000u), __uint_as_float(v[hx * 8 + 2 * e + 1])));
-            }
-          }
-        }
-      }
-      if (out_row >= 0) {
-        uint4 u0, u1;
-        u0.x = pack_bf16(__uint_as_float(v[0]) * inv, __uint_as_float(v[1]) * inv);
-        u0.y = pack_bf16(__uint_as_float(v[2]) * inv, __uint_as_float(v[3]) * inv);
-        u0.z = pack_bf16(__uint_as_float(v[4]) * inv, __uint_as_float(v[5]) * inv);
-        u0.w = pack_bf16(__uint_as_float(v[6]) * inv, __uint_as_float(v[7]) * inv);
-        u1.x = pack_bf16(__uint_as_float(v[8]) * inv, __uint_as_float(v[9]) * inv);
-        u1.y = pack_bf16(__uint_as_float(v[10]) * inv, __uint_as_float(v[11]) * inv);
-        u1.z = pack_bf16(__uint_as_float(v[12]) * inv, __uint_as_float(v[13]) * inv);
-        u1.w = pack_bf16(__uint_as_float(v[14]) * inv, __uint_as_float(v[15]) * inv);
-        *reinterpret_cast<uint4*>(orow + c * 16) = u0;
-        *reinterpret_cast<uint4*>(orow + c * 16 + 8) = u1;
-      }
-      __syncwarp();
-    }
-    ATT_TRACE(9);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 256);
-  }
-}
-
-template <int D>
-static int launch_attn_window(const AttnArgs& a, cudaStream_t stream) {
-  using C = WinCfg<D>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attn_window_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
-    if (e != cudaSuccess) return set_error("attention: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
-    attr_set = true;
-  }
-  const int d_model = a.heads * D, S = 14;
-  const int wpr = (a.grid + S - 1) / S;
-  const int groups = a.batch * wpr * wpr;
-  const long rows = (long)groups * 196;
-  CUtensorMap tmQ, tmKV, tmRT;
-  if (make_tmap_bf16_2d(&tmQ, a.qkv, rows, 3 * d_model, 3 * d_model, 128)) return -1;
-  if (make_tmap_bf16_2d(&tmKV, a.qkv, rows, 3 * d_model, 3 * d_model, WIN_NK)) return -1;
-  if (make_tmap_bf16_2d(&tmRT, a.rel_table, 64, C::NB * 64, C::NB * 64, 64)) return -1;
-  AttParams p;
-  p.out = a.out; p.d_model = d_model; p.grid = a.grid; p.scale_log2 = a.scale * 1.4426950408889634f;
-  p.trace = get_attn_trace();
-  prof_begin(stream, D == 64 ? "attn_window<64>" : "attn_window<80>", (double)groups * a.heads * (4.0 * 196 * 196 * D + 4.0 * 196 * S * D),
-             (double)groups * 196 * a.heads * D * 2 * 4);
-  attn_window_kernel<D><<<dim3(2, a.heads, groups), ATT_THREADS, C::SMEM_BYTES, stream>>>(tmQ, tmKV, tmRT, p);
-  prof_end(stream);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("window attention launch failed: %s", cudaGetErrorString(e));
-  count_launch();
-  return 0;
-}
-
 int launch_attention(const AttnArgs& a, cudaStream_t stream) {
   if (a.grid != 64) return set_error("attention: token grid %d unsupported (kernel is specialised for 64x64)", a.grid);
-  if (a.window == 0) {
-    return launch_attention_global(a, stream);
-  } else if (a.window == 14) {
-    if (a.head_dim == 64 || a.head_dim == 80) {
-      static const bool v1 = getenv("MSAM_WIN_V1") != nullptr;   // first-generation kernel (below), kept for A/B timing
-      if (!v1) return launch_attn_window2(a, stream);
-      return a.head_dim == 64 ? launch_attn_window<64>(a, stream) : launch_attn_window<80>(a, stream);
-    }
-  }
+  if (a.window == 0) return launch_attention_global(a, stream);
+  if (a.window == 14 && (a.head_dim == 64 || a.head_dim == 80)) return launch_attn_window2(a, stream);
   return set_error("attention: unsupported head_dim=%d window=%d", a.head_dim, a.window);
 }
 

@@ -1,22 +1,18 @@
-// Global (64x64 = 4096 token) ViT-encoder attention for sm_100a, one CTA per (128-query tile, head, image):
+// Global (64x64 = 4096 token) ViT-encoder attention for sm_90a, one CTA per (128-query tile, head, image):
 //   softmax(scale * Q K^T + rel_h[q, kh] + rel_w[q, kw]) V      (segment_anything Attention.forward + add_decomposed_rel_pos,
 //                                                                restated in oracle/sam_ref.py:Attention)
-// Second design (the first one -- attn_kernel<D, 64>, two-pass exact softmax on ONE softmax warpgroup -- ran at 220 TFLOP/s:
-// a single warp per scheduler cannot hide the tcgen05.ld / MUFU latencies, and S = Q K^T was computed twice):
-//   * ONE pass over the keys with an online softmax.  Two softmax warpgroups take alternate 128-key tiles; each owns its
-//     S tile, its P tile and its OWN accumulator O_w in TMEM with its own running reference maximum, so the warpgroups never
-//     synchronise with each other until the final merge  O = (f0 O_0 + f1 O_1) / (f0 l_0 + f1 l_1),  f_w = 2^(m_w - m).
-//   * the reference maximum is lazy: probabilities are formed against the current reference m_w (fp32 / bf16 have 8
-//     exponent bits, so values up to 2^64 above it are harmless); when a tile exceeds it by more than 2^8 the warpgroup
-//     rescales its O_w in TMEM before its next tile (after its previous P.V has completed); more than 2^64 -> the tile is
-//     redone at once against the new maximum (S is still in TMEM), so the result is exact for any input.
-//   * rel-pos bias: T_w = Q RelW^T (128 columns) is gathered into registers once (through shared memory); T_h = Q RelH[qh0 .. qh0+80)^T keeps the 65
-//     table rows this query tile can reach (80 TMEM columns), two values are re-read per key tile.
-//   * tcgen05.mma issued by one elected lane in warp-uniform control flow; K tiles double buffered, V tiles 2-4 stages.
-// TMEM: T_h [0,80) | S_0 [80,208) (T_w first) | S_1 [208,336) | O_0 [336,336+D) | O_1 [336+D, 336+2D)      (<= 496 columns)
+//   * two warpgroups, each owning 64 query rows (= one query grid row) over all 32 key tiles of 128 keys: S = Q K^T with
+//     wgmma m64n128k16 (fp32 accumulators in registers), online softmax straight from the accumulator fragments (row
+//     reductions across the quad of lanes that shares a row), P packed to bf16 in registers and fed back as the A operand
+//     of O += P V (wgmma with A from registers, V consumed MN-major);
+//   * rel-pos bias: T_w = Q RelW^T (128 columns) and T_h = Q RelH[qh0 .. qh0+80)^T (80 columns) are computed once, dumped to
+//     shared memory (over the K / V stages, before the first key tile is loaded) and gathered: 32 rel_w values per thread
+//     in registers, two rel_h values per row and key tile re-read from shared memory;
+//   * one TMA warp: Q and the rel-pos tables, then K / V tiles through 2-4 stage rings shared by both warpgroups.
 #include "kernels.h"
 #include "ptx.cuh"
 #include "tensormap.h"
+#include "wgmma.cuh"
 
 namespace msam {
 
@@ -31,18 +27,16 @@ struct GCfg {
   static constexpr int TILE = NB * BOX;
   static constexpr int KST = 2;
   static constexpr int VST = (D == 64) ? 4 : 2;
-  static constexpr int STREAMS = (D == 64) ? 1 : 2;   // MMA / TMA issue streams (see the MMA issuer section)
   static constexpr int RTH_ROWS = 80, RTH_BOX = RTH_ROWS * 128, RTW_BOX = 128 * 128;
+  static constexpr int TH_PITCH = 82, TW_PITCH = 130;  // fp32 scratch rows of T_h / T_w (padded against bank conflicts)
+  static constexpr int T_BYTES = 128 * (TH_PITCH + TW_PITCH) * 4;
   static constexpr int OFF_Q = 0;
-  static constexpr int OFF_K = OFF_Q + TILE;
-  static constexpr int OFF_V = OFF_K + KST * TILE;   // the rel-pos table tiles alias the V stages until T has been computed
-  static constexpr int OFF_P = OFF_V + VST * TILE;   // 2 x [128 x 128] bf16
-  static constexpr int OFF_ML = OFF_P + 4 * BOX;     // (m, l) of warpgroup 1 for the merge
-  static constexpr int OFF_BAR = OFF_ML + 1024;
+  static constexpr int OFF_K = OFF_Q + TILE;          // the T scratch aliases the K / V stages until the first K tile
+  static constexpr int OFF_V = OFF_K + KST * TILE;    // the rel-pos table tiles alias the V stages until T has been computed
+  static constexpr int KV_END = OFF_V + VST * TILE;
+  static constexpr int OFF_BAR = (KV_END > OFF_K + T_BYTES ? KV_END : OFF_K + T_BYTES + 1023) & ~1023;
   static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
-  static constexpr uint32_t TM_TH = 0, TM_S = 80, TM_O = 336;
   static_assert(NB * (RTH_BOX + RTW_BOX) <= VST * TILE, "rel-pos tiles must fit in the V stages");
-  static_assert(KST * TILE >= 128 * D * 4, "merge buffer must fit in the K stages");
 };
 
 struct GParams {
@@ -56,37 +50,23 @@ __device__ __forceinline__ float gex2(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait_g() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 template <int D>
-__global__ void __launch_bounds__(384, 1)
+__global__ void __launch_bounds__(288, 1)
 attn_global_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmRTh,
                    const __grid_constant__ CUtensorMap tmRTw, const GParams p) {
   using C = GCfg<D>;
   constexpr int NKT = 32;
+  constexpr float LOG2E = 1.4426950408889634f;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
   uint64_t* q_full = bars + 0;
-  uint64_t* t_full = bars + 1;
-  uint64_t* t_done = bars + 2;
-  uint64_t* kfull = bars + 3;     // [2]
-  uint64_t* kempty = bars + 5;    // [2]
-  uint64_t* vfull = bars + 7;     // [4]
-  uint64_t* vempty = bars + 11;   // [4]
-  uint64_t* s_full = bars + 15;   // [2]
-  uint64_t* s_empty = bars + 17;  // [2]
-  uint64_t* p_full = bars + 19;   // [2]
-  uint64_t* p_empty = bars + 21;  // [2]
-  uint64_t* o_full = bars + 23;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 24);
+  uint64_t* t_done = bars + 1;
+  uint64_t* kfull = bars + 2;     // [2]
+  uint64_t* kempty = bars + 4;    // [2]
+  uint64_t* vfull = bars + 6;     // [4]
+  uint64_t* vempty = bars + 10;   // [4]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int qt = blockIdx.x, head = blockIdx.y, img = blockIdx.z;
@@ -95,307 +75,185 @@ attn_global_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_const
 
   if (warp == 8 && lane == 0) {
     prefetch_tmap(&tmQKV); prefetch_tmap(&tmRTh); prefetch_tmap(&tmRTw);
-    mbar_init(q_full, 1); mbar_init(t_full, 1); mbar_init(t_done, 4);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&kfull[i], 1); mbar_init(&kempty[i], 1);
-      mbar_init(&s_full[i], 1); mbar_init(&s_empty[i], 4);
-      mbar_init(&p_full[i], 4); mbar_init(&p_empty[i], 1);
-    }
-    for (int i = 0; i < 4; ++i) { mbar_init(&vfull[i], 1); mbar_init(&vempty[i], 1); }
-    mbar_init(o_full, C::STREAMS);  // the last P.V of each stream
+    mbar_init(q_full, 1); mbar_init(t_done, 8);
+    for (int i = 0; i < C::KST; ++i) { mbar_init(&kfull[i], 1); mbar_init(&kempty[i], 8); }
+    for (int i = 0; i < C::VST; ++i) { mbar_init(&vfull[i], 1); mbar_init(&vempty[i], 8); }
     fence_barrier_init();
   }
-  if (warp == 9) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   pdl_wait();
   pdl_trigger();
   uint8_t* sQ = smem + C::OFF_Q;
   uint8_t* sK = smem + C::OFF_K;
   uint8_t* sV = smem + C::OFF_V;
 
-  if (warp == 8 || warp == 11) {
-    // =========================================================== TMA producers: one per key-tile stream (warp 8: even tiles
-    // + Q and the rel-pos tables, warp 11: odd tiles), so that a stalled stream never delays the other one's loads
-    if (lane == 0 && (C::STREAMS == 2 || warp == 8)) {
-      const int sw = warp == 8 ? 0 : 1;
+  if (warp == 8) {
+    // =========================================================== TMA producer
+    if (lane == 0) {
       const int qcol = head * D, kcol = p.d_model + head * D, vcol = 2 * p.d_model + head * D;
-      if (sw == 0) {
-        mbar_expect_tx(q_full, C::TILE + C::NB * (C::RTH_BOX + C::RTW_BOX));
-        for (int b = 0; b < C::NB; ++b) tma_load_2d(sQ + b * BOX, &tmQKV, q_full, qcol + b * 64, row0 + qt * 128);
-        for (int b = 0; b < C::NB; ++b) tma_load_2d(sV + b * C::RTH_BOX, &tmRTh, q_full, b * 64, qh0);
-        for (int b = 0; b < C::NB; ++b) tma_load_2d(sV + C::NB * C::RTH_BOX + b * C::RTW_BOX, &tmRTw, q_full, b * 64, 128);
-      }
-      auto load_k = [&](int j) {
-        const int st = j & 1;
-        mbar_wait(&kempty[st], ((j >> 1) & 1) ^ 1, 40);
-        mbar_expect_tx(&kfull[st], C::TILE);
-        for (int b = 0; b < C::NB; ++b) tma_load_2d(sK + st * C::TILE + b * BOX, &tmQKV, &kfull[st], kcol + b * 64, row0 + j * 128);
-      };
-      auto load_v = [&](int j) {
-        const int st = j % C::VST;
-        mbar_wait(&vempty[st], ((j / C::VST) & 1) ^ 1, 41);
-        mbar_expect_tx(&vfull[st], C::TILE);
-        for (int b = 0; b < C::NB; ++b) tma_load_2d(sV + st * C::TILE + b * BOX, &tmQKV, &vfull[st], vcol + b * 64, row0 + j * 128);
-      };
-      load_k(sw);
-      if (C::STREAMS == 1) load_k(1);
-      mbar_wait(t_full, 0, 42);  // the T MMAs have read the rel-pos tiles -> the V stages are free
-      load_v(sw);
-      if (C::STREAMS == 1) load_v(1);
-      for (int j = sw + 2; j < NKT; j += C::STREAMS) { load_k(j); load_v(j); }
-    }
-  } else if (warp == 9 || warp == 10) {
-    // =========================================================== MMA issuers, warp-uniform control flow with an elected lane.
-    // STREAMS == 2 (d = 80): one in-order stream per softmax warpgroup (warp 9: even key tiles, warp 10: odd) -- a single
-    // issuer blocked on P of tile j cannot issue S of tile j+3 for the other warpgroup (ncu: 40 % of the stall samples on
-    // that wait, profiles/r1_ncu_attn_global_d80.txt; 870 -> 800 us per block).  d = 64 measured faster with one issuer.
-    const int sw = warp - 9;
-    if (C::STREAMS == 1 && sw == 1) goto done;
-    constexpr uint32_t idescTh = make_idesc_bf16(128, C::RTH_ROWS);
-    constexpr uint32_t idescS = make_idesc_bf16(128, 128);
-    constexpr uint32_t idescO = make_idesc_bf16(128, D, 1);  // B (= V) is MN-major
-    const uint32_t aQ = smem_u32(sQ), aK = smem_u32(sK), aV = smem_u32(sV), aP = smem_u32(smem + C::OFF_P);
-    auto kdesc = [](uint32_t base, uint32_t box_bytes, int ks) {  // K-major operand, K step ks: box ks/4, +32 B per step
-      return make_desc_sw128(base + (uint32_t)(ks >> 2) * box_bytes + (uint32_t)(ks & 3) * 32u, 0, 1024);
-    };
-    mbar_wait(q_full, 0, 50);
-    tc_fence_after();
-    if (sw == 0) {
-      if (elect_one()) {
-#pragma unroll
-        for (int ks = 0; ks < C::KSTEPS; ++ks)
-          umma_bf16(tmem + C::TM_TH, kdesc(aQ, BOX, ks), kdesc(aV, C::RTH_BOX, ks), idescTh, ks > 0);
-#pragma unroll
-        for (int ks = 0; ks < C::KSTEPS; ++ks)
-          umma_bf16(tmem + C::TM_S, kdesc(aQ, BOX, ks), kdesc(aV + C::NB * C::RTH_BOX, C::RTW_BOX, ks), idescS, ks > 0);
-        umma_commit(t_full);
-      }
-      __syncwarp();
-      mbar_wait(t_done, 0, 51);  // T_w (aliases S_0) has been gathered into registers
-      tc_fence_after();
-    }
-    auto issue_S = [&](int j) {
-      const int w = j & 1, n = j >> 1;
-      mbar_wait(&kfull[w], n & 1, 52);
-      mbar_wait(&s_empty[w], (n & 1) ^ 1, 53);
-      tc_fence_after();
-      if (elect_one()) {
-#pragma unroll
-        for (int ks = 0; ks < C::KSTEPS; ++ks)
-          umma_bf16(tmem + C::TM_S + w * 128, kdesc(aQ, BOX, ks), kdesc(aK + w * C::TILE, BOX, ks), idescS, ks > 0);
-        umma_commit(&s_full[w]);
-        umma_commit(&kempty[w]);
-      }
-      __syncwarp();
-    };
-    issue_S(sw);
-    if (C::STREAMS == 1) issue_S(1);
-    for (int j = sw; j < NKT; j += C::STREAMS) {
-      if (j + 2 < NKT) issue_S(j + 2);
-      const int w = j & 1, n = j >> 1, vs = j % C::VST;
-      mbar_wait(&p_full[w], n & 1, 54);
-      mbar_wait(&vfull[vs], (j / C::VST) & 1, 55);
-      tc_fence_after();
-      if (elect_one()) {
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks) {
-          const uint64_t da = make_desc_sw128(aP + w * 2 * BOX + (uint32_t)(ks >> 2) * BOX + (uint32_t)(ks & 3) * 32u, 0, 1024);
-          // V tile: rows = keys (K), 128-B rows of 64 head-dim elements (MN); 16 keys = 2048 B; next 64-col block = one box
-          const uint64_t db = make_desc_sw128(aV + vs * C::TILE + (uint32_t)ks * 2048u, BOX, 1024);
-          umma_bf16(tmem + C::TM_O + w * D, da, db, idescO, (n | ks) != 0);
-        }
-        umma_commit(&p_empty[w]);
-        umma_commit(&vempty[vs]);
-        if (j + C::STREAMS >= NKT) umma_commit(o_full);
-      }
-      __syncwarp();
-    }
-  } else {
-    // =========================================================== softmax warpgroups (thread r <-> query row r)
-    const int w = warp >> 2;                 // warpgroup: key tiles j = 2n + w
-    const int quad = warp & 3, r = quad * 32 + lane;
-    const uint32_t tlane = tmem + ((uint32_t)(quad * 32) << 16);
-    const int qi = qt * 128 + r;
-    const int dq = quad >> 1;                // query grid row inside the tile (warp-uniform)
-    constexpr float LOG2E = 1.4426950408889634f;
-    float yw[64];                            // rel_w[q, kw] * log2e
-    // T_w[q][qw - kw + 63] needs a per-lane column offset (qw), which TMEM addressing cannot express: warpgroup 0 dumps its
-    // rows of T_w to shared memory as [column][row] (the P tiles are still unused), then every thread of both warpgroups
-    // gathers its 64 values with conflict-free loads (consecutive lanes: consecutive rows AND consecutive columns).
-    float* tw = reinterpret_cast<float*>(smem + C::OFF_P);  // [128 columns][128 rows] fp32 = 64 KB
-    if (w == 0) {
-      mbar_wait(t_full, 0, 60);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t v[32];
-        tmem_ld32(tlane + C::TM_S + c * 32, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) tw[(c * 32 + i) * 128 + r] = __uint_as_float(v[i]);
-      }
-      tc_fence_before();
-    }
-    named_bar_sync(1, 256);
-    {
-      const int qw = qi & 63;
-#pragma unroll
-      for (int kw = 0; kw < 64; ++kw) yw[kw] = tw[(qw + 63 - kw) * 128 + r] * LOG2E;
-    }
-    named_bar_sync(1, 256);  // everyone has gathered: the P tiles may be written, S_0 may overwrite T_w
-    if (w == 0 && lane == 0) mbar_arrive(t_done);
-
-    const float sl2 = p.scale_log2;
-    const uint32_t prow = smem_u32(smem + C::OFF_P) + w * 2 * BOX + r * 128;
-    const uint32_t tS = tlane + C::TM_S + w * 128, tO = tlane + C::TM_O + w * D;
-    float m_used = 0.f, l = 0.f, pend = 0.f;
-
-    auto rescale_o = [&](float f) {  // O_w row *= f (warp-collective)
-#pragma unroll 1
-      for (int c = 0; c < D / 16; ++c) {
-        uint32_t v[16];
-        tmem_ld16(tO + c * 16, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * f);
-        tmem_st16(tO + c * 16, v);
-      }
-      tmem_st_wait_g();
-    };
-
-#pragma unroll 1
-    for (int n = 0; n < NKT / 2; ++n) {
-      const int j = 2 * n + w;
-      mbar_wait(&s_full[w], n & 1, 61);
-      tc_fence_after();
-      float rh0, rh1;
-      {
-        uint32_t a, b;
-        tmem_ld2(tlane + C::TM_TH + (uint32_t)(dq + 62 - 2 * j), a, b);  // T_h[q][dq + 62 - 2j], [dq + 63 - 2j]
-        tmem_ld_wait();
-        rh1 = __uint_as_float(a) * LOG2E;  // kh = 2j + 1
-        rh0 = __uint_as_float(b) * LOG2E;  // kh = 2j
-      }
-      if (n == 0) {  // exact row maximum of the first tile -> initial reference
-        float mx = -INFINITY;
-#pragma unroll 1
-        for (int cp = 0; cp < 2; ++cp) {
-          const float rh = cp ? rh1 : rh0;
-#pragma unroll
-          for (int ch = 0; ch < 2; ++ch) {
-            uint32_t v[32];
-            tmem_ld32(tS + cp * 64 + ch * 32, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) mx = fmaxf(mx, fmaf(__uint_as_float(v[i]), sl2, yw[ch * 32 + i] + rh));
-          }
-        }
-        m_used = mx;
-      }
-      // the previous P.V of this warpgroup has completed: its P tile may be overwritten and O_w is quiescent
-      mbar_wait(&p_empty[w], (n & 1) ^ 1, 62);
-      tc_fence_after();
-      if (__any_sync(0xffffffffu, pend > 0.f)) {  // deferred rescale requested by the previous tile
-        rescale_o(gex2(-pend));
-        l *= gex2(-pend);
-        m_used += pend;
-        pend = 0.f;
-      }
-      float mx, ls;
-      while (true) {
-        const float c0 = rh0 - m_used, c1 = rh1 - m_used;
-        mx = -INFINITY;
-        float l4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll 1
-        for (int cp = 0; cp < 2; ++cp) {      // 64 keys = one key grid row = one P box
-          const float cc = cp ? c1 : c0;
-#pragma unroll
-          for (int ch = 0; ch < 2; ++ch) {
-            uint32_t v[32];
-            tmem_ld32(tS + cp * 64 + ch * 32, v);
-            tmem_ld_wait();
-            uint32_t pk[16];
-#pragma unroll
-            for (int i = 0; i < 32; i += 2) {
-              const float a0 = fmaf(__uint_as_float(v[i]), sl2, yw[ch * 32 + i] + cc);
-              const float a1 = fmaf(__uint_as_float(v[i + 1]), sl2, yw[ch * 32 + i + 1] + cc);
-              mx = fmaxf(mx, fmaxf(a0, a1));
-              const float p0 = gex2(a0), p1 = gex2(a1);
-              l4[(i >> 1) & 3] += p0 + p1;
-              pk[i >> 1] = pack_bf16(p0, p1);
-            }
-            // P tile, K-major SW128: row r = 128 B, logical 16-B chunk -> physical chunk ^ (r & 7)
-#pragma unroll
-            for (int q = 0; q < 4; ++q)
-              st_shared_v4(prow + cp * BOX + (((ch * 4 + q) ^ (r & 7)) << 4),
-                           make_uint4(pk[q * 4], pk[q * 4 + 1], pk[q * 4 + 2], pk[q * 4 + 3]));
-          }
-        }
-        ls = (l4[0] + l4[1]) + (l4[2] + l4[3]);
-        if (!__any_sync(0xffffffffu, mx > 64.f)) break;
-        // a row of this tile exceeds the reference by more than 2^64: fold it in now and redo the tile (S is still in TMEM)
-        const float d = mx > 8.f ? mx : 0.f, f = gex2(-d);
-        if (n > 0) rescale_o(f);
-        l *= f;
-        m_used += d;
-      }
-      l += ls;
-      if (mx > 8.f) pend = mx;  // more than 2^8 above the reference: rescale before the next tile
-      tc_fence_before();
-      fence_proxy_async_smem();  // generic-proxy P writes -> visible to the UMMA (async proxy) reads
-      __syncwarp();
-      if (lane == 0) { mbar_arrive(&s_empty[w]); mbar_arrive(&p_full[w]); }
-    }
-
-    // ---- merge the two accumulators and write O / l
-    mbar_wait(o_full, 0, 63);
-    tc_fence_after();
-    float* xo = reinterpret_cast<float*>(sK);              // [D][128] fp32 (K stages are dead: every MMA has completed)
-    float2* ml = reinterpret_cast<float2*>(smem + C::OFF_ML);
-    if (w == 1) {
-#pragma unroll 1
-      for (int c = 0; c < D / 16; ++c) {
-        uint32_t v[16];
-        tmem_ld16(tO + c * 16, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 16; ++i) xo[(c * 16 + i) * 128 + r] = __uint_as_float(v[i]);
-      }
-      ml[r] = make_float2(m_used, l);
-    }
-    named_bar_sync(1, 256);
-    if (w == 0) {
-      const float2 o = ml[r];
-      const float m = fmaxf(m_used, o.x);
-      const float f0 = gex2(m_used - m), f1 = gex2(o.x - m);
-      const float inv = 1.0f / (f0 * l + f1 * o.y);
-      const float g0 = f0 * inv, g1 = f1 * inv;
-      __nv_bfloat16* orow = p.out + ((size_t)row0 + qi) * p.d_model + head * D;
-#pragma unroll 1
-      for (int c = 0; c < D / 16; ++c) {
-        uint32_t v[16];
-        tmem_ld16(tO + c * 16, v);
-        tmem_ld_wait();
-        float y[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) y[i] = __uint_as_float(v[i]) * g0 + xo[(c * 16 + i) * 128 + r] * g1;
-        *reinterpret_cast<uint4*>(orow + c * 16) =
-            make_uint4(pack_bf16(y[0], y[1]), pack_bf16(y[2], y[3]), pack_bf16(y[4], y[5]), pack_bf16(y[6], y[7]));
-        *reinterpret_cast<uint4*>(orow + c * 16 + 8) =
-            make_uint4(pack_bf16(y[8], y[9]), pack_bf16(y[10], y[11]), pack_bf16(y[12], y[13]), pack_bf16(y[14], y[15]));
+      mbar_expect_tx(q_full, C::TILE + C::NB * (C::RTH_BOX + C::RTW_BOX));
+      for (int b = 0; b < C::NB; ++b) tma_load_2d(sQ + b * BOX, &tmQKV, q_full, qcol + b * 64, row0 + qt * 128);
+      for (int b = 0; b < C::NB; ++b) tma_load_2d(sV + b * C::RTH_BOX, &tmRTh, q_full, b * 64, qh0);
+      for (int b = 0; b < C::NB; ++b) tma_load_2d(sV + C::NB * C::RTH_BOX + b * C::RTW_BOX, &tmRTw, q_full, b * 64, 128);
+      mbar_wait(t_done, 0, 42);  // T has been computed and gathered: the K / V stages are free
+      for (int j = 0; j < NKT; ++j) {
+        const int ks = j % C::KST, vs = j % C::VST;
+        mbar_wait(&kempty[ks], ((j / C::KST) & 1) ^ 1, 40);
+        mbar_expect_tx(&kfull[ks], C::TILE);
+        for (int b = 0; b < C::NB; ++b) tma_load_2d(sK + ks * C::TILE + b * BOX, &tmQKV, &kfull[ks], kcol + b * 64, row0 + j * 128);
+        mbar_wait(&vempty[vs], ((j / C::VST) & 1) ^ 1, 41);
+        mbar_expect_tx(&vfull[vs], C::TILE);
+        for (int b = 0; b < C::NB; ++b) tma_load_2d(sV + vs * C::TILE + b * BOX, &tmQKV, &vfull[vs], vcol + b * 64, row0 + j * 128);
       }
     }
+    return;
   }
 
-done:
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 512);
+  // =========================================================== warpgroup g: query rows [64 g, 64 g + 64) = grid row qh0 + g.
+  // Fragment element i of a thread: row 64 g + 16 wq + qr + 8 ((i >> 1) & 1), column 8 (i >> 2) + qc + (i & 1).
+  const int g = warp >> 2, wq = warp & 3, qr = lane >> 2, qc = 2 * (lane & 3);
+  const int rbase = 64 * g + 16 * wq + qr;
+  const uint32_t aQ = smem_u32(sQ) + (uint32_t)g * 8192u, aK = smem_u32(sK), aV = smem_u32(sV);
+  auto kdesc = [](uint32_t base, uint32_t box_bytes, int ks) {  // K-major operand, K step ks: box ks/4, +32 B per step
+    return make_desc_sw128(base + (uint32_t)(ks >> 2) * box_bytes + (uint32_t)(ks & 3) * 32u, 0, 1024);
+  };
+  float* th = reinterpret_cast<float*>(sK);                         // [128][TH_PITCH]
+  float* tw = th + 128 * C::TH_PITCH;                               // [128][TW_PITCH]
+
+  mbar_wait(q_full, 0, 50);
+  {
+    float t_h[C::RTH_ROWS / 2], t_w[64];
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < C::KSTEPS; ++ks) wgmma<C::RTH_ROWS>(t_h, kdesc(aQ, BOX, ks), kdesc(aV, C::RTH_BOX, ks), ks > 0);
+#pragma unroll
+    for (int ks = 0; ks < C::KSTEPS; ++ks)
+      wgmma<128>(t_w, kdesc(aQ, BOX, ks), kdesc(aV + C::NB * C::RTH_BOX, C::RTW_BOX, ks), ks > 0);
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc(t_h);
+    wg_fence_acc(t_w);
+    named_bar_sync(1, 256);   // both warpgroups have read the rel-pos tables: the scratch may overwrite them
+#pragma unroll
+    for (int rs = 0; rs < 2; ++rs) {
+      const int r = rbase + 8 * rs;
+#pragma unroll
+      for (int j = 0; j < C::RTH_ROWS / 8; ++j)
+        *reinterpret_cast<float2*>(th + r * C::TH_PITCH + 8 * j + qc) = make_float2(t_h[4 * j + 2 * rs], t_h[4 * j + 2 * rs + 1]);
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+        *reinterpret_cast<float2*>(tw + r * C::TW_PITCH + 8 * j + qc) = make_float2(t_w[4 * j + 2 * rs], t_w[4 * j + 2 * rs + 1]);
+    }
+  }
+  named_bar_sync(1, 256);
+  // rel_w[q, kw] * log2e = T_w[q][qw - kw + 63] for this thread's key columns kw = 8 jj + qc + e (the same in both key grid
+  // rows of a tile); rel_h[q, kh] * log2e = T_h[q][g + 63 - kh], kh = 2 j + (column >> 6)
+  float yw[2][16];
+#pragma unroll
+  for (int rs = 0; rs < 2; ++rs) {
+    const int r = rbase + 8 * rs, qw = (qt * 128 + r) & 63;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) yw[rs][2 * jj + e] = tw[r * C::TW_PITCH + qw + 63 - (8 * jj + qc + e)] * LOG2E;
+  }
+  float rhv[2][64 / 4];   // rel_h of this thread's rows for kh = 4 t + (lane & 3): the lane of the quad that holds it
+#pragma unroll
+  for (int rs = 0; rs < 2; ++rs) {
+    const int r = rbase + 8 * rs;
+#pragma unroll
+    for (int t = 0; t < 16; ++t) rhv[rs][t] = th[r * C::TH_PITCH + g + 63 - (4 * t + (lane & 3))] * LOG2E;
+  }
+  named_bar_sync(1, 256);   // everyone has gathered: K / V may overwrite the scratch
+  __syncwarp();
+  if (lane == 0) mbar_arrive(t_done);
+
+  const float sl2 = p.scale_log2;
+  float o[D / 2];
+#pragma unroll
+  for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+#pragma unroll 1
+  for (int j = 0; j < NKT; ++j) {
+    const int ks_ = j % C::KST, vs = j % C::VST;
+    float sacc[64];
+    mbar_wait(&kfull[ks_], (j / C::KST) & 1, 61);
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < C::KSTEPS; ++ks) wgmma<128>(sacc, kdesc(aQ, BOX, ks), kdesc(aK + ks_ * C::TILE, BOX, ks), ks > 0);
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc(sacc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&kempty[ks_]);
+
+    uint32_t pk[32];
+#pragma unroll
+    for (int rs = 0; rs < 2; ++rs) {
+      // kh = 2 j + h for the two key grid rows of the tile: rel_h from the quad lane that holds kh = 4 t + (lane & 3)
+      float rh[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int kh = 2 * j + h;
+        float v = 0.f;
+#pragma unroll
+        for (int t = 0; t < 16; ++t) v = (t == (kh >> 2)) ? rhv[rs][t] : v;
+        rh[h] = __shfl_sync(0xffffffffu, v, (lane & ~3) | (kh & 3));
+      }
+      float mx = -INFINITY;
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) {
+        const float b = rh[jj >> 3];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float& x = sacc[4 * jj + 2 * rs + e];
+          x = fmaf(x, sl2, yw[rs][2 * (jj & 7) + e] + b);
+          mx = fmaxf(mx, x);
+        }
+      }
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[rs], mx);
+      const float f = gex2(m_run[rs] - m_new);
+      m_run[rs] = m_new;
+      float ls = 0.f;
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) {
+        const float p0 = gex2(sacc[4 * jj + 2 * rs] - m_new), p1 = gex2(sacc[4 * jj + 2 * rs + 1] - m_new);
+        ls += p0 + p1;
+        pk[2 * jj + rs] = pack_bf16(p0, p1);
+      }
+      l_run[rs] = l_run[rs] * f + ls;
+#pragma unroll
+      for (int jd = 0; jd < D / 8; ++jd) { o[4 * jd + 2 * rs] *= f; o[4 * jd + 2 * rs + 1] *= f; }
+    }
+    // O += P V: A fragment of keys [16 ks, 16 ks + 16) = (row, cols 16 ks + qc), (row + 8, ...), (row, + 8), (row + 8, + 8)
+    mbar_wait(&vfull[vs], (j / C::VST) & 1, 62);
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks) {
+      const uint32_t a[4] = {pk[4 * ks], pk[4 * ks + 1], pk[4 * ks + 2], pk[4 * ks + 3]};
+      // V tile: rows = keys (K), 128-B rows of 64 head-dim elements (MN); 16 keys = 2048 B; next 64-col block = one box
+      wgmma_rs<D, 1>(o, a, make_desc_sw128(aV + vs * C::TILE + (uint32_t)ks * 2048u, BOX, 1024), 1);
+    }
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc(o);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&vempty[vs]);
+  }
+
+#pragma unroll
+  for (int rs = 0; rs < 2; ++rs) {
+    float l = l_run[rs];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = 1.0f / l;
+    const int qi = qt * 128 + rbase + 8 * rs;
+    __nv_bfloat16* orow = p.out + ((size_t)row0 + qi) * p.d_model + head * D;
+#pragma unroll
+    for (int jd = 0; jd < D / 8; ++jd)
+      *reinterpret_cast<uint32_t*>(orow + 8 * jd + qc) = pack_bf16(o[4 * jd + 2 * rs] * inv, o[4 * jd + 2 * rs + 1] * inv);
   }
 }
 
@@ -418,7 +276,7 @@ int launch_global_t(const AttnArgs& a, cudaStream_t stream) {
   p.out = a.out; p.d_model = d_model; p.scale_log2 = a.scale * 1.4426950408889634f;
   prof_begin(stream, D == 64 ? "attn_global<64>" : "attn_global<80>", (double)a.batch * a.heads * (4.0 * 4096 * 4096 * D + 4.0 * 4096 * 64 * D),
              (double)a.batch * 4096 * a.heads * D * 2 * 4);
-  launch_pdl(attn_global_kernel<D>, dim3(32, a.heads, a.batch), dim3(384), C::SMEM_BYTES, stream, tmQKV, tmRTh, tmRTw, p);
+  launch_pdl(attn_global_kernel<D>, dim3(32, a.heads, a.batch), dim3(288), C::SMEM_BYTES, stream, tmQKV, tmRTh, tmRTw, p);
   prof_end(stream);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error("global attention launch failed: %s", cudaGetErrorString(e));

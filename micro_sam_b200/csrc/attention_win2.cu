@@ -1,7 +1,7 @@
 // Windowed ViT attention (head_dim 64 / 80, 14x14 windows, 196 keys incl. the zero-pad tokens), second generation.
 // Restates segment_anything's Attention.forward + add_decomposed_rel_pos (oracle/sam_ref.py:Attention) like attention.cu,
-// but moves everything except max / exp off the CUDA cores (profiles/r1_ncu_attn_window_d80.txt: the first kernel spends
-// ~10 instructions per logit and holds 28 bias values per thread; 168 registers, 30 % issue slots, 12.7 us per CTA):
+// with everything except max / exp on the tensor core (a CUDA-core bias costs ~10 instructions per logit and 28 bias values per
+// thread):
 //   * rel-pos bias inside the S MMA: T = Q R^T (as before) is shifted per query row, scaled by 1/scale and written as 28
 //     extra bf16 K-columns next to Q (box 1, columns 16..43) plus their bf16 rounding residuals (a second tile over the dead
 //     R table: hi + lo carries 16 mantissa bits, the bias stays at fp32-accumulator accuracy); the key tile gets the matching
@@ -11,23 +11,25 @@
 //     probabilities (the same values the P V product sees);
 //   * keys 192..195 (P covers 3 boxes = 192 keys) as a 13th k-step whose A tile lives in unused columns of the V tile
 //     (box 1, columns 32..47), instead of 320 CUDA-core FMAs per row in the epilogue;
-//   * row max with 3-input max (0.5 instructions / logit), exp pass = fma + ex2 + half a pack;
-//   * TMEM loads double buffered (the next 32 columns are in flight while the current ones are processed).
+//   * row max, exp pass = fma + ex2 + half a pack, straight from the wgmma accumulator fragments (row
+//     reductions across the quad of lanes that shares a row).
 // Layout: [box A0 16 KB | box A1 16 KB | R 16 KB | box B0 26 KB | box B1 26 KB]; P (keys 0..191, 3 boxes) goes over A0 | A1 | R
 // once S is complete, V is loaded over K (B0 / B1).  head_dim 80: A0 | A1 = Q (80 of 128 columns), the bias columns sit in A1
 // columns 16..47, the one-hot columns in B1 (= K box 1) columns 16..47, the ones column in V box 1 column 16.  head_dim 64:
 // A0 = Q, A1 = the bias tile (columns 0..31), B0 = K / V, B1 = the one-hot tile (columns 0..31; column 0 becomes the ones
 // column once S is complete): the same byte offsets, only the column offset inside box 1 differs.
-// Warp roles: warps 0-3 softmax / epilogue (thread r <-> query row r <-> TMEM lane r), warp 4 TMA, warp 5 TMEM + MMA.
+// Warp roles: warps 0-3 / 4-7 = two warpgroups that each issue the wgmma chains (T, S, O) for 64 of the 128 query rows and
+// run their softmax / epilogue; warp 8 TMA.
 #include "kernels.h"
 #include "ptx.cuh"
 #include "tensormap.h"
+#include "wgmma.cuh"
 
 namespace msam {
 
 namespace {
 
-constexpr int W8_THREADS = 192;
+constexpr int W8_THREADS = 288;
 constexpr int W8_QBOX = 128 * 128;   // 128 rows x 64 bf16
 constexpr int W8_NK = 208;           // keys padded to a multiple of 16
 constexpr int W8_KBOX = W8_NK * 128;
@@ -51,42 +53,27 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
+__device__ __forceinline__ float fmax3(float a, float b, float c) { return fmaxf(a, fmaxf(b, c)); }
 __device__ __forceinline__ unsigned long long gtimer() {
   unsigned long long t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
-// 16 columns into the low half of a 32-register buffer
-__device__ __forceinline__ void tmem_ld16_lo(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+__device__ __forceinline__ void st_shared_u16(uint32_t addr, uint16_t v) {
+  asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"(v) : "memory");
 }
-// x[i] <- x[i + sh] for i < 14, per-lane shift sh in [0, 14), static register indices only (x holds >= 29 valid values)
-__device__ __forceinline__ void lane_shift14(float (&x)[32], int sh) {
-#pragma unroll
-  for (int i = 0; i < 21; ++i) x[i] = (sh & 8) ? x[i + 8] : x[i];
-#pragma unroll
-  for (int i = 0; i < 17; ++i) x[i] = (sh & 4) ? x[i + 4] : x[i];
-#pragma unroll
-  for (int i = 0; i < 15; ++i) x[i] = (sh & 2) ? x[i + 2] : x[i];
-#pragma unroll
-  for (int i = 0; i < 14; ++i) x[i] = (sh & 1) ? x[i + 1] : x[i];
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+// byte address of bf16 element `col` (0..63) of row `r` in a K-major SWIZZLE_128B tile at `base`
+__device__ __forceinline__ uint32_t sw128_addr(uint32_t base, int r, int col) {
+  return base + (uint32_t)r * 128u + ((uint32_t)((col >> 3) ^ (r & 7)) << 4) + (uint32_t)(col & 7) * 2u;
 }
 
 #define W8_TRACE(slot) do { if (tr) tr[slot] = gtimer(); } while (0)
 
 template <int D>
-__global__ void __launch_bounds__(W8_THREADS, 2)
+__global__ void __launch_bounds__(W8_THREADS, 1)
 attn_window2_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                      const __grid_constant__ CUtensorMap tmRT, const W8Params p) {
   constexpr int S = 14, G = 196;
@@ -100,40 +87,30 @@ attn_window2_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   uint8_t* sRT = smem + W8_OFF_RT;
   uint8_t* sK = smem + W8_OFF_K;   // V later
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + W8_OFF_BAR);
-  uint64_t *ld_full = bars, *v_full = bars + 1, *t_full = bars + 2, *t_done = bars + 3, *s_full = bars + 4,
-           *p_full = bars + 5, *o_full = bars + 6, *q_full = bars + 7;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
+  uint64_t *ld_full = bars, *v_full = bars + 1, *s_done = bars + 2, *q_full = bars + 3;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int qt = blockIdx.x, head = blockIdx.y, group = blockIdx.z;
   unsigned long long* tr = nullptr;
   if (p.trace && threadIdx.x == 0 && qt == 0 && head == 0 && group < 64) tr = p.trace + group * 16;
   W8_TRACE(0);
 
-  if (warp == 4 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     prefetch_tmap(&tmQ);
     prefetch_tmap(&tmKV);
     prefetch_tmap(&tmRT);
     mbar_init(ld_full, 1);
     mbar_init(q_full, 1);
     mbar_init(v_full, 1);
-    mbar_init(t_full, 1);
-    mbar_init(t_done, 128);
-    mbar_init(s_full, 1);
-    mbar_init(p_full, 128);
-    mbar_init(o_full, 1);
+    mbar_init(s_done, 8);
     fence_barrier_init();
   }
-  if (warp == 5) tmem_alloc(tmem_slot, 256);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   const int row0 = group * G;
   pdl_wait();
   pdl_trigger();
   W8_TRACE(1);
 
-  if (warp == 4) {
+  if (warp == 8) {
     if (lane == 0) {
       const int qcol = head * D, kcol = p.d_model + head * D, vcol = 2 * p.d_model + head * D;
       mbar_expect_tx(q_full, NB * (W8_QBOX + W8_RTBOX));   // T = Q R^T can start before K has landed
@@ -143,236 +120,179 @@ attn_window2_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       }
       mbar_expect_tx(ld_full, NB * W8_KBOX);
       for (int b = 0; b < NB; ++b) tma_load_2d(sK + b * W8_KBOX, &tmKV, ld_full, kcol + b * 64, row0);
-      mbar_wait(s_full, 0, 44);  // S has been computed: V goes over the dead K tile
+      mbar_wait(s_done, 0, 44);  // both S chains have completed: V goes over the dead K tile
       mbar_expect_tx(v_full, NB * W8_KBOX);
       for (int b = 0; b < NB; ++b) tma_load_2d(sK + b * W8_KBOX, &tmKV, v_full, vcol + b * 64, row0);
     }
-  } else if (warp == 5) {
-    constexpr uint32_t idescT = make_idesc_bf16(128, 64);
-    constexpr uint32_t idescS = make_idesc_bf16(128, W8_NK);
-    constexpr uint32_t idescO = make_idesc_bf16(128, NO, 1);   // D value columns + the ones column (+ 15 unused)
-    const uint32_t aQ = smem_u32(sQ), aK = smem_u32(sK), aRT = smem_u32(sRT);
-    auto kdesc = [](uint32_t base, uint32_t box_bytes, int ks) {
-      return make_desc_sw128(base + (uint32_t)(ks >> 2) * box_bytes + (uint32_t)(ks & 3) * 32u, 0, 1024);
-    };
-    mbar_wait(q_full, 0, 40);
-    tc_fence_after();
-    if (elect_one()) {
+    return;
+  }
+
+  // ---- two warpgroups; warpgroup g owns query rows [64 g, 64 g + 64) of the tile.  Fragment element i of a thread holds
+  // row 64 g + 16 wq + qr + 8 ((i >> 1) & 1), column 8 (i >> 2) + qc + (i & 1).
+  const int g = warp >> 2, wq = warp & 3, qr = lane >> 2, qc = 2 * (lane & 3);
+  const int rbase = 64 * g + 16 * wq + qr;   // + 8 rs
+  const uint32_t aQ = smem_u32(sQ), aK = smem_u32(sK), aRT = smem_u32(sRT);
+  const uint32_t own = (uint32_t)(64 * g) * 128u;   // byte offset of this warpgroup's rows in a 128-row K-major tile
+  auto kdesc = [](uint32_t base, uint32_t box_bytes, int ks) {
+    return make_desc_sw128(base + (uint32_t)(ks >> 2) * box_bytes + (uint32_t)(ks & 3) * 32u, 0, 1024);
+  };
+
+  // T = Q R^T (64 columns: rel_h over [0, 27), rel_w over [32, 59))
+  mbar_wait(q_full, 0, 40);
+  W8_TRACE(2);
+  {
+    float t[32];
+    wg_fence();
 #pragma unroll
-      for (int ks = 0; ks < KS; ++ks) umma_bf16(tmem, kdesc(aQ, W8_QBOX, ks), kdesc(aRT, W8_RTBOX, ks), idescT, ks > 0);
-      umma_commit(t_full);
-    }
-    __syncwarp();
-    mbar_wait(t_done, 0, 41);  // T is in registers, the bias (hi next to Q, lo over R) / one-hot columns are in shared memory
-    mbar_wait(ld_full, 0, 45);
-    tc_fence_after();
-    if (elect_one()) {
+    for (int ks = 0; ks < KS; ++ks) wgmma<64>(t, kdesc(aQ + own, W8_QBOX, ks), kdesc(aRT, W8_RTBOX, ks), ks > 0);
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc(t);
+    named_bar_sync(1, 256);   // both warpgroups have read R: its tile takes the bias residuals now
+    // bias columns of row q: e = kh in [0, 14) <- T[q, 13 + qh - kh], e = 14 + kw <- T[q, 32 + 13 + qw - kw], e in [28, 32) = 0;
+    // hi = bf16(T / scale) next to Q (box 1), lo = bf16(T / scale - hi) in its own tile over the dead R table
 #pragma unroll
-      for (int ks = 0; ks < KS; ++ks) umma_bf16(tmem, kdesc(aQ, W8_QBOX, ks), kdesc(aK, W8_KBOX, ks), idescS, ks > 0);
-#pragma unroll
-      for (int ks = 0; ks < 2; ++ks) {   // bias (hi, then its rounding residuals) against the one-hot columns of box 1
-        const uint64_t de = make_desc_sw128(aK + W8_KBOX + (uint32_t)(AUGC * 16 + ks * 32), 0, 1024);
-        umma_bf16(tmem, make_desc_sw128(aQ + W8_QBOX + (uint32_t)(AUGC * 16 + ks * 32), 0, 1024), de, idescS, 1);
-        umma_bf16(tmem, make_desc_sw128(aRT + (uint32_t)ks * 32u, 0, 1024), de, idescS, 1);
-      }
-      umma_commit(s_full);
-    }
-    __syncwarp();
-    mbar_wait(p_full, 0, 42);  // P written (over Q | R), ones column in V, S fully consumed
-    mbar_wait(v_full, 0, 43);
-    tc_fence_after();
-    if (elect_one()) {
-#pragma unroll
-      for (int ks = 0; ks < 12; ++ks) {
-        const uint64_t da = make_desc_sw128(aQ + (uint32_t)(ks >> 2) * W8_QBOX + (uint32_t)(ks & 3) * 32u, 0, 1024);
-        const uint64_t db = make_desc_sw128(aK + (uint32_t)ks * 2048u, W8_KBOX, 1024);
-        umma_bf16(tmem, da, db, idescO, ks > 0);   // O over the dead S columns [0, NO)
-      }
-      // keys 192..207: A = the tail probabilities parked in V box 1 columns 32..47, B = V rows 192..207
-      umma_bf16(tmem, make_desc_sw128(aK + W8_KBOX + 64u, 0, 1024), make_desc_sw128(aK + 12u * 2048u, W8_KBOX, 1024), idescO, 1);
-      umma_commit(o_full);
-    }
-    __syncwarp();
-  } else {
-    const int r = threadIdx.x;
-    const uint32_t tlane = tmem + ((uint32_t)(warp * 32) << 16);
-    const int qi = qt * 128 + r;
-    const bool live = (qt * 128 + warp * 32) < G;   // warp-uniform: this warp holds at least one real query row
-    const uint32_t aQ = smem_u32(sQ), aK = smem_u32(sK);
-    mbar_wait(t_full, 0, 50);
-    tc_fence_after();
-    W8_TRACE(2);
-    if (live) {
+    for (int rs = 0; rs < 2; ++rs) {
+      const int r = rbase + 8 * rs;
+      const int qi = qt * 128 + r;
       int qh = qi / S;
       const int qw = qi - qh * S;
       if (qh > S - 1) qh = S - 1;
-      uint32_t w[16], wl[16];
-      uint32_t v[32];
-      float x[32];
-      // hi = bf16(y), lo = bf16(y - hi): packs a pair of each
-      auto split = [](float a, float b, uint32_t& hi, uint32_t& lo) {
-        hi = pack_bf16(a, b);
-        lo = pack_bf16(a - __uint_as_float(hi << 16), b - __uint_as_float(hi & 0xffff0000u));
-      };
-      tmem_ld32(tlane + 0, v);
-      tmem_ld_wait();
+      const uint32_t qrow = aQ + W8_QBOX, lrow = aRT;
 #pragma unroll
-      for (int i = 0; i < 32; ++i) x[i] = __uint_as_float(v[i]) * p.inv_scale;
-      tmem_ld32(tlane + 32, v);       // in flight during the shift
-      lane_shift14(x, qh);   // x[i] = T[q, i + qh]
-#pragma unroll
-      for (int j = 0; j < 7; ++j) split(x[S - 1 - 2 * j], x[S - 2 - 2 * j], w[j], wl[j]);   // yh[kh] = x[13 - kh]
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 32; ++i) x[i] = __uint_as_float(v[i]) * p.inv_scale;
-      lane_shift14(x, qw);
-#pragma unroll
-      for (int j = 0; j < 7; ++j) split(x[S - 1 - 2 * j], x[S - 2 - 2 * j], w[7 + j], wl[7 + j]);
-      w[14] = 0u; w[15] = 0u; wl[14] = 0u; wl[15] = 0u;
-      const uint32_t qrow = aQ + W8_QBOX + (uint32_t)r * 128u;          // hi: Q box 1, columns 16..47
-      const uint32_t lrow = smem_u32(sRT) + (uint32_t)r * 128u;         // lo: its own tile over the dead R table, columns 0..31
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        st_shared_v4(qrow + ((uint32_t)((c + AUGC) ^ (r & 7)) << 4), make_uint4(w[4 * c], w[4 * c + 1], w[4 * c + 2], w[4 * c + 3]));
-        st_shared_v4(lrow + ((uint32_t)(c ^ (r & 7)) << 4), make_uint4(wl[4 * c], wl[4 * c + 1], wl[4 * c + 2], wl[4 * c + 3]));
+      for (int i = 0; i < 32; ++i) {
+        if (((i >> 1) & 1) != rs) continue;
+        const int c = 8 * (i >> 2) + qc + (i & 1);
+        const int e = c < 32 ? 13 + qh - c : 14 + 13 + qw - (c - 32);
+        if (c < 32 ? (e < 0 || e > 13) : (e < 14 || e > 27)) continue;
+        const float y = t[i] * p.inv_scale;
+        const __nv_bfloat16 hi = __float2bfloat16_rn(y);
+        const __nv_bfloat16 lo = __float2bfloat16_rn(y - __bfloat162float(hi));
+        st_shared_u16(sw128_addr(qrow, r, AUGC * 8 + e), __bfloat16_as_ushort(hi));
+        st_shared_u16(sw128_addr(lrow, r, e), __bfloat16_as_ushort(lo));
+      }
+      if ((lane & 3) == 0) {   // e = 28..31: the second half of chunk 3 of the bias columns
+        asm volatile("st.shared.v2.b32 [%0], {%1, %1};" ::"r"(sw128_addr(qrow, r, AUGC * 8 + 28)), "r"(0u) : "memory");
+        asm volatile("st.shared.v2.b32 [%0], {%1, %1};" ::"r"(sw128_addr(lrow, r, 28)), "r"(0u) : "memory");
       }
     }
-    // one-hot key columns: rows r and r + 128 of box B1.  head_dim 80: B1 is K box 1 -- wait until the K tile has landed (its
-    // TMA box covers these columns with the next head's data); head_dim 64: B1 is a tile of its own
-    if constexpr (D == 80) mbar_wait(ld_full, 0, 54);
-    for (int k = r; k < W8_NK; k += 128) {
-      unsigned long long bits = 0ull;
-      if (k < G) {
-        const int kh = k / S, kw = k - kh * S;
-        bits = (1ull << kh) | (1ull << (S + kw));
-      }
-      const uint32_t krow = aK + W8_KBOX + (uint32_t)k * 128u;
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t e[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int col = 2 * (4 * c + j);
-          e[j] = (((bits >> col) & 1ull) ? 0x3F80u : 0u) | (((bits >> (col + 1)) & 1ull) ? 0x3F800000u : 0u);
-        }
-        st_shared_v4(krow + ((uint32_t)((c + AUGC) ^ (k & 7)) << 4), make_uint4(e[0], e[1], e[2], e[3]));
-      }
-    }
-    fence_proxy_async_smem();
-    tc_fence_before();
-    mbar_arrive(t_done);
-    W8_TRACE(3);
-
-    mbar_wait(s_full, 0, 51);
-    tc_fence_after();
-    W8_TRACE(4);
-    uint32_t ptail[2] = {0u, 0u};   // probabilities of keys 192..195 (bf16 pairs), A operand of the 13th P V k-step
-    if (live) {
-      uint32_t va[32], vb[32];
-      float m = -INFINITY, nmsl2 = 0.f;
-      const float sl2 = p.sl2;
-      tmem_ld32(tlane, va);
-      // 14 steps: chunks 0..6 for the row max, then chunks 0..6 again for exp; the next chunk is always in flight
-#pragma unroll
-      for (int s = 0; s < 14; ++s) {
-        const int c = s % 7, cn = (s + 1) % 7;
-        uint32_t(&cur)[32] = (s & 1) ? vb : va;
-        uint32_t(&nxt)[32] = (s & 1) ? va : vb;
-        tmem_ld_wait();
-        if (s + 1 < 14) {
-          if (cn < 6) tmem_ld32(tlane + cn * 32, nxt);
-          else tmem_ld16_lo(tlane + 192, nxt);
-        }
-        if (s < 7) {
-          if (c < 6) {
-#pragma unroll
-            for (int i = 0; i < 32; i += 2) m = fmax3(m, __uint_as_float(cur[i]), __uint_as_float(cur[i + 1]));
-          } else {
-            m = fmax3(m, __uint_as_float(cur[0]), __uint_as_float(cur[1]));
-            m = fmax3(m, __uint_as_float(cur[2]), __uint_as_float(cur[3]));
-            nmsl2 = -m * sl2;
-            W8_TRACE(5);
-          }
-        } else if (c < 6) {
-          uint32_t pk[16];
-#pragma unroll
-          for (int i = 0; i < 32; i += 2)
-            pk[i >> 1] = pack_bf16(ex2_approx(fmaf(__uint_as_float(cur[i]), sl2, nmsl2)),
-                                   ex2_approx(fmaf(__uint_as_float(cur[i + 1]), sl2, nmsl2)));
-          const uint32_t prow = aQ + (uint32_t)(c >> 1) * W8_QBOX + (uint32_t)r * 128u;
-#pragma unroll
-          for (int q = 0; q < 4; ++q)
-            st_shared_v4(prow + ((uint32_t)(((c & 1) * 4 + q) ^ (r & 7)) << 4),
-                         make_uint4(pk[q * 4], pk[q * 4 + 1], pk[q * 4 + 2], pk[q * 4 + 3]));
-        } else {
-          ptail[0] = pack_bf16(ex2_approx(fmaf(__uint_as_float(cur[0]), sl2, nmsl2)), ex2_approx(fmaf(__uint_as_float(cur[1]), sl2, nmsl2)));
-          ptail[1] = pack_bf16(ex2_approx(fmaf(__uint_as_float(cur[2]), sl2, nmsl2)), ex2_approx(fmaf(__uint_as_float(cur[3]), sl2, nmsl2)));
-        }
-      }
-    }
-    W8_TRACE(6);
-    // V has landed: ones column (box 1, column 16) for all key rows, and this row's tail probabilities (keys 192..207, zero
-    // beyond 195) into box 1 columns 32..47 = the K-major A tile of the 13th k-step
-    mbar_wait(v_full, 0, 53);
-    for (int k = r; k < W8_NK; k += 128) {
-      const uint32_t a = aK + W8_KBOX + (uint32_t)k * 128u + ((uint32_t)(AUGC ^ (k & 7)) << 4);
-      asm volatile("st.shared.u16 [%0], %1;" ::"r"(a), "h"((unsigned short)0x3F80) : "memory");
-    }
-    {
-      const uint32_t a = aK + W8_KBOX + (uint32_t)r * 128u;
-      st_shared_v4(a + ((uint32_t)(4 ^ (r & 7)) << 4), make_uint4(ptail[0], ptail[1], 0u, 0u));
-      st_shared_v4(a + ((uint32_t)(5 ^ (r & 7)) << 4), make_uint4(0u, 0u, 0u, 0u));
-    }
-    tc_fence_before();
-    fence_proxy_async_smem();
-    mbar_arrive(p_full);
-    W8_TRACE(7);
-
-    mbar_wait(o_full, 0, 52);
-    tc_fence_after();
-    W8_TRACE(8);
-    long out_row = -1;
-    {
-      const int wpr = (p.grid + S - 1) / S;
-      const int b = group / (wpr * wpr), wy = (group / wpr) % wpr, wx = group % wpr;
-      const int y = wy * S + qi / S, x = wx * S + qi % S;
-      if (qi < G && y < p.grid && x < p.grid) out_row = (long)b * p.grid * p.grid + y * p.grid + x;
-    }
-    if (live) {
-      __nv_bfloat16* orow = p.out + (out_row < 0 ? 0 : out_row) * p.d_model + head * D;
-      uint32_t va[32], vb[32];
-      tmem_ld32(tlane + 64, va);   // head_dim 80: 16 value columns + the row sum at column 80; head_dim 64: the row sum at column 64
-      tmem_ld_wait();
-      tmem_ld32(tlane + 0, vb);
-      const float inv = 1.0f / __uint_as_float(va[D - 64]);
-      auto store = [&](const uint32_t(&v)[32], int c0, int n) {
-        if (out_row < 0) return;
-#pragma unroll
-        for (int cc = 0; cc < 32; cc += 8) {
-          if (cc >= n) break;
-          uint4 u;
-          u.x = pack_bf16(__uint_as_float(v[cc + 0]) * inv, __uint_as_float(v[cc + 1]) * inv);
-          u.y = pack_bf16(__uint_as_float(v[cc + 2]) * inv, __uint_as_float(v[cc + 3]) * inv);
-          u.z = pack_bf16(__uint_as_float(v[cc + 4]) * inv, __uint_as_float(v[cc + 5]) * inv);
-          u.w = pack_bf16(__uint_as_float(v[cc + 6]) * inv, __uint_as_float(v[cc + 7]) * inv);
-          *reinterpret_cast<uint4*>(orow + c0 + cc) = u;
-        }
-      };
-      if constexpr (D == 80) store(va, 64, 16);
-      tmem_ld_wait();
-      tmem_ld32(tlane + 32, va);
-      store(vb, 0, 32);
-      tmem_ld_wait();
-      store(va, 32, 32);
-    }
-    W8_TRACE(9);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 256);
+  // one-hot key columns: rows k of box B1.  head_dim 80: B1 is K box 1 -- wait until the K tile has landed (its TMA box
+  // covers these columns with the next head's data); head_dim 64: B1 is a tile of its own
+  mbar_wait(ld_full, 0, 54);
+  for (int k = threadIdx.x; k < W8_NK; k += 256) {
+    unsigned long long bits = 0ull;
+    if (k < G) {
+      const int kh = k / S, kw = k - kh * S;
+      bits = (1ull << kh) | (1ull << (S + kw));
+    }
+    const uint32_t krow = aK + W8_KBOX + (uint32_t)k * 128u;
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      uint32_t e[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int col = 2 * (4 * c + j);
+        e[j] = (((bits >> col) & 1ull) ? 0x3F80u : 0u) | (((bits >> (col + 1)) & 1ull) ? 0x3F800000u : 0u);
+      }
+      st_shared_v4(krow + ((uint32_t)((c + AUGC) ^ (k & 7)) << 4), make_uint4(e[0], e[1], e[2], e[3]));
+    }
   }
+  fence_proxy_async_smem();
+  named_bar_sync(1, 256);
+  W8_TRACE(3);
+
+  // S = Q K^T + (T / scale) E^T : KS k-steps, then bias hi and lo against the one-hot columns
+  float sacc[W8_NK / 2];
+  wg_fence();
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) wgmma<W8_NK>(sacc, kdesc(aQ + own, W8_QBOX, ks), kdesc(aK, W8_KBOX, ks), ks > 0);
+#pragma unroll
+  for (int ks = 0; ks < 2; ++ks) {
+    const uint64_t de = make_desc_sw128(aK + W8_KBOX + (uint32_t)(AUGC * 16 + ks * 32), 0, 1024);
+    wgmma<W8_NK>(sacc, make_desc_sw128(aQ + W8_QBOX + own + (uint32_t)(AUGC * 16 + ks * 32), 0, 1024), de, 1);
+    wgmma<W8_NK>(sacc, make_desc_sw128(aRT + own + (uint32_t)ks * 32u, 0, 1024), de, 1);
+  }
+  wg_commit();
+  wg_wait<0>();
+  wg_fence_acc(sacc);
+  __syncwarp();
+  if (lane == 0) mbar_arrive(s_done);
+  W8_TRACE(4);
+
+  // softmax over keys 0..195: P (keys 0..191) over this warpgroup's rows of A0 | A1 | R, keys 192..207 parked in V box 1
+  // columns 32..47 once V has landed (zero beyond 195)
+  const float sl2 = p.sl2;
+  uint32_t ptail[2][2] = {{0u, 0u}, {0u, 0u}};
+#pragma unroll
+  for (int rs = 0; rs < 2; ++rs) {
+    const int r = rbase + 8 * rs;
+    float m = -INFINITY;
+#pragma unroll
+    for (int j = 0; j < W8_NK / 8; ++j) {
+      const int c = 8 * j + qc;
+      const float a0 = sacc[4 * j + 2 * rs], a1 = sacc[4 * j + 2 * rs + 1];
+      if (c < G) m = fmax3(m, a0, a1);   // G % 2 == 0: the pair is entirely inside or outside
+    }
+    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+    const float nmsl2 = -m * sl2;
+#pragma unroll
+    for (int j = 0; j < W8_NK / 8; ++j) {
+      const int c = 8 * j + qc;
+      const uint32_t pk = pack_bf16(ex2_approx(fmaf(sacc[4 * j + 2 * rs], sl2, nmsl2)), ex2_approx(fmaf(sacc[4 * j + 2 * rs + 1], sl2, nmsl2)));
+      if (c < 192) st_shared_u32(sw128_addr(aQ + (uint32_t)(c >> 6) * W8_QBOX, r, c & 63), pk);
+      else if (c < G) ptail[rs][(c - 192) >> 1] = pk;
+    }
+  }
+  W8_TRACE(5);
+  // V has landed: ones column (box 1, column 8 AUGC) for all key rows, and this warpgroup's tail probabilities
+  mbar_wait(v_full, 0, 53);
+  for (int k = threadIdx.x; k < W8_NK; k += 256) st_shared_u16(sw128_addr(aK + W8_KBOX, k, AUGC * 8), (uint16_t)0x3F80);
+#pragma unroll
+  for (int rs = 0; rs < 2; ++rs) {
+    const int r = rbase + 8 * rs;
+#pragma unroll
+    for (int j = 24; j < 26; ++j) {
+      const int c = 8 * j + qc;
+      st_shared_u32(sw128_addr(aK + W8_KBOX, r, 32 + c - 192), c < G ? ptail[rs][(c - 192) >> 1] : 0u);
+    }
+  }
+  fence_proxy_async_smem();
+  named_bar_sync(1, 256);   // the ones column is written by both warpgroups
+  W8_TRACE(6);
+
+  // O = P V (+ the row sums in column D): 12 k-steps over keys 0..191, a 13th over keys 192..207
+  float oacc[NO / 2];
+  wg_fence();
+#pragma unroll
+  for (int ks = 0; ks < 12; ++ks) {
+    const uint64_t da = make_desc_sw128(aQ + own + (uint32_t)(ks >> 2) * W8_QBOX + (uint32_t)(ks & 3) * 32u, 0, 1024);
+    const uint64_t db = make_desc_sw128(aK + (uint32_t)ks * 2048u, W8_KBOX, 1024);
+    wgmma<NO, 0, 1>(oacc, da, db, ks > 0);
+  }
+  wgmma<NO, 0, 1>(oacc, make_desc_sw128(aK + W8_KBOX + own + 64u, 0, 1024), make_desc_sw128(aK + 12u * 2048u, W8_KBOX, 1024), 1);
+  wg_commit();
+  wg_wait<0>();
+  wg_fence_acc(oacc);
+  W8_TRACE(8);
+
+  const int wpr = (p.grid + S - 1) / S;
+  const int b = group / (wpr * wpr), wy = (group / wpr) % wpr, wx = group % wpr;
+#pragma unroll
+  for (int rs = 0; rs < 2; ++rs) {
+    const int qi = qt * 128 + rbase + 8 * rs;
+    // row sum = column D, held by the lane with qc == 0 of the quad
+    const float sum = __shfl_sync(0xffffffffu, oacc[4 * (D / 8) + 2 * rs], lane & ~3);
+    const int y = wy * S + qi / S, x = wx * S + qi % S;
+    if (qi >= G || y >= p.grid || x >= p.grid) continue;
+    const float inv = 1.0f / sum;
+    __nv_bfloat16* orow = p.out + ((long)b * p.grid * p.grid + y * p.grid + x) * p.d_model + head * D;
+#pragma unroll
+    for (int j = 0; j < D / 8; ++j)
+      *reinterpret_cast<uint32_t*>(orow + 8 * j + qc) = pack_bf16(oacc[4 * j + 2 * rs] * inv, oacc[4 * j + 2 * rs + 1] * inv);
+  }
+  W8_TRACE(9);
 }
 
 unsigned long long* g_attn_trace = nullptr;

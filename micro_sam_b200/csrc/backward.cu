@@ -193,7 +193,7 @@ __global__ void window_gather_kernel(const __nv_bfloat16* __restrict__ x, int B,
 // with T = Q RelTable^T (rows [0, 2 side - 1) = rel_pos_h, rows [woff, woff + 2 side - 1) = rel_pos_w), exactly the forward kernels.
 // P = softmax_k(scale * S + bias)  (bf16 out, the operand of dV = P^T dO)
 // Three passes over the row (max, sum, write): the 0.8 .. 16 KB row stays in L1 / L2 between them.  (A register-resident variant --
-// 128 logits per lane for the 4096-key rows -- was measured: 255 registers, one block per SM, 23 ms instead of 9 ms per step.)
+// 128 logits per lane for the 4096-key rows -- needs 255 registers and runs one block per SM.)
 __global__ void attn_probs_kernel(const float* __restrict__ S, const float* __restrict__ T, long n_rows, AttnBwdGeom g, int pitch_s,
                                   int pitch_p, float scale, __nv_bfloat16* __restrict__ P) {
   const long row = ((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -205,9 +205,8 @@ __global__ void attn_probs_kernel(const float* __restrict__ S, const float* __re
   const float* t = T + row * g.nt;
   __nv_bfloat16* p = P + row * pitch_p;
   const int oh = qh + g.side - 1, ow = g.woff + qw + g.side - 1;
-  // flat key loop, all 32 lanes busy for every geometry.  Measured alternatives (profiles/r3_bench_cfg5*.json.log): a (kh, kw) double loop
-  // without the integer divisions is SLOWER (11.1 vs 9.0 ms per step: idle lanes for the 14-wide windows, twice the loop overhead for
-  // the 64-wide rows); 128 logits per lane in registers is slower still (255 registers, 23 ms).
+  // flat key loop, all 32 lanes busy for every geometry (a (kh, kw) double loop without the integer divisions leaves lanes idle for
+  // the 14-wide windows and doubles the loop overhead for the 64-wide rows).
   float m = -INFINITY;
   for (int k = lane; k < g.n_tok; k += 32) m = fmaxf(m, fmaf(s[k], scale, t[oh - k / g.side] + t[ow - k % g.side]));
   m = warp_max(m);
@@ -337,7 +336,7 @@ int launch_layernorm_bwd(const float* x, int rows, int D, const float* gamma, fl
   if (D % 4 != 0 || D > LNB_V4 * 128) return set_error("layernorm_bwd: unsupported D=%d", D);
   if (rows <= 0) return 0;
   int blocks = (rows + LNB_WARPS - 1) / LNB_WARPS;
-  if (blocks > 592) blocks = 592;   // 4 x 148: bounds the number of global atomics per column
+  if (blocks > 528) blocks = 528;   // 4 x 132 SMs: bounds the number of global atomics per column
   prof_begin(stream, "layernorm_bwd", 0.0, (double)rows * D * 12);
   layernorm_bwd_kernel<<<blocks, LNB_WARPS * 32, 2 * D * sizeof(float), stream>>>(x, rows, D, gamma, eps, dy, window_mode, grid, ws,
                                                                                  accumulate, dx, dgamma, dbeta);

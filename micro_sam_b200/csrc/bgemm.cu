@@ -6,11 +6,13 @@
 // the (feature, row) extents of the map -- which a 2-D map over the packed buffer cannot do (the neighbours are in bounds).
 // Each operand is either K-major (contraction along the contiguous feature dimension: S = Q K^T, dP = dO V^T, T = Q R^T) or
 // MN-major (contraction along the rows: dV = P^T dO, dK = dS^T Q, dQ = dS K), as in gemm_tn.cu.
-// One CTA per 128 x 128 output tile and batch entry; 3-stage TMA ring over 64-wide contraction blocks; fp32 accumulator in TMEM.
+// One CTA per 128 x 128 output tile and batch entry; 3-stage TMA ring over 64-wide contraction blocks; one consumer warpgroup
+// (wgmma m64n128k16 on both 64-row halves, fp32 accumulators in registers).
 // Reference arithmetic: torch autograd of (q @ k^T, softmax, @ v) in oracle/sam_ref.py:Attention; checked in tests/gpu_diag.py.
 #include "kernels.h"
 #include "ptx.cuh"
 #include "tensormap.h"
+#include "wgmma.cuh"
 
 namespace msam {
 
@@ -41,37 +43,25 @@ struct BgParams {
   int accumulate;
 };
 
-// kind::f16, BF16 x BF16 -> FP32; bit 15: A major (1 = MN), bit 16: B major (1 = MN)
-__host__ __device__ constexpr uint32_t bg_idesc(uint32_t M, uint32_t N, uint32_t a_mn, uint32_t b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn << 15) | (b_mn << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-
 template <bool A_MN, bool B_MN>
-__global__ void __launch_bounds__(bg::THREADS, 2)
+__global__ void __launch_bounds__(bg::THREADS, 1)
 bgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const BgParams p) {
   using namespace bg;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* acc_full = empty_bar + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
   const int h = blockIdx.z % p.heads, w = blockIdx.z / p.heads;
   const int k_blocks = (p.K + BK - 1) / BK;
 
-  if (warp == 0 && lane == 0) { prefetch_tmap(&tmA); prefetch_tmap(&tmB); }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    mbar_init(acc_full, 1);
+  if (warp == 0 && lane == 0) {
+    prefetch_tmap(&tmA); prefetch_tmap(&tmB);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 4); }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, BN);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     if (lane == 0) {
@@ -100,62 +90,59 @@ bgemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = bg_idesc(BM, BN, A_MN ? 1u : 0u, B_MN ? 1u : 0u);
-    int stage = 0;
+  } else if (warp >= 4) {
+    const int wq = warp & 3, qr = lane >> 2, qc = 2 * (lane & 3);
+    float acc[2][BN / 2];
+    int stage = 0, prev = -1;
     uint32_t phase = 0;
     for (int kb = 0; kb < k_blocks; ++kb) {
       mbar_wait(&full_bar[stage], phase, 61);
-      tc_fence_after();
       const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES), sb = sa + A_BYTES;
-      if (elect_one()) {
+      wg_fence();
 #pragma unroll
-        for (int kk = 0; kk < BK / 16; ++kk) {
-          // MN-major: 16 contraction rows further = +2048 B, 64-feature blocks SUB apart.  K-major: +32 B inside the 128-B row;
-          // the two 64-row boxes are contiguous (8-row groups 1024 B apart)
-          const uint64_t da = A_MN ? make_desc_sw128(sa + kk * 2048, SUB, 1024) : make_desc_sw128(sa + kk * 32, 0, 1024);
-          const uint64_t db = B_MN ? make_desc_sw128(sb + kk * 2048, SUB, 1024) : make_desc_sw128(sb + kk * 32, 0, 1024);
-          umma_bf16(tmem_base, da, db, idesc, (kb | kk) != 0);
+      for (int kk = 0; kk < BK / 16; ++kk) {
+        // MN-major: 16 contraction rows further = +2048 B, 64-feature blocks SUB apart.  K-major: +32 B inside the 128-B row;
+        // the two 64-row boxes are contiguous (8-row groups 1024 B apart)
+        const uint64_t db = B_MN ? make_desc_sw128(sb + kk * 2048, SUB, 1024) : make_desc_sw128(sb + kk * 32, 0, 1024);
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+          const uint64_t da = A_MN ? make_desc_sw128(sa + hf * SUB + kk * 2048, SUB, 1024) : make_desc_sw128(sa + hf * SUB + kk * 32, 0, 1024);
+          wgmma<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[hf], da, db, (kb | kk) != 0);
         }
-        umma_commit(&empty_bar[stage]);
-        if (kb == k_blocks - 1) umma_commit(acc_full);
       }
-      __syncwarp();
+      wg_commit();
+      wg_wait<1>();
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
+      prev = stage;
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
-  } else if (warp >= 4) {
-    const int quad = warp & 3, r = quad * 32 + lane, row = m0 + r;
+    wg_wait<0>();
+    wg_fence_acc(acc[0]);
+    wg_fence_acc(acc[1]);
     float* obase = p.out + (long)w * p.o_wstride + (long)h * p.o_hstride;
-    mbar_wait(acc_full, 0, 62);
-    tc_fence_after();
-#pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-      if (n0 + 32 * c >= p.N) break;   // uniform
-      uint32_t v[32];
-      tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + 32 * c, v);
-      tmem_ld_wait();
-      if (row < p.M) {
-        float* dst = obase + (size_t)row * p.ldc + n0 + 32 * c;
 #pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          if (n0 + 32 * c + j < p.N) {   // N % 4 == 0
-            float4 o = make_float4(__uint_as_float(v[j]) * p.alpha, __uint_as_float(v[j + 1]) * p.alpha,
-                                   __uint_as_float(v[j + 2]) * p.alpha, __uint_as_float(v[j + 3]) * p.alpha);
-            if (p.accumulate) {
-              const float4 t = *reinterpret_cast<const float4*>(dst + j);
-              o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w;
-            }
-            *reinterpret_cast<float4*>(dst + j) = o;
+    for (int hf = 0; hf < 2; ++hf) {
+#pragma unroll
+      for (int rs = 0; rs < 2; ++rs) {
+        const int row = m0 + 64 * hf + 16 * wq + qr + 8 * rs;
+        if (row >= p.M) continue;
+        float* dst = obase + (size_t)row * p.ldc;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int col = n0 + 8 * j + qc;
+          if (col >= p.N) continue;   // N % 4 == 0
+          float2 o = make_float2(acc[hf][4 * j + 2 * rs] * p.alpha, acc[hf][4 * j + 2 * rs + 1] * p.alpha);
+          if (p.accumulate) {
+            const float2 t = *reinterpret_cast<const float2*>(dst + col);
+            o.x += t.x; o.y += t.y;
           }
+          *reinterpret_cast<float2*>(dst + col) = o;
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, BN);
   }
 }
 

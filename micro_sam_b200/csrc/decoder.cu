@@ -2,7 +2,7 @@
 // restated in oracle/sam_ref.py) batched over P prompts of one image embedding.
 //
 // Layout: image tokens are rows (token-major [4096, 256]); per-prompt image-side tensors are [P*4096, C].  All dense
-// projections run on the tcgen05 GEMM (gemm.cu); this file adds the small fused CUDA-core kernels around them
+// projections run on the wgmma GEMM (gemm.cu); this file adds the small fused CUDA-core kernels around them
 // (prompt PE, 7-token self attention, token->image and image->token attention cores, hyper-network mask product).
 // Exact algebraic hoist: in layer 0 the image-side projections (k/v of token->image, q of image->token) act on
 // `image_embedding + dense (+ pe)`, identical for every prompt when no mask prompt is given -> computed once per
@@ -659,7 +659,7 @@ static int decode_chunk(Engine& E, cudaStream_t st, const float* points, const f
   // token -> image attention core: t_q128 -> t_att128 (t2i_fused.cu)
   auto t2i = [&](const AttnW& A, int mode) -> int {
     // T <= 8: 64 rows per prompt (row pp*64 + h*8 + t).  Shared image tokens (mode 0): two prompts per 128-row item;
-    // own keys (mode 1): one 64-row item per prompt (tcgen05 M = 64).  T > 8: 128 rows per prompt (h*16 + t).
+    // own keys (mode 1): one 64-row item per prompt (one warpgroup).  T > 8: 128 rows per prompt (h*16 + t).
     const int small = T <= 8 ? 1 : 0;
     const int prep_items = small ? (P + 1) / 2 : P;   // 128-row blocks of the Q' operand
     if (launch_t2i_prep(d.t_q128, P, T, small, prep_items, d.qexp, st)) return -1;

@@ -5,8 +5,8 @@
 // upscale_fused fold projections into each other and keep nothing, so they cannot be differentiated through); checked against torch
 // autograd in tests/test_gpu_backward.py.
 //
-// Structure: a tape.  Every forward op (linear, LayerNorm, add+cast, attention, GELU, ...) runs on the existing kernels -- tcgen05
-// GEMMs (gemm.cu / gemm2.cu), the batched attention GEMM (bgemm.cu), LayerNorm -- allocates its output from a per-slot arena
+// Structure: a tape.  Every forward op (linear, LayerNorm, add+cast, attention, GELU, ...) runs on the existing kernels -- wgmma
+// GEMMs (gemm.cu), the batched attention GEMM (bgemm.cu), LayerNorm -- allocates its output from a per-slot arena
 // and pushes its backward closure; backward() replays the closures in reverse.  Tensors carry an fp32 value, an fp32 gradient
 // (accumulated: every consumer ADDS) and a bf16 copy (the GEMM operand).  Parameter gradients accumulate across calls (images,
 // sub-iterations) until msam_decoder_zero_grads.  Supported prompts: points and / or boxes (dense prompt = no_mask_embed).

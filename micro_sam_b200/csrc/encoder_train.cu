@@ -7,8 +7,8 @@
 // GELU(fc1) are recomputed (HBM-bound, cheaper than keeping them).  Per block, in reverse:
 //   MLP    dW2 = dy^T h | dh = dy W2 | dpre = dh o gelu'(pre) | dW1 = dpre^T LN2(x_mid) | dxn = dpre W1 | dx += LN2'(dxn)
 //   attn   dWp = dy^T a | da = dy Wp | (dq, dk, dv, drel) = attention'(qkv, da) | dWqkv = dqkv^T LN1(x_in) | dxn = dqkv Wqkv | dx += LN1'(dxn)
-// dgrad products use the forward tcgen05 GEMMs on weights transposed once per weight update (W^T as the K-major operand: the
-// 2-SM kernel and its epilogues apply), wgrad products the MN-major GEMM of gemm_tn.cu, the five attention products the batched
+// dgrad products use the forward wgmma GEMMs on weights transposed once per weight update (W^T as the K-major operand: the
+// GEMM of gemm.cu and its epilogues apply), wgrad products the MN-major GEMM of gemm_tn.cu, the five attention products the batched
 // GEMM of bgemm.cu (one launch per product for all windows / images and heads), with S / P / dS materialised in HBM per block
 // (window blocks: 0.1 GB, global blocks: 0.07 GB per image and head).  Gradients are fp32, operands bf16.
 #include "engine.h"

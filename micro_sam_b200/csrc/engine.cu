@@ -21,8 +21,8 @@ int set_error(const char* fmt, ...) {
 }
 void count_launch() { ++g_launches; }
 bool pdl_enabled() {
-  // measured on B200 (profiles/r3_pdl_ab.txt): no gain for this chain (every kernel needs its predecessor's output at once, so only
-  // the ~2 us prologues overlap, and the 2-SM GEMMs occupy a whole SM each) -> off unless MSAM_PDL=1
+  // every kernel of the chain needs its predecessor's output at once, so only the short prologues could overlap -> off unless
+  // MSAM_PDL=1
   static const bool on = getenv("MSAM_PDL") != nullptr;
   return on;
 }
@@ -396,7 +396,7 @@ int msam_create(const msam_config* cfg, int device, msam_handle** out) {
   if (device < 0 || device >= ndev) return set_error("msam_create: bad device %d (have %d)", device, ndev);
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, device);
-  if (prop.major != 10) return set_error("msam_create: device %d is sm_%d%d; this library is sm_100a only", device, prop.major, prop.minor);
+  if (prop.major != 9) return set_error("msam_create: device %d is sm_%d%d; this library is sm_90a only", device, prop.major, prop.minor);
   if (cfg->depth == 0) {   // MobileSAM TinyViT (vit_t): fixed architecture, see csrc/tinyvit.cu
     if (cfg->embed_dim != 320 || cfg->num_heads != 10) return set_error("vit_t (depth 0) takes embed_dim 320 / num_heads 10");
   } else {
@@ -713,7 +713,7 @@ int msam_op_layernorm_bwd(const float* x, int rows, int D, const float* gamma, f
   return launch_layernorm_bwd(x, rows, D, gamma, eps, dy, window_mode, 64, 14, accumulate, dx, dgamma, dbeta, (cudaStream_t)stream);
 }
 
-// debug hook (profiles/scripts/win_attn_probe.py): device buffer of 64 x 16 uint64 phase timestamps, or NULL to switch off
+// debug hook: device buffer of 64 x 16 uint64 phase timestamps, or NULL to switch off
 int msam_debug_attn_trace(void* dev_buf) {
   set_attn_trace((unsigned long long*)dev_buf);
   return 0;

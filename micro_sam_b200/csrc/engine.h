@@ -83,7 +83,7 @@ struct DecTrain;      // decoder_train.cu
 
 struct Engine {
   msam_config cfg{};
-  int device = 0, num_sms = 148;
+  int device = 0, num_sms = 132;
   bool finalized = false;
   std::unordered_map<std::string, HostTensor> host_weights;
   std::vector<void*> allocs;

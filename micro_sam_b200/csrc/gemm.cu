@@ -1,47 +1,39 @@
-// Persistent warp-specialised bf16 GEMM for sm_100a:  C[M,N] = epilogue(A[M,K] * W[N,K]^T)
+// Persistent warp-specialised bf16 GEMM for sm_90a:  C[M,N] = epilogue(A[M,K] * W[N,K]^T)
 //   * operands: TMA (SWIZZLE_128B boxes of 64 K-elements) -> shared memory ring (mbarrier full/empty)
-//   * math:     tcgen05.mma cta_group::1 kind::f16, M=128 x N=BN x K=16, fp32 accumulators in TMEM (2 stages)
-//   * epilogue: BN/64 column groups x 4 warps (warp%4 = TMEM lane quadrant); tcgen05.ld 32x32b -> registers ->
-//               bias / GELU(erf) / ReLU / residual (fp32 or bf16, row modulus), or a fused LayerNorm over N=256 ->
-//               128-byte rows in a swizzled shared-memory staging tile -> TMA store (cp.async.bulk.tensor, coalesced,
-//               asynchronous: the row-per-thread global stores of the first version saturated the LSU queue --
-//               ncu: stall lg_throttle 8.9, tensor pipe 51 %, profiles/r1_ncu_gemm_plain_v1.txt).
+//   * math:     one consumer warpgroup per 64-column group of the BN-wide tile; each issues wgmma m64n64k16 for both 64-row
+//               halves of the 128-row tile (fp32 accumulators in registers) and keeps one k-block of MMAs in flight while
+//               it releases the previous ring slot
+//   * epilogue: straight from the accumulator fragments: bias / GELU(erf) / ReLU / residual (fp32 or bf16, row modulus), or a
+//               fused LayerNorm over N=256 (row statistics reduced across the quad, then across the four column groups
+//               through shared memory) -> fp32 / bf16 stores (a quad writes 16 or 32 contiguous bytes of a row).
 // One CTA per SM; tiles are distributed round-robin, N-block fastest so that the CTAs that run concurrently share the
 // same A row-block through L2.
 //
-// Replaces (on the B200 path) the nn.Linear / 1x1-conv / conv-transpose / patch-embed conv calls inside
-// segment_anything's ImageEncoderViT / MaskDecoder that micro_sam reaches through util.py:674 (image_encoder) and
-// SamPredictor.predict_torch (inference.py:248, instance_segmentation.py:361).
+// Replaces the nn.Linear / 1x1-conv / conv-transpose / patch-embed conv calls inside segment_anything's ImageEncoderViT /
+// MaskDecoder that micro_sam reaches through util.py:674 (image_encoder) and SamPredictor.predict_torch (inference.py:248,
+// instance_segmentation.py:361).
 #include "kernels.h"
 #include "ptx.cuh"
 #include "tensormap.h"
+#include "wgmma.cuh"
 
 namespace msam {
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;
-constexpr int STG_BYTES = 128 * 128; // staging tile of one column group: 128 rows x 128 B
 
 enum { EPI_PLAIN = 0, EPI_LN256 = 1 };
 
-// SK = two shallow CTAs per SM (2 pipeline stages, BN = 128) for short-K GEMMs.  Measured SLOWER than one deep CTA on
-// every decoder GEMM (profiles/r1_launches_amg_vit_b_1tile_sk.txt: hyper 3.4 -> 5.3 ms, kvq 1.8 -> 2.1 ms, LN64 1.7 -> 2.4 ms;
-// register cap 85/thread -> spills, A re-read per N block), so no launch path selects it; kept for the record only.
-template <int BN, bool SK = false, int CPW_ = 64>
+template <int BN>
 struct GemmCfg {
-  static constexpr int CPW = CPW_;                      // accumulator columns per epilogue thread
-  static constexpr int NG = BN / CPW;                   // epilogue column groups
-  static constexpr int THREADS = 128 + NG * 128;        // warp0 TMA, warp1 MMA, warp2 TMEM alloc, warp3 idle, epilogue
+  static constexpr int NG = BN / 64;                    // consumer warpgroups = 64-column groups
+  static constexpr int THREADS = 128 + NG * 128;        // warp 0: TMA producer (warps 1-3 idle), then the consumers
   static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;
   static constexpr int B_BYTES = BN * GEMM_BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = SK ? 2 : ((BN == 256) ? 3 : ((BN == 128) ? 5 : 6));
-  static constexpr int MIN_CTAS = SK ? 2 : 1;
-  static_assert(!SK || BN == 128, "short-K variant is instantiated for BN = 128");
-  static constexpr int OFF_STG = STAGES * STAGE_BYTES;  // one staging tile per column group (none for the hyper epilogue)
-  static constexpr int OFF_BAR = OFF_STG + (CPW == 64 ? NG : 0) * STG_BYTES;
-  static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024 /*align slack*/;   // + 11 KB static (exch, rowp)
-  static constexpr int TMEM_COLS = 2 * BN;              // power of two >= 32 for BN in {64,128,256}
+  static constexpr int STAGES = (BN == 256) ? 4 : ((BN == 128) ? 6 : 8);
+  static constexpr int OFF_BAR = STAGES * STAGE_BYTES;
+  static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024 /*align slack*/;   // + 7 KB static (exch, rowp)
 };
 
 struct GemmParams {
@@ -49,7 +41,8 @@ struct GemmParams {
   const float* bias;      // [N] or null
   const void* residual;   // fp32 (or bf16 if res_bf16) [res_rows, ldr] or null; row index = row % res_rows
   int res_rows, ldr, res_bf16;
-  int res_tma;            // fp32 residual fetched by TMA into the staging tile (fp32 output, res_rows % 128 == 0)
+  void* out;
+  int ldc;
   int out_fp32;
   int act;                // 0 none, 1 GELU(erf), 2 ReLU
   int act_after_res;      // apply act after the residual add
@@ -63,8 +56,7 @@ __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + e
 // erf from Abramowitz-Stegun 7.1.25 (three terms, |abs err| <= 2.5e-5 -- measured 2.6e-5 on the GELU over [-10, 10],
 // two orders below the bf16 rounding of the operands it feeds), branch-free with the approximate MUFU ops:
 //   erf(|u|) = 1 - P(t) e^{-u^2}, t = 1 / (1 + p |u|)   =>   GELU(x) = max(x, 0) - |x| * (0.5 P(t)) * e^{-x^2 / 2}
-// 12 instructions (2 MUFU) instead of ~40 for erff() + IEEE reciprocal (ncu: the hyper epilogue is issue bound).  The
-// fp32-output paths keep erff().
+// 12 instructions (2 MUFU) instead of ~40 for erff() + IEEE reciprocal.  The fp32-output paths keep erff().
 __device__ __forceinline__ float gelu_fast(float x) {
   const float z = fabsf(x);
   float t;
@@ -81,35 +73,16 @@ __device__ __forceinline__ float apply_act(float x, int act) {
   if (act == 2) return fmaxf(x, 0.0f);
   return x;
 }
-__device__ __forceinline__ void bf16x8_to_f32(const uint4& r, float* f) {
-  const uint32_t w[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    f[2 * q] = __uint_as_float(w[q] << 16);
-    f[2 * q + 1] = __uint_as_float(w[q] & 0xffff0000u);
-  }
-}
-// 16-byte chunk `ch` (0..7) of row `r` in a 128-B-row staging tile with the TMA SWIZZLE_128B pattern
-__device__ __forceinline__ void stg_write(uint8_t* stg, int r, int ch, const uint4& v) {
-  st_shared_v4(smem_u32(stg) + r * 128 + ((ch ^ (r & 7)) << 4), v);
-}
 
-template <int EPI> struct EpiCols { static constexpr int value = 64; };
-
-template <int BN, int EPI, bool SK>
-__global__ void __launch_bounds__(GemmCfg<BN, SK, EpiCols<EPI>::value>::THREADS, GemmCfg<BN, SK, EpiCols<EPI>::value>::MIN_CTAS)
-gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR, const GemmParams p) {
-  using Cfg = GemmCfg<BN, SK, EpiCols<EPI>::value>;
-  constexpr int NG = Cfg::NG, CPW = Cfg::CPW;
+template <int BN, int EPI>
+__global__ void __launch_bounds__(GemmCfg<BN>::THREADS, 1)
+gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+  using Cfg = GemmCfg<BN>;
+  constexpr int NG = Cfg::NG;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
   uint64_t* empty_bar = full_bar + Cfg::STAGES;
-  uint64_t* tfull_bar = empty_bar + Cfg::STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-  uint64_t* res_bar = tempty_bar + 3;  // [NG] residual tile landed in the staging buffer of the column group
   // statically declared so that the compiler emits LDS/STS (not generic LD/ST through the LG path)
   __shared__ __align__(16) float2 exch[2 * 4 * 128];  // EPI_LN256 statistics exchange, double buffered by tile parity
   __shared__ __align__(16) float rowp[768];           // [0,256) bias, [256,512) gamma, [512,768) beta (fused epilogues)
@@ -124,31 +97,19 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
-    prefetch_tmap(&tmC);
-  }
-  if (warp == 1 && lane == 0) {
     for (int i = 0; i < Cfg::STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], NG * 4);  // one arrive per consumer warp
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], NG * 4);  // one arrive per epilogue warp
-    }
-    for (int i = 0; i < NG; ++i) mbar_init(&res_bar[i], 1);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
   if constexpr (EPI != EPI_PLAIN) {  // N <= 256: per-column parameters -> shared memory (indexed by global column)
     for (int i = threadIdx.x; i < p.N && i < 256; i += Cfg::THREADS) {
       rowp[i] = p.bias ? p.bias[i] : 0.f;
       if constexpr (EPI == EPI_LN256) { rowp[256 + i] = p.ln_gamma[i]; rowp[512 + i] = p.ln_beta[i]; }
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();      // the previous kernel's outputs (A, residual) are complete and visible from here on
   pdl_trigger();
 
@@ -170,329 +131,200 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer (whole warp in uniform control flow, one
-    // elected lane issues)
-    {
-      constexpr uint32_t idesc = make_idesc_bf16(GEMM_BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-        const int as = it & 1;
-        const uint32_t aphase = (it >> 1) & 1;
-        mbar_wait(&tempty_bar[as], aphase ^ 1, 2);  // epilogue drained this accumulator stage
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * BN;
-        for (int kb = 0; kb < k_blocks; ++kb) {
-          mbar_wait(&full_bar[stage], phase, 3);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-          const uint32_t sb = sa + Cfg::A_BYTES;
-          const uint64_t da = make_desc_sw128(sa, 0, 1024);
-          const uint64_t db = make_desc_sw128(sb, 0, 1024);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < GEMM_BK / 16; ++k) {
-              // +32 B per K=16 step inside the 128-B swizzle atom -> +2 on the encoded (>>4) start address
-              umma_bf16(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb | k) != 0);
-            }
-            umma_commit(&empty_bar[stage]);  // smem slot free once these MMAs have read it
-            if (kb == k_blocks - 1) umma_commit(&tfull_bar[as]);
-          }
-          __syncwarp();
-          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
   } else if (warp >= 4) {
-    // ------------------------------------------------------------ epilogue: TMEM -> regs -> staging smem -> TMA store
-    const int quad = warp & 3;           // TMEM lane quadrant this warp may access
+    // ------------------------------------------------------------ consumers: MMA + epilogue of one 64-column group
     const int grp = (warp - 4) >> 2;     // 64-column group of the tile
-    const int r = quad * 32 + lane;      // row inside the tile
-    uint8_t* stg = smem + Cfg::OFF_STG + grp * STG_BYTES;
-    const bool issuer = (quad == 0 && lane == 0);
-    const int bar_id = 2 + grp;          // named barrier of this column group (128 threads)
+    const int wq = warp & 3;             // warp inside the warpgroup: fragment rows 16 wq .. 16 wq + 15 of each half
+    const int qr = lane >> 2, qc = 2 * (lane & 3);
+    int stage = 0;
+    uint32_t phase = 0;
     int it = 0;
-    uint32_t res_cnt = 0;  // residual tiles consumed by this column group (parity of res_bar)
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
       const int m_blk = tile / n_blocks, n_blk = tile % n_blocks;
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      const int row = m_blk * GEMM_BM + r;
-      const bool row_ok = row < p.M;
-      const int colbase = n_blk * BN + grp * CPW;
-      const uint32_t tcol = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(as * BN + grp * CPW);
-      auto release_acc = [&]() {  // this warp's reads of the accumulator stage are complete -> hand it back to the MMA warp
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[as]);
-      };
-      // staging protocol: (a) the previous TMA store has finished reading the tile, (b) every row is written and visible
-      // to the async proxy, then one thread issues the store of the [128 x 128 B] box (rows / columns beyond M / N are clipped)
-      auto stg_acquire = [&]() {
-        if (issuer) tma_store_wait_read();
-        named_bar_sync(bar_id, 128);
-      };
-      auto stg_publish = [&](int col) {
-        fence_proxy_async_smem();
-        named_bar_sync(bar_id, 128);
-        if (issuer) {
-          tma_store_2d(&tmC, stg, col, m_blk * GEMM_BM);
-          tma_store_commit();
+      float acc[2][32];
+      int prev = -1;
+      for (int kb = 0; kb < k_blocks; ++kb) {
+        mbar_wait(&full_bar[stage], phase, 3);
+        const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
+        const uint32_t sb = sa + Cfg::A_BYTES + grp * 64 * 128;
+        wg_fence();
+#pragma unroll
+        for (int k = 0; k < GEMM_BK / 16; ++k) {
+          // +32 B per K=16 step inside the 128-B swizzle atom
+          const uint64_t db = make_desc_sw128(sb + 32 * k, 0, 1024);
+          wgmma<64>(acc[0], make_desc_sw128(sa + 32 * k, 0, 1024), db, (kb | k) != 0);
+          wgmma<64>(acc[1], make_desc_sw128(sa + 8192 + 32 * k, 0, 1024), db, (kb | k) != 0);
         }
-      };
-
-      if constexpr (EPI == EPI_PLAIN) {
-        if (p.res_tma) {
-          // fp32 output + fp32 residual: the residual tile [128 x 32] of each chunk is fetched by TMA straight into the
-          // staging tile (the row-per-thread 16-byte loads of the first version cost one L1 line per lane: 8K cycles per
-          // tile, more than the MMA time of a K = 768 tile -- profiles/r1_gemm_shapes_after_elect.log, "proj +res"),
-          // each thread then adds its accumulators in place and the same tile is stored.
-          const uint32_t stg_a = smem_u32(stg) + r * 128;
-          const int rrow = (m_blk * GEMM_BM) % p.res_rows;
-          const bool on0 = colbase < p.N, on1 = colbase + 32 < p.N;
-          if (issuer && on0) {  // chunk 0: prefetched while the tile is still being accumulated
-            tma_store_wait_read();
-            mbar_expect_tx(&res_bar[grp], STG_BYTES);
-            tma_load_2d(stg, &tmR, &res_bar[grp], colbase, rrow);
-          }
-          mbar_wait(&tfull_bar[as], aphase, 4);
-          tc_fence_after();
-#pragma unroll 1
-          for (int c = 0; c < 2; ++c) {
-            const int col0 = colbase + c * 32;
-            uint32_t v[32];
-            tmem_ld32(tcol + c * 32, v);
-            tmem_ld_wait();
-            if (c == 1) release_acc();
-            if (!(c ? on1 : on0)) continue;  // uniform across the column group
-            float f[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-            if (p.bias) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + j));
-                f[j] += b.x; f[j + 1] += b.y; f[j + 2] += b.z; f[j + 3] += b.w;
-              }
-            }
-            if (p.act) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) f[j] = apply_act(f[j], p.act);
-            }
-            mbar_wait(&res_bar[grp], res_cnt & 1, 5);
-            ++res_cnt;
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const uint32_t a = stg_a + ((q ^ (r & 7)) << 4);
-              const uint4 rr = ld_shared_v4(a);
-              st_shared_v4(a, make_uint4(__float_as_uint(f[4 * q] + __uint_as_float(rr.x)),
-                                         __float_as_uint(f[4 * q + 1] + __uint_as_float(rr.y)),
-                                         __float_as_uint(f[4 * q + 2] + __uint_as_float(rr.z)),
-                                         __float_as_uint(f[4 * q + 3] + __uint_as_float(rr.w))));
-            }
-            stg_publish(col0);
-            if (c == 0 && on1 && issuer) {  // residual of the second chunk, once the store has read the tile
-              tma_store_wait_read();
-              mbar_expect_tx(&res_bar[grp], STG_BYTES);
-              tma_load_2d(stg, &tmR, &res_bar[grp], col0 + 32, rrow);
-            }
-          }
+        wg_commit();
+        wg_wait<1>();   // the MMAs of the previous k-block have read their slot
+        if (prev >= 0) {
           __syncwarp();
-          continue;
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
         }
-        const bool has_res = p.residual != nullptr && row_ok;
-        const float* res_f = nullptr;
-        const __nv_bfloat16* res_b = nullptr;
-        if (has_res) {
-          const size_t off = (size_t)(row % p.res_rows) * p.ldr + colbase;
-          if (p.res_bf16) res_b = reinterpret_cast<const __nv_bfloat16*>(p.residual) + off;
-          else res_f = reinterpret_cast<const float*>(p.residual) + off;
-        }
-        mbar_wait(&tfull_bar[as], aphase, 4);
-        tc_fence_after();
-#pragma unroll 1
-        for (int c = 0; c < 2; ++c) {  // two 32-column chunks
-          const int col0 = colbase + c * 32;
-          const bool on = col0 < p.N;  // N % 32 == 0: a chunk is entirely inside or outside
-          uint32_t v[32];
-          tmem_ld32(tcol + c * 32, v);
-          tmem_ld_wait();
-          if (c == 1) release_acc();
-          float f[32];
+        prev = stage;
+        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+      }
+      wg_wait<0>();
+      wg_fence_acc(acc[0]);
+      wg_fence_acc(acc[1]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+
+      const int colbase = n_blk * BN + grp * 64;
+      if constexpr (EPI == EPI_PLAIN) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-          if (on) {
-            if (p.bias) {
+        for (int h = 0; h < 2; ++h) {
 #pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + j));
-                f[j] += b.x; f[j + 1] += b.y; f[j + 2] += b.z; f[j + 3] += b.w;
+          for (int rs = 0; rs < 2; ++rs) {
+            const int row = m_blk * GEMM_BM + 64 * h + 16 * wq + qr + 8 * rs;
+            if (row >= p.M) continue;
+            const float* res_f = nullptr;
+            const __nv_bfloat16* res_b = nullptr;
+            if (p.residual) {
+              const size_t off = (size_t)(row % p.res_rows) * p.ldr;
+              if (p.res_bf16) res_b = reinterpret_cast<const __nv_bfloat16*>(p.residual) + off;
+              else res_f = reinterpret_cast<const float*>(p.residual) + off;
+            }
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const int col = colbase + 8 * j + qc;
+              if (col >= p.N) continue;   // N % 32 == 0: the pair is entirely inside or outside
+              float x0 = acc[h][4 * j + 2 * rs], x1 = acc[h][4 * j + 2 * rs + 1];
+              if (p.bias) {
+                const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+                x0 += b.x; x1 += b.y;
               }
-            }
-            if (p.act_after_res) {
-              // activation applied below, after the residual
-            } else if (p.act == 1 && !p.out_fp32) {  // bf16 output: the fast erf is exact to well below the output rounding
-#pragma unroll
-              for (int j = 0; j < 32; ++j) f[j] = gelu_fast(f[j]);
-            } else if (p.act) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) f[j] = apply_act(f[j], p.act);
-            }
-            if (res_f) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float4 rr = *reinterpret_cast<const float4*>(res_f + c * 32 + j);
-                f[j] += rr.x; f[j + 1] += rr.y; f[j + 2] += rr.z; f[j + 3] += rr.w;
+              if (p.act_after_res) {
+                // activation applied below, after the residual
+              } else if (p.act == 1 && !p.out_fp32) {  // bf16 output: the fast erf is exact to well below the output rounding
+                x0 = gelu_fast(x0); x1 = gelu_fast(x1);
+              } else if (p.act) {
+                x0 = apply_act(x0, p.act); x1 = apply_act(x1, p.act);
               }
-            } else if (res_b) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 8) {
-                float r8[8];
-                bf16x8_to_f32(*reinterpret_cast<const uint4*>(res_b + c * 32 + j), r8);
-#pragma unroll
-                for (int q = 0; q < 8; ++q) f[j + q] += r8[q];
+              if (res_f) {
+                const float2 r = *reinterpret_cast<const float2*>(res_f + col);
+                x0 += r.x; x1 += r.y;
+              } else if (res_b) {
+                const uint32_t r = *reinterpret_cast<const uint32_t*>(res_b + col);
+                x0 += __uint_as_float(r << 16); x1 += __uint_as_float(r & 0xffff0000u);
               }
+              if (p.act_after_res && p.act) { x0 = apply_act(x0, p.act); x1 = apply_act(x1, p.act); }
+              if (p.out_fp32)
+                *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.out) + (size_t)row * p.ldc + col) = make_float2(x0, x1);
+              else
+                *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + (size_t)row * p.ldc + col) = pack_bf16(x0, x1);
             }
-            if (p.act_after_res && p.act) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) f[j] = apply_act(f[j], p.act);
-            }
-          }
-          if (p.out_fp32) {  // 32 fp32 columns fill the 128-B staging row: one store per chunk
-            if (!on) continue;  // uniform across the column group (depends on col0 only)
-            stg_acquire();
-#pragma unroll
-            for (int q = 0; q < 8; ++q)
-              stg_write(stg, r, q, make_uint4(__float_as_uint(f[4 * q]), __float_as_uint(f[4 * q + 1]),
-                                              __float_as_uint(f[4 * q + 2]), __float_as_uint(f[4 * q + 3])));
-            stg_publish(col0);
-          } else {           // 64 bf16 columns per staging row: one store per tile
-            if (c == 0) stg_acquire();
-#pragma unroll
-            for (int q = 0; q < 4; ++q)
-              stg_write(stg, r, c * 4 + q, make_uint4(pack_bf16(f[8 * q], f[8 * q + 1]), pack_bf16(f[8 * q + 2], f[8 * q + 3]),
-                                                      pack_bf16(f[8 * q + 4], f[8 * q + 5]), pack_bf16(f[8 * q + 6], f[8 * q + 7])));
-            if (c == 1) stg_publish(colbase);
           }
         }
       } else {
-        // ---- fused row epilogues (N == BN): this thread's 64 columns of the row live in registers
-        float f[CPW];
-        // residual (bf16 only in these modes): pulled towards L1 before the accumulator is ready, read after it
-        const bool has_res = (EPI == EPI_LN256) && p.residual != nullptr && row_ok;
-        const __nv_bfloat16* rp = nullptr;
-        if (has_res) {
-          rp = reinterpret_cast<const __nv_bfloat16*>(p.residual) + (size_t)(row % p.res_rows) * p.ldr + colbase;
-          prefetch_l1(rp);
+        // ---- fused LayerNorm over the full 256-wide row (N == BN == 256): exact two-pass statistics per 64-column group
+        // (quad shuffles), combined across the four groups with Chan's formula through shared memory.
+        float2* ex = exch + (it & 1) * (NG * 128);
+        float mean_r[4], rstd_r[4];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int rs = 0; rs < 2; ++rs) {
+            const int rt = 64 * h + 16 * wq + qr + 8 * rs;
+            const int row = m_blk * GEMM_BM + rt;
+            const bool has_res = p.residual != nullptr && row < p.M;
+            const __nv_bfloat16* rp =
+                has_res ? reinterpret_cast<const __nv_bfloat16*>(p.residual) + (size_t)(row % p.res_rows) * p.ldr : nullptr;
+            float s = 0.f;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const int col = colbase + 8 * j + qc;
+              float& x0 = acc[h][4 * j + 2 * rs];
+              float& x1 = acc[h][4 * j + 2 * rs + 1];
+              x0 += rowp[col]; x1 += rowp[col + 1];
+              if (has_res) {
+                const uint32_t r = *reinterpret_cast<const uint32_t*>(rp + col);
+                x0 += __uint_as_float(r << 16); x1 += __uint_as_float(r & 0xffff0000u);
+              }
+              s += x0 + x1;
+            }
+            s += __shfl_xor_sync(0xffffffffu, s, 1);
+            s += __shfl_xor_sync(0xffffffffu, s, 2);
+            const float mean_g = s * (1.0f / 64);
+            float q = 0.f;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const float d0 = acc[h][4 * j + 2 * rs] - mean_g, d1 = acc[h][4 * j + 2 * rs + 1] - mean_g;
+              q = fmaf(d0, d0, fmaf(d1, d1, q));
+            }
+            q += __shfl_xor_sync(0xffffffffu, q, 1);
+            q += __shfl_xor_sync(0xffffffffu, q, 2);
+            if ((lane & 3) == 0) ex[grp * 128 + rt] = make_float2(mean_g, q);
+          }
         }
-        mbar_wait(&tfull_bar[as], aphase, 4);
-        tc_fence_after();
+        named_bar_sync(1, NG * 128);
 #pragma unroll
-        for (int c = 0; c < CPW / 32; ++c) {
-          uint32_t v[32];
-          tmem_ld32(tcol + c * 32, v);
-          tmem_ld_wait();
+        for (int h = 0; h < 2; ++h) {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) f[c * 32 + j] = __uint_as_float(v[j]) + rowp[colbase + c * 32 + j];
+          for (int rs = 0; rs < 2; ++rs) {
+            const int rt = 64 * h + 16 * wq + qr + 8 * rs;
+            float mean = 0.f;
+            float2 st[NG];
+#pragma unroll
+            for (int g = 0; g < NG; ++g) { st[g] = ex[g * 128 + rt]; mean += st[g].x; }
+            mean *= (1.0f / NG);
+            float m2 = 0.f;
+#pragma unroll
+            for (int g = 0; g < NG; ++g) { const float d = st[g].x - mean; m2 += st[g].y + d * d * 64; }
+            mean_r[2 * h + rs] = mean;
+            rstd_r[2 * h + rs] = rsqrtf(m2 * (1.0f / (NG * 64)) + p.ln_eps);
+          }
         }
-        release_acc();
-
-        if constexpr (EPI == EPI_LN256) {
-          if (has_res) {
 #pragma unroll
-            for (int j = 0; j < CPW / 8; ++j) {
-              float r8[8];
-              bf16x8_to_f32(*reinterpret_cast<const uint4*>(rp + 8 * j), r8);
+        for (int h = 0; h < 2; ++h) {
 #pragma unroll
-              for (int q = 0; q < 8; ++q) f[8 * j + q] += r8[q];
+          for (int rs = 0; rs < 2; ++rs) {
+            const int row = m_blk * GEMM_BM + 64 * h + 16 * wq + qr + 8 * rs;
+            if (row >= p.M) continue;
+            const float mean = mean_r[2 * h + rs], rstd = rstd_r[2 * h + rs];
+            __nv_bfloat16* orow = reinterpret_cast<__nv_bfloat16*>(p.out) + (size_t)row * p.ldc;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const int col = colbase + 8 * j + qc;
+              const float y0 = (acc[h][4 * j + 2 * rs] - mean) * rstd * rowp[256 + col] + rowp[512 + col];
+              const float y1 = (acc[h][4 * j + 2 * rs + 1] - mean) * rstd * rowp[256 + col + 1] + rowp[512 + col + 1];
+              *reinterpret_cast<uint32_t*>(orow + col) = pack_bf16(y0, y1);
             }
           }
-          // LayerNorm over the full 256-wide row: exact two-pass statistics per 64-column group, combined across the four
-          // groups with Chan's formula through shared memory.
-          float s4[4] = {0.f, 0.f, 0.f, 0.f};  // 4 independent chains
-#pragma unroll
-          for (int j = 0; j < CPW; ++j) s4[j & 3] += f[j];
-          const float mean_g = ((s4[0] + s4[1]) + (s4[2] + s4[3])) * (1.0f / CPW);
-          float q4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-          for (int j = 0; j < CPW; ++j) { const float d = f[j] - mean_g; q4[j & 3] = fmaf(d, d, q4[j & 3]); }
-          const float m2_g = (q4[0] + q4[1]) + (q4[2] + q4[3]);
-          float2* ex = exch + (it & 1) * (NG * 128);
-          ex[grp * 128 + r] = make_float2(mean_g, m2_g);
-          named_bar_sync(1, NG * 128);
-          float mean = 0.f;
-          float2 st[NG];
-#pragma unroll
-          for (int g = 0; g < NG; ++g) { st[g] = ex[g * 128 + r]; mean += st[g].x; }
-          mean *= (1.0f / NG);
-          float m2 = 0.f;
-#pragma unroll
-          for (int g = 0; g < NG; ++g) { const float d = st[g].x - mean; m2 += st[g].y + d * d * CPW; }
-          const float rstd = rsqrtf(m2 * (1.0f / (NG * CPW)) + p.ln_eps);
-          stg_acquire();
-#pragma unroll
-          for (int j = 0; j < CPW; j += 8) {
-            float y[8];
-#pragma unroll
-            for (int q = 0; q < 8; ++q)
-              y[q] = (f[j + q] - mean) * rstd * rowp[256 + colbase + j + q] + rowp[512 + colbase + j + q];
-            stg_write(stg, r, j >> 3, make_uint4(pack_bf16(y[0], y[1]), pack_bf16(y[2], y[3]), pack_bf16(y[4], y[5]),
-                                                  pack_bf16(y[6], y[7])));
-          }
-          stg_publish(colbase);
         }
       }
-      __syncwarp();
     }
-    if (issuer) tma_store_wait_all();  // all bulk stores of this thread have completed before the CTA exits
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
   }
 }
 
-template <int BN, int EPI, bool SK = false>
+template <int BN, int EPI>
 static int launch_gemm_bn(const GemmArgs& a, int num_sms, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN, SK, EpiCols<EPI>::value>;
+  using Cfg = GemmCfg<BN>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e =
-        cudaFuncSetAttribute(gemm_bf16_kernel<BN, EPI, SK>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+        cudaFuncSetAttribute(gemm_bf16_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
     if (e != cudaSuccess) return set_error("gemm: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
     attr_set = true;
   }
-  const int ldc = a.ldc > 0 ? a.ldc : a.N;
-  CUtensorMap tmA, tmB, tmC, tmR;
+  CUtensorMap tmA, tmB;
   if (make_tmap_bf16_2d(&tmA, a.A, a.M, a.K, a.lda, GEMM_BM)) return -1;
   if (make_tmap_bf16_2d(&tmB, a.W, a.N, a.K, a.ldw, BN)) return -1;
-  if (make_tmap_2d(&tmC, a.out, a.out_fp32 ? 4 : 2, a.M, a.N, ldc, GEMM_BM)) return -1;
   GemmParams p;
-  const int res_rows = a.res_rows > 0 ? a.res_rows : a.M, ldr = a.ldr > 0 ? a.ldr : a.N;
-  p.res_tma = (EPI == EPI_PLAIN && a.residual && !a.res_bf16 && a.out_fp32 && res_rows % GEMM_BM == 0 && ldr % 4 == 0 && !a.act_after_res) ? 1 : 0;
-  if (p.res_tma) {
-    if (make_tmap_2d(&tmR, a.residual, 4, res_rows, a.N, ldr, GEMM_BM)) return -1;
-  } else {
-    tmR = tmA;  // unused
-  }
   p.M = a.M; p.N = a.N; p.K = a.K;
   p.bias = a.bias;
   p.residual = a.residual;
   p.res_bf16 = a.res_bf16;
   p.res_rows = a.res_rows > 0 ? a.res_rows : a.M;
   p.ldr = a.ldr > 0 ? a.ldr : a.N;
+  p.out = a.out;
+  p.ldc = a.ldc > 0 ? a.ldc : a.N;
   p.out_fp32 = a.out_fp32;
   p.act = a.act;
   p.act_after_res = a.act_after_res;
   p.ln_gamma = a.ln_gamma; p.ln_beta = a.ln_beta; p.ln_eps = a.ln_eps;
   const int tiles = ((a.M + GEMM_BM - 1) / GEMM_BM) * ((a.N + BN - 1) / BN);
-  const int max_ctas = num_sms * Cfg::MIN_CTAS;
-  const int grid = tiles < max_ctas ? tiles : max_ctas;
+  const int grid = tiles < num_sms ? tiles : num_sms;
   {
     const double out_b = (double)a.M * a.N * (a.out_fp32 ? 4 : 2);
     const double res_b = a.residual ? (double)(a.res_rows > 0 ? a.res_rows : a.M) * a.N * (a.res_bf16 ? 2 : 4) : 0.0;
@@ -500,7 +332,7 @@ static int launch_gemm_bn(const GemmArgs& a, int num_sms, cudaStream_t stream) {
                      : (a.K >= 512 ? "gemm_bf16 plain K>=512" : "gemm_bf16 plain K<512");
     prof_begin(stream, nm, 2.0 * a.M * a.N * a.K, (double)a.M * a.K * 2 + (double)a.N * a.K * 2 + out_b + res_b);
   }
-  launch_pdl(gemm_bf16_kernel<BN, EPI, SK>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, stream, tmA, tmB, tmC, tmR, p);
+  launch_pdl(gemm_bf16_kernel<BN, EPI>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, stream, tmA, tmB, p);
   prof_end(stream);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error("gemm launch failed: %s", cudaGetErrorString(e));
@@ -520,12 +352,9 @@ int launch_gemm(const GemmArgs& a, int num_sms, cudaStream_t stream) {
     return launch_gemm_bn<256, EPI_LN256>(a, num_sms, stream);
   }
   if (a.epi != EPI_PLAIN) return set_error("gemm: unknown epilogue %d", a.epi);
-  {  // large plain products (the encoder GEMMs): CTA-pair kernel
-    const int r2 = launch_gemm_2sm(a, num_sms, stream);
-    if (r2 != 0) return r2 < 0 ? -1 : 0;
-  }
-  // BN=256 keeps the tensor pipe at its 1-CTA rate with the fewest smem bytes per flop; fall back to 128 / 64 when N is
-  // not a multiple (or is small), to avoid wasted columns.
+  if ((a.ldc > 0 ? a.ldc : a.N) % 2 != 0) return set_error("gemm: ldc must be even");
+  // BN=256 reads the A tile once per 256 output columns; fall back to 128 / 64 when N is not a multiple (or is small), to
+  // avoid wasted columns.
   if (a.N % 256 == 0) return launch_gemm_bn<256, EPI_PLAIN>(a, num_sms, stream);
   if (a.N % 128 == 0) return launch_gemm_bn<128, EPI_PLAIN>(a, num_sms, stream);
   return launch_gemm_bn<64, EPI_PLAIN>(a, num_sms, stream);

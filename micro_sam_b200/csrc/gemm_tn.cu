@@ -3,15 +3,17 @@
 //   dgrad (A_MN = false):  dX[M, N] (fp32) = A B,    A = dY [M, K] bf16 (tokens x out-features, K-major as in the forward GEMM),
 //                                                    B = W [K, N] (out-features x in-features: the forward weight as stored)
 // In both the B operand -- and in wgrad also A -- is contracted over its SLOW dimension:
-// such operands are fed to tcgen05.mma as MN-major tiles: TMA loads
-// [64 tokens x 64 features] boxes (SWIZZLE_128B, 128-byte rows along the feature = M/N dimension) and the UMMA descriptors
-// carry a_major = b_major = MN (leading-dimension byte offset = distance between 64-feature blocks, stride = 8 token rows).
-// One CTA per 128 x 128 output tile, 4-stage TMA ring over 64-token K blocks, fp32 accumulator in TMEM, row-per-thread
-// epilogue (dW is weight-sized: the epilogue is negligible next to the token-long mainloop).
+// such operands are fed to wgmma as MN-major (transposed) tiles: TMA loads
+// [64 tokens x 64 features] boxes (SWIZZLE_128B, 128-byte rows along the feature = M/N dimension) and the matrix descriptors
+// carry leading-dimension byte offset = distance between 64-feature blocks, stride = 8 token rows.
+// One CTA per 128 x 128 output tile, 4-stage TMA ring over 64-token K blocks, one consumer warpgroup (wgmma m64n128k16 on both
+// 64-row halves, fp32 accumulators in registers) that stores straight from the accumulator fragments (dW is weight-sized: the
+// epilogue is negligible next to the token-long mainloop).
 // Reference arithmetic: torch autograd of nn.Linear (dW = dY^T X), checked in tests/gpu_diag.py.
 #include "kernels.h"
 #include "ptx.cuh"
 #include "tensormap.h"
+#include "wgmma.cuh"
 
 namespace msam {
 
@@ -25,11 +27,6 @@ constexpr int SMEM_BYTES = OFF_BAR + 128 + 1024;
 constexpr int THREADS = 256;
 }  // namespace wg
 
-// kind::f16, BF16 x BF16 -> FP32; bit 15: A major (1 = MN), bit 16: B major (1 = MN)
-__host__ __device__ constexpr uint32_t make_idesc_bf16_mn(uint32_t M, uint32_t N, uint32_t a_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn << 15) | (1u << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-
 template <bool A_MN>
 __global__ void __launch_bounds__(wg::THREADS, 1)
 gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, float* __restrict__ out,
@@ -39,8 +36,6 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* acc_full = empty_bar + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
   // split-K over gridDim.z: the token dimension is long (8192 .. 400k rows) and the output weight-sized, so one CTA per tile would
@@ -51,17 +46,12 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int kb1 = (kb0 + kb_per < k_blocks_all) ? kb0 + kb_per : k_blocks_all;
   const bool atomic_out = gridDim.z > 1;
 
-  if (warp == 0 && lane == 0) { prefetch_tmap(&tmA); prefetch_tmap(&tmB); }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    mbar_init(acc_full, 1);
+  if (warp == 0 && lane == 0) {
+    prefetch_tmap(&tmA); prefetch_tmap(&tmB);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 4); }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, BN);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     if (lane == 0) {
@@ -82,60 +72,60 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = make_idesc_bf16_mn(BM, BN, A_MN ? 1u : 0u);
-    int stage = 0;
+  } else if (warp >= 4) {
+    const int wq = warp & 3, qr = lane >> 2, qc = 2 * (lane & 3);
+    float acc[2][BN / 2];
+    int stage = 0, prev = -1;
     uint32_t phase = 0;
     for (int kb = kb0; kb < kb1; ++kb) {
       mbar_wait(&full_bar[stage], phase, 51);
-      tc_fence_after();
       const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES), sb = sa + A_BYTES;
-      if (elect_one()) {
+      wg_fence();
 #pragma unroll
-        for (int kk = 0; kk < BK / 16; ++kk) {  // 16 token rows = 2048 B further down the MN-major tile
-          const uint64_t da = A_MN ? make_desc_sw128(sa + kk * 2048, SUB, 1024) : make_desc_sw128(sa + kk * 32, 0, 1024);
-          const uint64_t db = make_desc_sw128(sb + kk * 2048, SUB, 1024);
-          umma_bf16(tmem_base, da, db, idesc, (kb > kb0) || (kk != 0));
+      for (int kk = 0; kk < BK / 16; ++kk) {  // 16 token rows = 2048 B further down the MN-major tile
+        const uint64_t db = make_desc_sw128(sb + kk * 2048, SUB, 1024);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint64_t da = A_MN ? make_desc_sw128(sa + h * SUB + kk * 2048, SUB, 1024) : make_desc_sw128(sa + h * 8192 + kk * 32, 0, 1024);
+          wgmma<BN, A_MN ? 1 : 0, 1>(acc[h], da, db, (kb > kb0) || (kk != 0));
         }
-        umma_commit(&empty_bar[stage]);
-        if (kb == kb1 - 1) umma_commit(acc_full);
       }
-      __syncwarp();
+      wg_commit();
+      wg_wait<1>();
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
+      prev = stage;
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
-  } else if (warp >= 4) {
-    const int quad = warp & 3, r = quad * 32 + lane, row = m0 + r;
-    mbar_wait(acc_full, 0, 52);
-    tc_fence_after();
-#pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-      uint32_t v[32];
-      tmem_ld32(tmem_base + ((uint32_t)(quad * 32) << 16) + 32 * c, v);
-      tmem_ld_wait();
-      if (row < M) {
-        float* dst = out + (size_t)row * ldc + n0 + 32 * c;
+    wg_wait<0>();
+    wg_fence_acc(acc[0]);
+    wg_fence_acc(acc[1]);
 #pragma unroll
-        for (int j = 0; j < 32; j += 4)
-          if (n0 + 32 * c + j < N) {
-            float4 o = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-            if (atomic_out) {
-              atomicAdd(dst + j, o.x); atomicAdd(dst + j + 1, o.y); atomicAdd(dst + j + 2, o.z); atomicAdd(dst + j + 3, o.w);
-              continue;
-            }
-            if (accumulate) {   // gradient accumulation over images / sub-iterations (decoder_train.cu)
-              const float4 t = *reinterpret_cast<const float4*>(dst + j);
-              o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w;
-            }
-            *reinterpret_cast<float4*>(dst + j) = o;
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int rs = 0; rs < 2; ++rs) {
+        const int row = m0 + 64 * h + 16 * wq + qr + 8 * rs;
+        if (row >= M) continue;
+        float* dst = out + (size_t)row * ldc;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int col = n0 + 8 * j + qc;
+          if (col >= N) continue;   // N % 8 == 0
+          float2 o = make_float2(acc[h][4 * j + 2 * rs], acc[h][4 * j + 2 * rs + 1]);
+          if (atomic_out) {
+            atomicAdd(dst + col, o.x); atomicAdd(dst + col + 1, o.y);
+            continue;
           }
+          if (accumulate) {   // gradient accumulation over images / sub-iterations (decoder_train.cu)
+            const float2 t = *reinterpret_cast<const float2*>(dst + col);
+            o.x += t.x; o.y += t.y;
+          }
+          *reinterpret_cast<float2*>(dst + col) = o;
+        }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, BN);
   }
 }
 
@@ -157,9 +147,9 @@ static int launch_gemm_mn(const __nv_bfloat16* A, const __nv_bfloat16* B, int M,
   if (A_MN ? make_tmap_bf16_2d(&tmA, A, K, M, lda, BK) : make_tmap_bf16_2d(&tmA, A, M, K, lda, BM)) return -1;
   if (make_tmap_bf16_2d(&tmB, B, K, N, ldb, BK)) return -1;
   dim3 grid((M + BM - 1) / BM, (N + BN - 1) / BN);
-  {   // split-K until ~2 CTAs per SM, at least 8 k-blocks per split
+  {   // split-K until ~2 CTAs per SM (132 SMs), at least 8 k-blocks per split
     const int k_blocks = (K + BK - 1) / BK, tiles = grid.x * grid.y;
-    int splits = (296 + tiles - 1) / tiles;
+    int splits = (264 + tiles - 1) / tiles;
     if (splits > (k_blocks + 7) / 8) splits = (k_blocks + 7) / 8;
     if (splits < 1) splits = 1;
     const int per = (k_blocks + splits - 1) / splits;

@@ -9,15 +9,16 @@
 // so per 128-row tile the tensor core runs  S = X Mq^T (+ PE Mq^T),  O = X I (residual, exact) + P V'  and the CUDA cores
 // only do the 8-head x T softmax and the LayerNorm.  Mq / V'^T come from two small plain GEMMs (decoder.cu).
 //
-// CTA = 1 TMA warp + 1 MMA thread + 16 row warps (4 column groups x 4 TMEM lane quadrants); persistent over a contiguous
-// range of (prompt, row-tile) items so Mq / V' stay resident while the prompt does not change.
+// CTA = 2 warpgroups + 1 TMA warp (64 rows of the tile each: wgmma chains, softmax and LayerNorm straight from the
+// accumulator fragments, P fed back from registers); persistent over a contiguous range of (prompt, row-tile) items so
+// Mq / V' stay resident while the prompt does not change.
 //   ring (3 stages x 32 KB): [a0_j | a1_j], j = 64-column slice of the 256 channels
 //     mode 1 (per-prompt keys): a0 = keys tile, a1 = pe tile:       S += a0 Mq_j^T + a1 Mq_j^T ; O[:, 64j..] = a0 I
 //     mode 0 (layer 0, shared): a0 = (src+pe) tile, a1 = src tile: S += a0 Mq_j^T             ; O[:, 64j..] = a1 I
-//   TMEM: O = columns [0,256), S = columns [256,320).
 #include "kernels.h"
 #include "ptx.cuh"
 #include "tensormap.h"
+#include "wgmma.cuh"
 
 namespace msam {
 
@@ -27,13 +28,10 @@ constexpr int SUB = 128 * 128;                 // [128 rows x 64 bf16] SWIZZLE_1
 constexpr int STAGE_BYTES = 2 * SUB;
 constexpr int OFF_M = STAGES * STAGE_BYTES;    // Mq[p]: 4 K-slices of [64 x 64]
 constexpr int OFF_V = OFF_M + 32768;           // V'^T[p]: [256 x 64]
-constexpr int OFF_P = OFF_V + 32768;           // probabilities [128 x 64]
-constexpr int OFF_I = OFF_P + 16384;           // identity [64 x 64]
-constexpr int OFF_STG = OFF_I + 8192;          // 2 output staging tiles [128 x 64]
-constexpr int OFF_BAR = OFF_STG + 2 * 16384;
+constexpr int OFF_I = OFF_V + 32768;           // identity [64 x 64]
+constexpr int OFF_BAR = OFF_I + 8192;
 constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
-constexpr int THREADS = 128 + 128 + 512;  // 4 control warps, 4 softmax warps, 16 LayerNorm warps
-constexpr uint32_t TM_O = 0, TM_S = 256, TMEM_COLS = 512;
+constexpr int THREADS = 256 + 128;             // 2 warpgroups, then a warpgroup whose first warp issues the TMA loads
 constexpr int TILES = 32;                      // 4096 image tokens / 128 rows
 constexpr int PF_AHEAD = 2;                    // L2 prefetch distance in work items
 }  // namespace i2t
@@ -53,8 +51,8 @@ __device__ __forceinline__ float ex2_approx(float x) {
 
 __global__ void __launch_bounds__(i2t::THREADS, 1)
 i2t_fused_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
-                 const __grid_constant__ CUtensorMap tmM, const __grid_constant__ CUtensorMap tmV,
-                 const __grid_constant__ CUtensorMap tmOut, const I2tParams p) {
+                 const __grid_constant__ CUtensorMap tmM, const __grid_constant__ CUtensorMap tmV, const I2tParams p,
+                 __nv_bfloat16* __restrict__ out) {
   using namespace i2t;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -62,32 +60,18 @@ i2t_fused_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* mv_full = empty_bar + STAGES;
   uint64_t* mv_empty = mv_full + 1;
-  uint64_t* s_full = mv_empty + 1;
-  uint64_t* p_full = s_full + 1;
-  uint64_t* o_full = p_full + 1;
-  uint64_t* o_empty = o_full + 1;
-  uint64_t* stg_full = o_empty + 1;   // [2] staging tile written (4 warps)
-  uint64_t* stg_free = stg_full + 2;  // [2] TMA store has read the tile
-  uint64_t* ln_done = stg_free + 2;   // every LayerNorm warp has read the statistics exchange of the item
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(ln_done + 1);
-  __shared__ __align__(16) float2 exch[4 * 128];
   __shared__ __align__(16) float rowp[768];  // out-proj bias | gamma | beta
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long total = (long)p.P * TILES;
   const int it_begin = (int)(total * blockIdx.x / gridDim.x), it_end = (int)(total * (blockIdx.x + 1) / gridDim.x);
 
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmA0); prefetch_tmap(&tmA1); prefetch_tmap(&tmM); prefetch_tmap(&tmV); prefetch_tmap(&tmOut);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    mbar_init(mv_full, 1); mbar_init(mv_empty, 1); mbar_init(s_full, 1); mbar_init(p_full, 4);
-    mbar_init(o_full, 1); mbar_init(o_empty, 16); mbar_init(ln_done, 16);
-    for (int i = 0; i < 2; ++i) { mbar_init(&stg_full[i], 4); mbar_init(&stg_free[i], 1); }
+  if (warp == 8 && lane == 0) {
+    prefetch_tmap(&tmA0); prefetch_tmap(&tmA1); prefetch_tmap(&tmM); prefetch_tmap(&tmV);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 8); }
+    mbar_init(mv_full, 1); mbar_init(mv_empty, 8);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, TMEM_COLS);
   for (int i = threadIdx.x; i < 256; i += THREADS) { rowp[i] = p.bias[i]; rowp[256 + i] = p.gamma[i]; rowp[512 + i] = p.beta[i]; }
   for (int i = threadIdx.x; i < 64 * 8; i += THREADS) {  // identity, K-major SW128: row n, 16-byte chunk c
     const int n = i >> 3, c = i & 7;
@@ -100,14 +84,14 @@ i2t_fused_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
     st_shared_v4(smem_u32(smem + OFF_I) + n * 128 + ((c ^ (n & 7)) << 4), v);
   }
   fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp >= 8) {
+    // O (128 registers) + S (32): the loading warpgroup hands its registers to the two consumer warpgroups
+    // (2 x 128 x 232 + 128 x 40 <= 64 K registers, the per-sub-partition split included)
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
     // ------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+    if (warp == 8 && lane == 0) {
       int stage = 0, cur_p = -1, nload = 0;
       uint32_t phase = 0;
       for (int item = it_begin; item < it_end; ++item) {
@@ -136,188 +120,123 @@ i2t_fused_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer (warp-uniform control flow, elected lane issues)
-    {
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, 64);
-      constexpr uint32_t idesc_o = make_idesc_bf16(128, 256);
-      const uint64_t di = make_desc_sw128(smem_u32(smem + OFF_I), 0, 1024);
-      const uint64_t dp = make_desc_sw128(smem_u32(smem + OFF_P), 0, 1024);
-      const uint64_t dv = make_desc_sw128(smem_u32(smem + OFF_V), 0, 1024);
-      int stage = 0, cur_p = -1, nload = 0, it = 0;
-      uint32_t phase = 0;
-      for (int item = it_begin; item < it_end; ++item, ++it) {
-        const int pp = item / TILES;
-        if (pp != cur_p) {
-          mbar_wait(mv_full, nload & 1, 12);
-          cur_p = pp; ++nload;
-        }
-        for (int j = 0; j < 4; ++j) {
-          mbar_wait(&full_bar[stage], phase, 13);
-          if (j == 0 && it > 0) mbar_wait(o_empty, (it - 1) & 1, 14);  // the row warps have pulled the previous O out of TMEM
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-          const uint64_t d0 = make_desc_sw128(sa, 0, 1024), d1 = make_desc_sw128(sa + SUB, 0, 1024);
-          const uint64_t dm = make_desc_sw128(smem_u32(smem + OFF_M + j * 8192), 0, 1024);
-          const uint64_t dr = p.mode ? d0 : d1;
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) umma_bf16(tmem_base + TM_S, d0 + 2 * k, dm + 2 * k, idesc_s, (j | k) != 0);
-            if (p.mode) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k) umma_bf16(tmem_base + TM_S, d1 + 2 * k, dm + 2 * k, idesc_s, 1);
-            }
-#pragma unroll
-            for (int k = 0; k < 4; ++k) umma_bf16(tmem_base + TM_O + 64 * j, dr + 2 * k, di + 2 * k, idesc_s, k != 0);
-            umma_commit(&empty_bar[stage]);
-            if (j == 3) umma_commit(s_full);
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        mbar_wait(p_full, it & 1, 15);
-        tc_fence_after();
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_bf16(tmem_base + TM_O, dp + 2 * k, dv + 2 * k, idesc_o, 1);
-          umma_commit(o_full);
-          if (item + 1 == it_end || (item + 1) / TILES != pp) umma_commit(mv_empty);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp < 4) {
-    // ------------------------------------------------------------ store warps: warp 2 -> staging tile 0, warp 3 -> tile 1.
-    // Each tile is used twice per item: column group sb (use 2*it), then column group sb + 2 (use 2*it + 1).
-    if (lane == 0) {
-      const int sb = warp - 2;
-      const uint8_t* stg = smem + OFF_STG + sb * 16384;
-      uint32_t n = 0;
-      for (int item = it_begin; item < it_end; ++item) {
-        const int orow = (item / TILES) * 4096 + (item % TILES) * 128;
-        for (int round = 0; round < 2; ++round, ++n) {
-          mbar_wait(&stg_full[sb], n & 1, 18);
-          tma_store_2d(&tmOut, stg, 64 * (sb + 2 * round), orow);
-          tma_store_commit();
-          tma_store_wait_read();
-          mbar_arrive(&stg_free[sb]);
-        }
-      }
-      tma_store_wait_all();
-    }
-  } else if (warp < 8) {
-    // ------------------------------------------------------------ softmax warps: thread = image token (row), 8 heads x T tokens
-    const int quad = warp & 3, r = quad * 32 + lane;
-    const uint32_t tlane = tmem_base + ((uint32_t)(quad * 32) << 16);
-    const uint32_t prow = smem_u32(smem + OFF_P) + r * 128;
-    const int T = p.T;
-    int it = 0;
-    for (int item = it_begin; item < it_end; ++item, ++it) {
-      const float4* c4 = reinterpret_cast<const float4*>(p.sbias + (size_t)(item / TILES) * 64);
-      mbar_wait(s_full, it & 1, 16);
-      tc_fence_after();
-#pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        uint32_t v[32];
-        tmem_ld32(tlane + TM_S + 32 * half, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int hh = 0; hh < 4; ++hh) {
-          const float4 ca = __ldg(c4 + (half * 4 + hh) * 2), cb = __ldg(c4 + (half * 4 + hh) * 2 + 1);
-          const float c[8] = {ca.x, ca.y, ca.z, ca.w, cb.x, cb.y, cb.z, cb.w};
-          float sc[8], m = -1e30f;
-#pragma unroll
-          for (int t = 0; t < 8; ++t) {
-            sc[t] = (t < T) ? (__uint_as_float(v[hh * 8 + t]) + c[t]) * 1.4426950408889634f : -1e30f;
-            m = fmaxf(m, sc[t]);
-          }
-          float l = 0.f;
-#pragma unroll
-          for (int t = 0; t < 8; ++t) { sc[t] = ex2_approx(sc[t] - m); l += sc[t]; }
-          const float inv = __fdividef(1.0f, l);
-          st_shared_v4(prow + (((half * 4 + hh) ^ (r & 7)) << 4),
-                       make_uint4(pack_bf16(sc[0] * inv, sc[1] * inv), pack_bf16(sc[2] * inv, sc[3] * inv),
-                                  pack_bf16(sc[4] * inv, sc[5] * inv), pack_bf16(sc[6] * inv, sc[7] * inv)));
-        }
-      }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-    }
-  } else {
-    // ------------------------------------------------------------ LayerNorm warps: O = residual + P V' (+ bias) -> LN(256)
-    const int quad = warp & 3, grp = (warp - 8) >> 2, r = quad * 32 + lane;
-    const uint32_t tlane = tmem_base + ((uint32_t)(quad * 32) << 16);
-    const int sb = grp & 1;                                  // staging tile shared by groups sb and sb + 2
-    const uint32_t stg = smem_u32(smem + OFF_STG + sb * 16384);
-    int it = 0;
-    for (int item = it_begin; item < it_end; ++item, ++it) {
-      float f[64];
-      mbar_wait(o_full, it & 1, 17);
-      tc_fence_after();
-      float s4[4] = {0.f, 0.f, 0.f, 0.f}, q4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t v[32];
-        tmem_ld32(tlane + TM_O + 64 * grp + 32 * c, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const float x = __uint_as_float(v[j]) + rowp[64 * grp + c * 32 + j];
-          f[c * 32 + j] = x;
-          s4[j & 3] += x;
-          q4[j & 3] = fmaf(x, x, q4[j & 3]);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(o_empty);
-      // group statistics in one pass (fp32 sums of 64 O(1) values: the cancellation error is ~1e-5 of the variance),
-      // combined across the four column groups with Chan's formula
-      const float sum_g = (s4[0] + s4[1]) + (s4[2] + s4[3]);
-      const float mean_g = sum_g * (1.0f / 64);
-      const float m2_g = fmaxf(((q4[0] + q4[1]) + (q4[2] + q4[3])) - sum_g * mean_g, 0.f);
-      if (it > 0) mbar_wait(ln_done, (it - 1) & 1, 20);  // every warp has read the previous item's statistics
-      exch[grp * 128 + r] = make_float2(mean_g, m2_g);
-      named_bar_sync(1, 512);
-      float mean = 0.f;
-      float2 st[4];
-#pragma unroll
-      for (int g = 0; g < 4; ++g) { st[g] = exch[g * 128 + r]; mean += st[g].x; }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(ln_done);
-      mean *= 0.25f;
-      float m2 = 0.f;
-#pragma unroll
-      for (int g = 0; g < 4; ++g) { const float d = st[g].x - mean; m2 += st[g].y + d * d * 64.f; }
-      const float rstd = rsqrtf(m2 * (1.0f / 256) + p.eps);
-      const float shift = -mean * rstd;
-
-      // staging tile sb: use n = 2*it (+1 for column groups 2, 3); free once the store of use n-1 has read it
-      const uint32_t n = 2 * it + (grp >> 1);
-      if (grp >= 2) mbar_wait(&stg_free[sb], n & 1, 19);  // (use n-2 first: a parity wait only resolves one phase back)
-      mbar_wait(&stg_free[sb], (n & 1) ^ 1, 19);
-#pragma unroll
-      for (int j = 0; j < 64; j += 8) {
-        float y[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q)
-          y[q] = fmaf(fmaf(f[j + q], rstd, shift), rowp[256 + 64 * grp + j + q], rowp[512 + 64 * grp + j + q]);
-        st_shared_v4(stg + r * 128 + (((j >> 3) ^ (r & 7)) << 4),
-                     make_uint4(pack_bf16(y[0], y[1]), pack_bf16(y[2], y[3]), pack_bf16(y[4], y[5]), pack_bf16(y[6], y[7])));
-      }
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&stg_full[sb]);
-    }
+    return;
   }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
+  // ------------------------------------------------------------ warpgroup g: rows [64 g, 64 g + 64) of each tile.
+  // Fragment element i of a thread: row 64 g + 16 wq + qr + 8 ((i >> 1) & 1), column 8 (i >> 2) + qc + (i & 1).
+  const int g = warp >> 2, wq = warp & 3, qr = lane >> 2, qc = 2 * (lane & 3);
+  const uint32_t own = (uint32_t)g * 8192u;
+  const uint64_t di = make_desc_sw128(smem_u32(smem + OFF_I), 0, 1024);
+  const uint32_t aV = smem_u32(smem + OFF_V);
+  const int T = p.T;
+  int stage = 0, cur_p = -1, nload = 0;
+  uint32_t phase = 0;
+  for (int item = it_begin; item < it_end; ++item) {
+    const int pp = item / TILES, rt = item % TILES;
+    if (pp != cur_p) {
+      mbar_wait(mv_full, nload & 1, 12);
+      cur_p = pp; ++nload;
+    }
+    float sacc[32], o[128];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      mbar_wait(&full_bar[stage], phase, 13);
+      const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + own;
+      const uint64_t d0 = make_desc_sw128(sa, 0, 1024), d1 = make_desc_sw128(sa + SUB, 0, 1024);
+      const uint64_t dm = make_desc_sw128(smem_u32(smem + OFF_M + j * 8192), 0, 1024);
+      const uint64_t dr = p.mode ? d0 : d1;
+      float(&oj)[32] = *reinterpret_cast<float(*)[32]>(&o[32 * j]);   // columns [64 j, 64 j + 64) of O
+      wg_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma<64>(sacc, d0 + 2 * k, dm + 2 * k, (j | k) != 0);
+      if (p.mode) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma<64>(sacc, d1 + 2 * k, dm + 2 * k, 1);
+      }
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma<64>(oj, dr + 2 * k, di + 2 * k, k != 0);
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc(sacc);
+      wg_fence_acc(oj);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    // softmax over the T tokens of each head h (columns 8 h + t): this thread holds t = qc, qc + 1
+    const float* cb = p.sbias + (size_t)pp * 64;
+    uint32_t pk[16];
+#pragma unroll
+    for (int h = 0; h < 8; ++h) {
+      const float2 c = __ldg(reinterpret_cast<const float2*>(cb + 8 * h + qc));
+#pragma unroll
+      for (int rs = 0; rs < 2; ++rs) {
+        const float s0 = (qc < T) ? (sacc[4 * h + 2 * rs] + c.x) * 1.4426950408889634f : -1e30f;
+        const float s1 = (qc + 1 < T) ? (sacc[4 * h + 2 * rs + 1] + c.y) * 1.4426950408889634f : -1e30f;
+        float m = fmaxf(s0, s1);
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+        const float e0 = ex2_approx(s0 - m), e1 = ex2_approx(s1 - m);
+        float l = e0 + e1;
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        const float inv = __fdividef(1.0f, l);
+        pk[2 * h + rs] = pack_bf16(e0 * inv, e1 * inv);
+      }
+    }
+    // O += P V', per 64-column slice j (V'^T rows [64 j, 64 j + 64))
+    wg_fence();
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      float(&oj)[32] = *reinterpret_cast<float(*)[32]>(&o[32 * j]);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const uint32_t a[4] = {pk[4 * k], pk[4 * k + 1], pk[4 * k + 2], pk[4 * k + 3]};
+        wgmma_rs<64>(oj, a, make_desc_sw128(aV + 8192 * j + 32 * k, 0, 1024), 1);
+      }
+    }
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc(o);
+    if (item + 1 == it_end || (item + 1) / TILES != pp) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(mv_empty);
+    }
+    // + out-proj bias, LayerNorm over the 256 channels of each row (this thread: 64 of them, the quad: all)
+#pragma unroll
+    for (int rs = 0; rs < 2; ++rs) {
+      float sum = 0.f;
+#pragma unroll
+      for (int jj = 0; jj < 32; ++jj) {
+        const int col = 8 * jj + qc;
+        o[4 * jj + 2 * rs] += rowp[col];
+        o[4 * jj + 2 * rs + 1] += rowp[col + 1];
+        sum += o[4 * jj + 2 * rs] + o[4 * jj + 2 * rs + 1];
+      }
+      sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+      sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+      const float mean = sum * (1.0f / 256);
+      float q = 0.f;
+#pragma unroll
+      for (int jj = 0; jj < 32; ++jj) {
+        const float d0 = o[4 * jj + 2 * rs] - mean, d1 = o[4 * jj + 2 * rs + 1] - mean;
+        q = fmaf(d0, d0, fmaf(d1, d1, q));
+      }
+      q += __shfl_xor_sync(0xffffffffu, q, 1);
+      q += __shfl_xor_sync(0xffffffffu, q, 2);
+      const float rstd = rsqrtf(q * (1.0f / 256) + p.eps);
+      const float shift = -mean * rstd;
+      __nv_bfloat16* orow = out + ((size_t)pp * 4096 + rt * 128 + 64 * g + 16 * wq + qr + 8 * rs) * 256;
+#pragma unroll
+      for (int jj = 0; jj < 32; ++jj) {
+        const int col = 8 * jj + qc;
+        const float y0 = fmaf(fmaf(o[4 * jj + 2 * rs], rstd, shift), rowp[256 + col], rowp[512 + col]);
+        const float y1 = fmaf(fmaf(o[4 * jj + 2 * rs + 1], rstd, shift), rowp[256 + col + 1], rowp[512 + col + 1]);
+        *reinterpret_cast<uint32_t*>(orow + col) = pack_bf16(y0, y1);
+      }
+    }
   }
 }
 
@@ -330,20 +249,19 @@ int launch_i2t_fused(const I2tFusedArgs& a, int num_sms, cudaStream_t stream) {
     if (e != cudaSuccess) return set_error("i2t_fused: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
     attr_set = true;
   }
-  CUtensorMap tmA0, tmA1, tmM, tmV, tmOut;
+  CUtensorMap tmA0, tmA1, tmM, tmV;
   const uint64_t xrows = a.mode ? (uint64_t)a.P * 4096 : 4096;
   if (make_tmap_bf16_2d(&tmA0, a.a0, xrows, 256, 256, 128)) return -1;
   if (make_tmap_bf16_2d(&tmA1, a.a1, 4096, 256, 256, 128)) return -1;
   if (make_tmap_bf16_2d(&tmM, a.mq, (uint64_t)a.P * 64, 256, 256, 64)) return -1;
   if (make_tmap_bf16_2d(&tmV, a.vt, 256, (uint64_t)a.P * 64, (uint64_t)a.P * 64, 256)) return -1;
-  if (make_tmap_bf16_2d(&tmOut, a.out, (uint64_t)a.P * 4096, 256, 256, 128)) return -1;
   I2tParams p;
   p.P = a.P; p.T = a.T; p.mode = a.mode; p.sbias = a.sbias; p.bias = a.bias; p.gamma = a.gamma; p.beta = a.beta; p.eps = a.eps;
   const long total = (long)a.P * TILES;
   const int grid = total < num_sms ? (int)total : num_sms;
   const double bytes = (double)a.P * 4096 * 256 * 2 * (a.mode ? 2 : 1) + (double)a.P * 64 * 256 * 2 * 2;
   prof_begin(stream, a.mode ? "i2t_fused (own keys)" : "i2t_fused (shared image)", (double)a.P * 4096 * (2.0 * 256 * 64 * (a.mode ? 2 : 1) + 2.0 * 64 * 256), bytes);
-  i2t_fused_kernel<<<grid, THREADS, SMEM_BYTES, stream>>>(tmA0, tmA1, tmM, tmV, tmOut, p);
+  i2t_fused_kernel<<<grid, THREADS, SMEM_BYTES, stream>>>(tmA0, tmA1, tmM, tmV, p, a.out);
   prof_end(stream);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error("i2t_fused launch failed: %s", cudaGetErrorString(e));

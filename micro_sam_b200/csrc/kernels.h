@@ -9,7 +9,7 @@
 namespace msam {
 
 // Launch with programmatic dependent launch allowed (see ptx.cuh:pdl_wait).  ONLY for kernels in which every thread executes
-// pdl_wait() before touching global memory.  The attribute is only set when MSAM_PDL=1 (measured: no gain, see engine.cu).
+// pdl_wait() before touching global memory.  The attribute is only set when MSAM_PDL=1 (see engine.cu).
 bool pdl_enabled();   // engine.cu
 template <typename... KArgs, typename... Args>
 cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
@@ -50,8 +50,6 @@ struct GemmArgs {
   float ln_eps = 1e-5f;
 };
 int launch_gemm(const GemmArgs& a, int num_sms, cudaStream_t stream);
-// gemm2.cu: 2-SM (cta_group::2) kernel for large plain products; returns 1 if launched, 0 if the problem does not qualify
-int launch_gemm_2sm(const GemmArgs& a, int num_sms, cudaStream_t stream);
 
 // ---- gemm_tn.cu : out[M,N] fp32 = A[K,M]^T B[K,N]  (weight gradient dW = dY^T X; both operands MN-major)
 int launch_gemm_tn(const __nv_bfloat16* A, const __nv_bfloat16* B, int M, int N, int K, int lda, int ldb, float* out, int ldc,

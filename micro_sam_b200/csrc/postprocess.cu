@@ -125,8 +125,7 @@ mask_stats_kernel(const float* __restrict__ low_res, PostGeom g, float thr, cons
 // low-res rows (4 output rows per pair, weights 1/8, 3/8, 5/8, 7/8; the clamped border rows are handled apart).  The
 // horizontal interpolation is done once per row pair; the per-pixel work is one FMUL + FFMA for the value and, per
 // threshold, one FADD + IMAD.HI that adds the sign bit of (t - v) to the counter (v > t  <=>  sign(t - v) = 1) -- all on
-// the FMA pipe, because the first version (setp / iadd / sel per pixel) was bound by the ALU pipe (ncu: issue active
-// 87 %, 27 instructions per pixel).  Same interp_axis / bilerp arithmetic as the generic kernel: bit-identical results.
+// the FMA pipe, because a setp / iadd / sel per pixel (27 instructions per pixel) is bound by the ALU pipe.  Same interp_axis / bilerp arithmetic as the generic kernel: bit-identical results.
 // grid = n_masks, block = 512 (two row ranges x 256 low-res columns).
 __global__ void __launch_bounds__(512)
 mask_stats_x4_kernel(const float* __restrict__ low_res, PostGeom g, float thr, const float* __restrict__ thr_arr, float off,
@@ -784,8 +783,7 @@ paint_min_area_kernel(const float* __restrict__ low_res, const int32_t* __restri
 // Tile version for the common geometry input_size == original_size == (1024, 1024): one block paints a 32 x 32 pixel region
 // for ALL survivors.  The region depends on a 10 x 10 patch of each mask's low-res logits only, which the block stages in
 // shared memory (double buffered: the next mask's patch is fetched while the current one is evaluated) -- 0.1 global loads
-// per (pixel, mask) instead of 4, which is what bounded the per-pixel kernel with hundreds of overlapping survivors
-// (1.0 ms per tile at ~190 survivors, profiles/r2_launches_amg_vit_b_1tile.txt).  Survivors are visited in ascending
+// per (pixel, mask) instead of 4, which is what bounds a per-pixel kernel with hundreds of overlapping survivors.  Survivors are visited in ascending
 // (area, -position) order (block-local bitonic sort), so a pixel is final at its first hit and the block stops as soon as
 // all its 1024 pixels are decided.  Same interp_axis / bilerp arithmetic as `stage1`: bit-identical results.
 __global__ void __launch_bounds__(256)

@@ -1,5 +1,5 @@
-// sm_100a PTX wrappers: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), UMMA descriptors.
-// Hand-written for this repo; bit layouts follow the PTX ISA "tcgen05 matrix descriptors" tables.
+// sm_90a PTX wrappers: mbarrier, TMA (cp.async.bulk.tensor), wgmma synchronisation and shared-memory matrix descriptors.
+// Hand-written for this repo; bit layouts follow the PTX ISA "warpgroup-level matrix shared memory layout" tables.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -12,19 +12,10 @@ namespace msam {
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
 
-// One lane of a fully active warp.  Issuing tcgen05.mma / TMA from `if (elect_one())` inside warp-uniform control flow
-// lets the compiler keep descriptors in uniform registers; under `if (lane == 0)` it emits a per-lane "waterfall"
-// (ELECT + 5 x R2UR + branch, ~17 instructions and ~100 cycles per MMA), which starves the tensor pipe for N <= 128.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-
 // ------------------------------------------------------------------ programmatic dependent launch
 // Every kernel of the encoder chain is launched with the programmatic-stream-serialization attribute (kernels.h:launch_pdl): its
 // CTAs may become resident while the previous kernel of the stream is still draining, run their prologue (barrier init,
-// tensor-map prefetch, TMEM allocation) and then block here until the previous grid has completed and flushed -- every thread
+// tensor-map prefetch) and then block here until the previous grid has completed and flushed -- every thread
 // executes the wait before its first global-memory access, so the memory semantics are those of ordinary stream order.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -51,16 +42,14 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Spin with a watchdog: a protocol bug traps (-> a CUDA error the host reports) instead of hanging the GPU box.
-static __device__ __noinline__ void mbar_timeout(uint32_t bar, uint32_t parity, int tag) {
-  printf("msam: mbarrier timeout tag=%d block=(%d,%d,%d) thread=%d bar=%u parity=%u\n", tag, blockIdx.x, blockIdx.y,
-         blockIdx.z, threadIdx.x, bar, parity);
-  __trap();
-}
+// Spin with a watchdog: a protocol bug traps (-> a CUDA error the host reports) instead of hanging the GPU.  No printf here:
+// a function call inside the spin loop would make ptxas serialise every wgmma whose pipeline crosses it.  `tag` names the
+// wait site for a debug build that prints it.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int tag = 0) {
+  (void)tag;
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 26)) mbar_timeout(smem_u32(bar), parity, tag);  // seconds: a protocol bug, not a slow tile
+    if (++spins > (1u << 26)) asm volatile("trap;");  // seconds: a protocol bug, not a slow tile
   }
 }
 
@@ -96,74 +85,30 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 __device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
-// generic-proxy smem writes -> visible to the async proxy (TMA / UMMA operand reads)
+// generic-proxy smem writes -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ------------------------------------------------------------------ tcgen05
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// Whole warp executes.  Writes the TMEM base address (lane 0, column base) to *dst_smem.
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; bf16 x bf16 -> fp32.  One thread issues.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrive once all previously issued tcgen05.mma of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// ------------------------------------------------------------------ wgmma (warpgroup MMA, wrappers in wgmma.cuh)
+// Order: wg_fence() before the first wgmma of a group (and whenever the accumulator registers were written by other
+// instructions), wg_commit() after the group, wg_wait<n>() until at most n groups are pending, then wg_fence_acc() so that the
+// compiler does not move reads of the accumulators above the wait.
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+template <int R>
+__device__ __forceinline__ void wg_fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// TMEM -> registers: this warp's 32 lanes (lane field of taddr must be 32*(warp_id%4)), N consecutive 32-bit columns.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
-      "[%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld2(uint32_t taddr, uint32_t& a, uint32_t& b) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x2.b32 {%0,%1}, [%2];" : "=r"(a), "=r"(b) : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ------------------------------------------------------------------ UMMA descriptors
-// Shared-memory matrix descriptor (64-bit):
+// ------------------------------------------------------------------ wgmma shared-memory matrix descriptors
+// 64-bit descriptor (sm_90):
 //   [0,14)  start address >> 4        [16,30) leading-dim byte offset >> 4   [32,46) stride-dim byte offset >> 4
-//   [46,48) version = 1 (sm_100)      [49,52) base offset = 0                [61,64) layout: 0 none, 2 = 128B swizzle
+//   [49,52) base offset = 0           [62,64) layout: 1 = 128B swizzle
 // K-major SW128 tile (rows of 64 bf16 = 128 B, TMA SWIZZLE_128B, 1024-B aligned):
 //   SBO = 1024 B (8 rows * 128 B); LBO unused.  Advancing K by 16 elements (32 B) inside the 128-B atom = +2 on the
-//   encoded start address.
+//   encoded start address.  The second 64-row half of a 128-row tile starts 8192 B further.
 // MN-major SW128 tile (smem rows indexed by K, 64 contiguous MN elements = 128 B per row):
 //   SBO = 1024 B (8 K-rows); LBO = byte distance between consecutive 64-element MN blocks.  Advancing K by 16 rows
 //   = +2048 B.
@@ -172,15 +117,8 @@ __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr, uint32_t
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
-}
-// Instruction descriptor for kind::f16, BF16 x BF16 -> FP32:
-//   [4,6) D fmt (1 = F32)  [7,10) A fmt (1 = BF16)  [10,13) B fmt (1 = BF16)  [15] A major (0 = K)  [16] B major
-//   (0 = K, 1 = MN)  [17,23) N >> 3   [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N, uint32_t b_mn_major = 0) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (b_mn_major << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
 }
 
 // explicit shared-space 16-byte store (pointers derived from the aligned dynamic-smem base are otherwise treated as

@@ -4,9 +4,9 @@
 //   out_h[t]         = Wv_h (sum_j p[(h,t), j] x_j) + bv_h                                   (k bias: softmax invariant)
 // i.e. a flash attention with "head dim" 256 in which the image tokens x ([4096, 256] bf16, read ONCE: 2 MB per prompt
 // instead of the 4 MB written + 4 MB read by the k/v projection GEMM and the attention core) are both K and V:
-//   S = Q' X^T (+ Q' PE^T)   tcgen05.mma 128 x 64 x 16, K-major operands         (X tile [64 keys x 256] via TMA, SW128)
-//   U += P X                 tcgen05.mma 128 x 256 x 16, X consumed MN-major from the same shared-memory tile
-// with the online softmax (lazy rescaling of U in TMEM) on 4 warps, thread = row (head, token).  The tiny per-head value
+//   S = Q' X^T (+ Q' PE^T)   wgmma m64n64k16, K-major operands                  (X tile [64 keys x 256] via TMA, SW128)
+//   U += P X                 wgmma m64n256k16, P from registers, X consumed MN-major from the same shared-memory tile
+// with the online softmax on the accumulator fragments; one warpgroup per 64 rows (head, token).  The tiny per-head value
 // projection runs afterwards (t2i_head_proj_kernel).
 //
 // One work item = 128 Q' rows against 4096 image tokens: mode 1 -> one prompt (rows h*16 + t, own keys); mode 0 (layer 0:
@@ -14,6 +14,7 @@
 #include "kernels.h"
 #include "ptx.cuh"
 #include "tensormap.h"
+#include "wgmma.cuh"
 
 namespace msam {
 
@@ -22,54 +23,40 @@ constexpr int PESLOTS = 4;
 constexpr int XT = 64;                              // image tokens per tile
 constexpr int SUBX = XT * 128;                      // [64 tokens x 64 channels] sub-tile, 8 KB
 constexpr int XSTAGE_BYTES = 4 * SUBX;              // 32 KB
-// ROWS = Q' rows per work item: 128 (tcgen05 M = 128), or 64 for one prompt with T <= 8 tokens (M = 64: the accumulator
-// rows live in lanes 0..15 of each TMEM sub-partition, the A tiles and their shared-memory reads halve, and the space
-// buys a 4th image-token stage).
+// ROWS = Q' rows per work item: 128 (two warpgroups), or 64 for one prompt with T <= 8 tokens (one warpgroup; the A tiles
+// and their shared-memory reads halve, and the space buys a 4th image-token stage).
 template <int ROWS>
 struct Cfg {
+  static constexpr int NWG = ROWS / 64;
+  static constexpr int THREADS = NWG * 128 + 128;   // consumer warpgroups, then a warpgroup whose first two warps load
   static constexpr int XSTAGES = ROWS == 64 ? 4 : 3;
   static constexpr int QSUB = ROWS * 128;           // one 64-channel slice of Q'
   static constexpr int OFF_PE = XSTAGES * XSTAGE_BYTES;
   static constexpr int OFF_Q = OFF_PE + PESLOTS * SUBX;
-  static constexpr int OFF_P = OFF_Q + 4 * QSUB;    // P [ROWS x 64]
-  static constexpr int OFF_BAR = OFF_P + QSUB;
+  static constexpr int OFF_BAR = OFF_Q + 4 * QSUB;
   static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
 };
-constexpr int THREADS = 256;
-constexpr uint32_t TM_U = 0, TM_S = 256, TMEM_COLS = 512;
 constexpr int NTILES = 4096 / XT;
-constexpr float RESCALE_T = 8.0f;                   // lazy rescale threshold (log2 units)
 }  // namespace t2i
 
 struct T2iParams {
-  int n_items, mode;
+  int n_items;
   float* out;  // [n_items * 128, 256] fp32: softmax-weighted mean of the image tokens per row
 };
 
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]),
-      "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]),
-      "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ float ex2f(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
 
-template <int ROWS>
-__global__ void __launch_bounds__(t2i::THREADS, 1)
+template <int ROWS, int MODE>
+__global__ void __launch_bounds__(t2i::Cfg<ROWS>::THREADS, 1)
 t2i_fused_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmXS,
                  const __grid_constant__ CUtensorMap tmQ, const T2iParams p) {
   using namespace t2i;
   using C = Cfg<ROWS>;
-  constexpr int XSTAGES = C::XSTAGES, QSUB = C::QSUB, OFF_PE = C::OFF_PE, OFF_Q = C::OFF_Q, OFF_P = C::OFF_P, OFF_BAR = C::OFF_BAR;
+  constexpr int NWG = C::NWG, XSTAGES = C::XSTAGES, QSUB = C::QSUB, OFF_PE = C::OFF_PE, OFF_Q = C::OFF_Q, OFF_BAR = C::OFF_BAR;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* xfull = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
@@ -78,31 +65,22 @@ t2i_fused_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
   uint64_t* peempty = pefull + PESLOTS;
   uint64_t* q_full = peempty + PESLOTS;
   uint64_t* q_empty = q_full + 1;
-  uint64_t* s_full = q_empty + 1;    // [2]
-  uint64_t* s_empty = s_full + 2;    // [2]
-  uint64_t* p_full = s_empty + 2;
-  uint64_t* p_empty = p_full + 1;
-  uint64_t* u_full = p_empty + 1;
-  uint64_t* u_empty = u_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(u_empty + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) { prefetch_tmap(&tmX); prefetch_tmap(&tmXS); prefetch_tmap(&tmQ); }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < XSTAGES; ++i) { mbar_init(&xfull[i], 1); mbar_init(&xempty[i], 1); }
-    for (int i = 0; i < PESLOTS; ++i) { mbar_init(&pefull[i], 1); mbar_init(&peempty[i], 1); }
-    mbar_init(q_full, 1); mbar_init(q_empty, 1);
-    for (int i = 0; i < 2; ++i) { mbar_init(&s_full[i], 1); mbar_init(&s_empty[i], 4); }
-    mbar_init(p_full, 4); mbar_init(p_empty, 1); mbar_init(u_full, 1); mbar_init(u_empty, 4);
+  if (warp == NWG * 4 && lane == 0) {
+    prefetch_tmap(&tmX); prefetch_tmap(&tmXS); prefetch_tmap(&tmQ);
+    for (int i = 0; i < XSTAGES; ++i) { mbar_init(&xfull[i], 1); mbar_init(&xempty[i], NWG * 4); }
+    for (int i = 0; i < PESLOTS; ++i) { mbar_init(&pefull[i], 1); mbar_init(&peempty[i], NWG * 4); }
+    mbar_init(q_full, 1); mbar_init(q_empty, NWG * 4);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp >= NWG * 4) {
+    // The U accumulator alone takes 128 registers: the loading warpgroup hands its registers to the consumer warpgroups
+    // (2 x 128 x 232 + 128 x 40 <= 64 K registers, the per-sub-partition split included).
+    if constexpr (NWG == 2) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    if (warp == NWG * 4) {
     // ------------------------------------------------------------ TMA producer: Q' per item, image-token tiles (K = V)
     if (lane == 0) {
       int stage = 0, ni = 0;
@@ -112,9 +90,9 @@ t2i_fused_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
         mbar_expect_tx(q_full, 4 * QSUB);
 #pragma unroll
         for (int j = 0; j < 4; ++j) tma_load_2d(smem + OFF_Q + j * QSUB, &tmQ, q_full, 64 * j, item * ROWS);
-        const int row0 = p.mode ? item * 4096 : 0;
+        const int row0 = MODE ? item * 4096 : 0;
         for (int kt = 0; kt < NTILES; ++kt) {
-          if (p.mode && kt + 8 < NTILES) {  // own keys: a tile 8 steps ahead -> L2
+          if (MODE && kt + 8 < NTILES) {  // own keys: a tile 8 steps ahead -> L2
 #pragma unroll
             for (int j = 0; j < 4; ++j) tma_prefetch_2d(&tmX, 64 * j, row0 + (kt + 8) * XT);
           }
@@ -127,7 +105,7 @@ t2i_fused_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
         }
       }
     }
-  } else if (warp == 2) {
+    } else if (warp == NWG * 4 + 1) {
     // ------------------------------------------------------------ TMA producer: second score operand (pe, or src + pe)
     if (lane == 0) {
       int slot = 0;
@@ -143,191 +121,124 @@ t2i_fused_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer (warp-uniform control flow, elected lane issues)
-    {
-      constexpr uint32_t idesc_s = make_idesc_bf16(ROWS, XT);
-      constexpr uint32_t idesc_u = make_idesc_bf16(ROWS, 256, 1);  // B = X consumed MN-major
-      const uint32_t aQ = smem_u32(smem + OFF_Q), aP = smem_u32(smem + OFF_P);
-      int sstage = 0, vstage = 0, slot = 0, ni = 0;
-      uint32_t sphase = 0, vphase = 0, pephase = 0;
-      uint32_t ns = 0, npv = 0;  // running tile counters (S tiles issued, PV tiles issued)
-      auto issue_pv = [&](bool first_of_item) {
-        mbar_wait(p_full, npv & 1, 23);
-        if (!p.mode) mbar_wait(&xfull[vstage], vphase, 24);  // mode 0: S did not wait for the value tile
-        if (first_of_item && ni > 0) mbar_wait(u_empty, (ni - 1) & 1, 25);
-        tc_fence_after();
-        const uint32_t xb = smem_u32(smem + vstage * XSTAGE_BYTES);
-        if (elect_one()) {
-#pragma unroll
-          for (int kk = 0; kk < XT / 16; ++kk) {
-            const uint64_t da = make_desc_sw128(aP + kk * 32, 0, 1024);
-            const uint64_t db = make_desc_sw128(xb + kk * 2048, SUBX, 1024);  // 16 tokens = 2048 B; next 64 channels = 8 KB
-            umma_bf16(tmem_base + TM_U, da, db, idesc_u, !(first_of_item && kk == 0));
-          }
-          umma_commit(&xempty[vstage]);
-          umma_commit(p_empty);
-        }
-        __syncwarp();
-        ++npv;
-        if (++vstage == XSTAGES) { vstage = 0; vphase ^= 1; }
-      };
-      for (int item = blockIdx.x; item < p.n_items; item += gridDim.x, ++ni) {
-        mbar_wait(q_full, ni & 1, 26);
-        for (int kt = 0; kt < NTILES; ++kt) {
-          const int b = ns & 1;
-          mbar_wait(&s_empty[b], ((ns >> 1) & 1) ^ 1, 27);
-          const uint32_t ts = tmem_base + TM_S + b * XT;
-          if (p.mode) {
-            mbar_wait(&xfull[sstage], sphase, 28);
-            tc_fence_after();
-            const uint32_t xb = smem_u32(smem + sstage * XSTAGE_BYTES);
-            if (elect_one()) {
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                  umma_bf16(ts, make_desc_sw128(aQ + j * QSUB + k * 32, 0, 1024), make_desc_sw128(xb + j * SUBX + k * 32, 0, 1024),
-                            idesc_s, (j | k) != 0);
-              }
-            }
-            __syncwarp();
-          }
-          if (++sstage == XSTAGES) { sstage = 0; sphase ^= 1; }
-          for (int j = 0; j < 4; ++j) {
-            mbar_wait(&pefull[slot], pephase, 29);
-            tc_fence_after();
-            const uint32_t pb = smem_u32(smem + OFF_PE + slot * SUBX);
-            if (elect_one()) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k)
-                umma_bf16(ts, make_desc_sw128(aQ + j * QSUB + k * 32, 0, 1024), make_desc_sw128(pb + k * 32, 0, 1024), idesc_s,
-                          (p.mode | j | k) != 0);
-              umma_commit(&peempty[slot]);
-              if (j == 3) {
-                umma_commit(&s_full[b]);
-                if (kt == NTILES - 1) umma_commit(q_empty);  // every read of Q' by this item has been issued
-              }
-            }
-            __syncwarp();
-            if (++slot == PESLOTS) { slot = 0; pephase ^= 1; }
-          }
-          ++ns;
-          if (kt >= 1) issue_pv(kt == 1);
-        }
-        issue_pv(false);
-        if (elect_one()) umma_commit(u_full);
-        __syncwarp();
-      }
     }
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------ softmax warps: thread = row (head, token)
-    // M = 128: row r <-> TMEM lane r.  M = 64: rows 16q .. 16q+15 live in lanes 0..15 of sub-partition q; lanes 16..31 idle
-    // (they still take part in the warp-collective tcgen05.ld / st and in the votes)
-    const int quad = warp & 3;
-    const bool active = ROWS == 128 || lane < 16;
-    const int r = ROWS == 128 ? quad * 32 + lane : quad * 16 + (lane & 15);
-    const uint32_t tlane = tmem_base + ((uint32_t)(quad * 32) << 16);
-    const uint32_t prow = smem_u32(smem + OFF_P) + r * 128;
-    uint32_t ns = 0;
-    int ni = 0;
-    for (int item = blockIdx.x; item < p.n_items; item += gridDim.x, ++ni) {
-      float m_used = 0.f, l = 0.f;
-      for (int kt = 0; kt < NTILES; ++kt, ++ns) {
-        const int b = ns & 1;
-        mbar_wait(&s_full[b], (ns >> 1) & 1, 30);
-        tc_fence_after();
-        float s[XT];
-#pragma unroll
-        for (int c = 0; c < XT / 32; ++c) {
-          uint32_t v[32];
-          tmem_ld32(tlane + TM_S + b * XT + 32 * c, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) s[c * 32 + j] = __uint_as_float(v[j]) * 1.4426950408889634f;
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&s_empty[b]);
-        float mt = s[0];
-#pragma unroll
-        for (int j = 1; j < XT; ++j) mt = fmaxf(mt, s[j]);
-        // the previous P.X has completed: P may be overwritten and U is quiescent
-        mbar_wait(p_empty, (ns & 1) ^ 1, 31);
-        tc_fence_after();
-        if (kt == 0) {
-          m_used = mt;
-        } else {
-          const bool need = active && mt > m_used + RESCALE_T;
-          if (__any_sync(0xffffffffu, need)) {  // lazy rescale of this warp's rows of U (warp-uniform: tcgen05.ld/st are collective)
-            const float f = need ? ex2f(m_used - mt) : 1.0f;
-#pragma unroll 1
-            for (int c = 0; c < 8; ++c) {
-              uint32_t v[32];
-              tmem_ld32(tlane + TM_U + 32 * c, v);
-              tmem_ld_wait();
-#pragma unroll
-              for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) * f);
-              tmem_st32(tlane + TM_U + 32 * c, v);
-            }
-            tmem_st_wait();
-            l *= f;
-            if (need) m_used = mt;
-          }
-        }
-        float ls[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-        for (int j = 0; j < XT; ++j) { s[j] = ex2f(s[j] - m_used); ls[j & 3] += s[j]; }
-        l += (ls[0] + ls[1]) + (ls[2] + ls[3]);
-        if (active) {
-#pragma unroll
-          for (int c = 0; c < 8; ++c)
-            st_shared_v4(prow + ((c ^ (r & 7)) << 4), make_uint4(pack_bf16(s[8 * c], s[8 * c + 1]), pack_bf16(s[8 * c + 2], s[8 * c + 3]),
-                                                                 pack_bf16(s[8 * c + 4], s[8 * c + 5]), pack_bf16(s[8 * c + 6], s[8 * c + 7])));
-        }
-        fence_proxy_async_smem();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(p_full);
-      }
-      // ---- item epilogue: U / l -> global
-      mbar_wait(u_full, ni & 1, 32);
-      tc_fence_after();
-      const float inv = 1.0f / l;
-      float* dst = p.out + ((size_t)item * ROWS + r) * 256;
-#pragma unroll 1
-      for (int c = 0; c < 8; ++c) {
-        uint32_t v[32];
-        tmem_ld32(tlane + TM_U + 32 * c, v);
-        tmem_ld_wait();
-        if (active) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            *reinterpret_cast<float4*>(dst + 32 * c + j) = make_float4(__uint_as_float(v[j]) * inv, __uint_as_float(v[j + 1]) * inv,
-                                                                       __uint_as_float(v[j + 2]) * inv, __uint_as_float(v[j + 3]) * inv);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(u_empty);
-    }
+    return;
   }
+  if constexpr (NWG == 2) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
+  // ------------------------------------------------------------ warpgroup g: rows [64 g, 64 g + 64) of the item.
+  // Fragment element i of a thread: row 64 g + 16 wq + qr + 8 ((i >> 1) & 1), column 8 (i >> 2) + qc + (i & 1).
+  const int g = warp >> 2, wq = warp & 3, qr = lane >> 2, qc = 2 * (lane & 3);
+  const uint32_t aQ = smem_u32(smem + OFF_Q) + (uint32_t)g * 8192u;
+  int stage = 0, slot = 0, ni = 0;
+  uint32_t phase = 0, pephase = 0;
+  for (int item = blockIdx.x; item < p.n_items; item += gridDim.x, ++ni) {
+    mbar_wait(q_full, ni & 1, 26);
+    float u[128];
+#pragma unroll
+    for (int i = 0; i < 128; ++i) u[i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+#pragma unroll 1
+    for (int kt = 0; kt < NTILES; ++kt) {
+      const uint32_t xb = smem_u32(smem + stage * XSTAGE_BYTES);
+      float s[32];
+      int slots[4];
+      // every operand of the S chain has landed before the first wgmma: no spin loop between the MMAs of one group
+      if constexpr (MODE) mbar_wait(&xfull[stage], phase, 28);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        mbar_wait(&pefull[slot], pephase, 29);
+        slots[j] = slot;
+        if (++slot == PESLOTS) { slot = 0; pephase ^= 1; }
+      }
+      wg_fence();
+      if constexpr (MODE) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            wgmma<64>(s, make_desc_sw128(aQ + j * QSUB + k * 32, 0, 1024), make_desc_sw128(xb + j * SUBX + k * 32, 0, 1024), (j | k) != 0);
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const uint32_t pb = smem_u32(smem + OFF_PE + slots[j] * SUBX);
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma<64>(s, make_desc_sw128(aQ + j * QSUB + k * 32, 0, 1024), make_desc_sw128(pb + k * 32, 0, 1024), (MODE | j | k) != 0);
+      }
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc(s);
+      __syncwarp();
+      if (lane == 0) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) mbar_arrive(&peempty[slots[j]]);
+        if (kt == NTILES - 1) mbar_arrive(q_empty);   // every read of Q' by this item has completed
+      }
+      // online softmax (log2 units)
+      uint32_t pk[16];
+#pragma unroll
+      for (int rs = 0; rs < 2; ++rs) {
+        float mt = -INFINITY;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          s[4 * j + 2 * rs] *= 1.4426950408889634f;
+          s[4 * j + 2 * rs + 1] *= 1.4426950408889634f;
+          mt = fmaxf(mt, fmaxf(s[4 * j + 2 * rs], s[4 * j + 2 * rs + 1]));
+        }
+        mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 1));
+        mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 2));
+        const float m_new = fmaxf(m_run[rs], mt);
+        const float f = ex2f(m_run[rs] - m_new);
+        m_run[rs] = m_new;
+        float ls = 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float p0 = ex2f(s[4 * j + 2 * rs] - m_new), p1 = ex2f(s[4 * j + 2 * rs + 1] - m_new);
+          ls += p0 + p1;
+          pk[2 * j + rs] = pack_bf16(p0, p1);
+        }
+        l_run[rs] = l_run[rs] * f + ls;
+#pragma unroll
+        for (int j = 0; j < 32; ++j) { u[4 * j + 2 * rs] *= f; u[4 * j + 2 * rs + 1] *= f; }
+      }
+      // U += P X (X consumed MN-major: 16 tokens = 2048 B; next 64 channels = 8 KB)
+      if constexpr (!MODE) mbar_wait(&xfull[stage], phase, 24);
+      wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < XT / 16; ++kk) {
+        const uint32_t a[4] = {pk[4 * kk], pk[4 * kk + 1], pk[4 * kk + 2], pk[4 * kk + 3]};
+        wgmma_rs<256, 1>(u, a, make_desc_sw128(xb + kk * 2048, SUBX, 1024), 1);
+      }
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc(u);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&xempty[stage]);
+      if (++stage == XSTAGES) { stage = 0; phase ^= 1; }
+    }
+    // ---- item epilogue: U / l -> global
+#pragma unroll
+    for (int rs = 0; rs < 2; ++rs) {
+      float l = l_run[rs];
+      l += __shfl_xor_sync(0xffffffffu, l, 1);
+      l += __shfl_xor_sync(0xffffffffu, l, 2);
+      const float inv = 1.0f / l;
+      float* dst = p.out + ((size_t)item * ROWS + 64 * g + 16 * wq + qr + 8 * rs) * 256;
+#pragma unroll
+      for (int j = 0; j < 32; ++j)
+        *reinterpret_cast<float2*>(dst + 8 * j + qc) = make_float2(u[4 * j + 2 * rs] * inv, u[4 * j + 2 * rs + 1] * inv);
+    }
   }
 }
 
-template <int ROWS>
+template <int ROWS, int MODE>
 static int launch_t2i_fused_t(const T2iFusedArgs& a, int num_sms, cudaStream_t stream) {
   using namespace t2i;
   using C = Cfg<ROWS>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(t2i_fused_kernel<ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(t2i_fused_kernel<ROWS, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
     if (e != cudaSuccess) return set_error("t2i_fused: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
     attr_set = true;
   }
@@ -337,11 +248,11 @@ static int launch_t2i_fused_t(const T2iFusedArgs& a, int num_sms, cudaStream_t s
   if (make_tmap_bf16_2d(&tmXS, a.xs, 4096, 256, 256, XT)) return -1;
   if (make_tmap_bf16_2d(&tmQ, a.qp, (uint64_t)a.n_items * ROWS, 256, 256, ROWS)) return -1;
   T2iParams p;
-  p.n_items = a.n_items; p.mode = a.mode; p.out = a.out;
+  p.n_items = a.n_items; p.out = a.out;
   const int grid = a.n_items < num_sms ? a.n_items : num_sms;
   prof_begin(stream, ROWS == 64 ? "t2i_fused<64>" : "t2i_fused<128>", (double)a.n_items * 4096 * ROWS * 256 * 2.0 * 3,
              (double)a.n_items * (ROWS * 256.0 * 2 + ROWS * 256.0 * 4) + (a.mode ? (double)a.n_items * 4096 * 512 : 0.0));
-  t2i_fused_kernel<ROWS><<<grid, THREADS, C::SMEM_BYTES, stream>>>(tmX, tmXS, tmQ, p);
+  t2i_fused_kernel<ROWS, MODE><<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(tmX, tmXS, tmQ, p);
   prof_end(stream);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error("t2i_fused launch failed: %s", cudaGetErrorString(e));
@@ -351,8 +262,8 @@ static int launch_t2i_fused_t(const T2iFusedArgs& a, int num_sms, cudaStream_t s
 
 int launch_t2i_fused(const T2iFusedArgs& a, int num_sms, cudaStream_t stream) {
   if (a.n_items <= 0) return set_error("t2i_fused: empty problem");
-  if (a.rows == 64) return launch_t2i_fused_t<64>(a, num_sms, stream);
-  if (a.rows == 128) return launch_t2i_fused_t<128>(a, num_sms, stream);
+  if (a.rows == 64) return a.mode ? launch_t2i_fused_t<64, 1>(a, num_sms, stream) : launch_t2i_fused_t<64, 0>(a, num_sms, stream);
+  if (a.rows == 128) return a.mode ? launch_t2i_fused_t<128, 1>(a, num_sms, stream) : launch_t2i_fused_t<128, 0>(a, num_sms, stream);
   return set_error("t2i_fused: rows per item must be 64 or 128 (%d)", a.rows);
 }
 

@@ -1,10 +1,10 @@
-// MobileSAM's TinyViT image encoder (`vit_t`, micro_sam/util.py:35-43,436-441) on sm_100a.  Restated in oracle/tinyvit_ref.py.
+// MobileSAM's TinyViT image encoder (`vit_t`, micro_sam/util.py:35-43,436-441) on sm_90a.  Restated in oracle/tinyvit_ref.py.
 //   stem        conv3x3/2 (3->32) + BN + GELU  [direct kernel, fused Sam.preprocess]  ->  conv3x3/2 (32->64) + BN  [im2col + GEMM]
 //   stage 0     2 x MBConv @256^2 (1x1 64->256 GELU | dw3x3 GELU | 1x1 256->64 + shortcut, GELU)  ->  PatchMerging 64->128 /2
 //   stage 1-3   TinyViTBlock: window attention (7 / 14 / 7, head_dim 32, learned bias table) + dw3x3 local conv + MLP,
 //               PatchMerging 128->160 /2, 160->320 /1
 //   neck        conv1x1 -> LN2d -> conv3x3 -> LN2d (shared with the ViT path)
-// Everything 1x1 / dense is the tcgen05 GEMM of gemm.cu with BatchNorm folded into weight + bias at load time; the
+// Everything 1x1 / dense is the wgmma GEMM of gemm.cu with BatchNorm folded into weight + bias at load time; the
 // depth-wise convolutions, the window LayerNorm (zero pad tokens BEFORE the norm -> pad rows = LN bias) and the small-window
 // attention are HBM-bound CUDA-core kernels.  Activations: bf16 NHWC in the conv stage, fp32 token-major residual stream after.
 #include "engine.h"

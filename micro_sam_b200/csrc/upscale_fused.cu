@@ -8,21 +8,23 @@
 //
 // so neither the 64-channel up-scaled embedding (2 MB per prompt written + read by the two-kernel version) nor the
 // 32-channel one ever leaves the SM: per prompt the kernel reads 2 MB of `keys` and writes 0.25 MB per mask.
-// The element-wise epilogues -- 3.2 G GELUs per 32x32-grid tile, what bounded the previous kernels at 62 % issue-slot
-// utilisation with the tensor pipe 5 % active (profiles/r1_ncu_hyper_final.txt) -- run in PACKED fp16x2 arithmetic:
+// The element-wise epilogues -- 3.2 G GELUs per 32x32-grid tile, instruction-issue bound in fp32 -- run in PACKED fp16x2
+// arithmetic:
 //   GELU(x) = 0.5 x (1 + erf(x / sqrt 2)),  erf(x / sqrt 2) ~ tanh(x (a + b x^2))   (minimax a, b: |err| <= 2.7e-4; with the
 //   fp16 rounding of the 6-instruction chain the N(0,1)-weighted rms error is 2.9e-4 -- a quarter of the bf16 rounding the
 //   two-kernel version applied when it stored the intermediate), one MUFU (tanh.approx.f16x2) per TWO elements,
 // the intermediate operand A2 and the conv-transpose-2 weights are fp16 (11-bit mantissa instead of bf16's 8), the hyper
 // product accumulates 2 x 8 fp16x2 FMAs per mask and finishes in fp32.
 //
-// CTA = TMA warp + MMA warp + 16 epilogue warps (4 TMEM lane quadrants x 4 column groups), persistent over a contiguous
-// range of (prompt, 128-token tile) items; TMEM: D1 = columns [0,256), D2 = 2 x 128 columns (double buffered over s).
+// CTA = 4 warpgroups (warpgroup s: sub-pixel s = D1 columns [64 s, 64 s + 64), its A2_s tile and D2_s; wgmma accumulators in
+// registers, epilogues straight from the fragments with row reductions across the quad of lanes that shares a row) + 1 TMA
+// warp, persistent over a contiguous range of (prompt, 128-token tile) items.
 #include <cuda_fp16.h>
 
 #include "kernels.h"
 #include "ptx.cuh"
 #include "tensormap.h"
+#include "wgmma.cuh"
 
 namespace msam {
 
@@ -35,8 +37,7 @@ constexpr int OFF_A2 = STAGES * STAGE_BYTES;    // 4 x [128 x 64] fp16
 constexpr int OFF_W2 = OFF_A2 + 4 * SUBA;       // [128 x 64] fp16
 constexpr int OFF_BAR = OFF_W2 + SUBA;
 constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
-constexpr int THREADS = 128 + 512;
-constexpr uint32_t TM_D1 = 0, TM_D2 = 256, TMEM_COLS = 512;
+constexpr int THREADS = 512 + 32;
 constexpr int TILES = 32;                       // 4096 image tokens / 128
 }  // namespace up
 
@@ -50,10 +51,6 @@ struct UpParams {
   const float* hyper;   // [P, 4, 32]
   float* out;           // [P, nm, 256, 256]
 };
-
-__host__ __device__ constexpr uint32_t make_idesc_f16(uint32_t M, uint32_t N) {  // kind::f16, A = B = F16 (format 0), D = F32
-  return (1u << 4) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
 
 __device__ __forceinline__ __half2 tanh_h2(__half2 x) {
   uint32_t r, a = *reinterpret_cast<uint32_t*>(&x);
@@ -79,44 +76,30 @@ upscale_fused_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* w2_full = empty_bar + STAGES;
-  uint64_t* d1_full = w2_full + 1;
-  uint64_t* d1_empty = d1_full + 1;
-  uint64_t* a2_full = d1_empty + 1;    // [4]
-  uint64_t* a2_empty = a2_full + 4;    // [4]
-  uint64_t* d2_full = a2_empty + 4;    // [2]
-  uint64_t* d2_empty = d2_full + 2;    // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(d2_empty + 2);
   __shared__ __align__(16) float b1_s[256];
   __shared__ __align__(16) __half2 gb_s[64];          // [0,32) gamma pairs, [32,64) beta pairs
   __shared__ __align__(16) __half2 b2_s[64];          // conv-transpose-2 bias pairs, index ss*16 + i
-  __shared__ __align__(16) __half2 hyp_s[16 * 2 * 64];  // per epilogue warp and item parity: [mask < 4][16 channel pairs]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long total = (long)p.P * TILES;
   const int it_begin = (int)(total * blockIdx.x / gridDim.x), it_end = (int)(total * (blockIdx.x + 1) / gridDim.x);
   const int n_items = it_end - it_begin;
 
-  if (warp == 0 && lane == 0) { prefetch_tmap(&tmX); prefetch_tmap(&tmW1); prefetch_tmap(&tmW2); }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    mbar_init(w2_full, 1); mbar_init(d1_full, 1); mbar_init(d1_empty, 16);
-    for (int i = 0; i < 4; ++i) { mbar_init(&a2_full[i], 4); mbar_init(&a2_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&d2_full[i], 1); mbar_init(&d2_empty[i], 16); }
+  if (warp == 16 && lane == 0) {
+    prefetch_tmap(&tmX); prefetch_tmap(&tmW1); prefetch_tmap(&tmW2);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 16); }
+    mbar_init(w2_full, 1);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, TMEM_COLS);
   for (int i = threadIdx.x; i < 256; i += THREADS) b1_s[i] = p.b1[i];
   for (int i = threadIdx.x; i < 32; i += THREADS) {
     gb_s[i] = __floats2half2_rn(p.gamma[2 * i], p.gamma[2 * i + 1]);
     gb_s[32 + i] = __floats2half2_rn(p.beta[2 * i], p.beta[2 * i + 1]);
   }
   for (int i = threadIdx.x; i < 64; i += THREADS) b2_s[i] = __floats2half2_rn(p.b2[2 * i], p.b2[2 * i + 1]);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 16) {
     // ------------------------------------------------------------ TMA producer
     if (lane == 0 && n_items > 0) {
       mbar_expect_tx(w2_full, SUBA);
@@ -140,156 +123,125 @@ upscale_fused_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_const
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer (warp-uniform control flow, elected lane issues)
-    constexpr uint32_t idesc1 = make_idesc_bf16(128, 256);
-    constexpr uint32_t idesc2 = make_idesc_f16(128, 128);
-    const uint64_t dw2 = make_desc_sw128(smem_u32(smem + OFF_W2), 0, 1024);
-    int stage = 0;
-    uint32_t phase = 0;
-    auto mma1 = [&](int it) {
-      if (it > 0) mbar_wait(d1_empty, (it - 1) & 1, 41);  // every epilogue warp has pulled the previous D1 out of TMEM
-      for (int j = 0; j < 4; ++j) {
-        mbar_wait(&full_bar[stage], phase, 42);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-        const uint64_t da = make_desc_sw128(sa, 0, 1024), db = make_desc_sw128(sa + SUBA, 0, 1024);
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_bf16(tmem_base + TM_D1, da + 2 * k, db + 2 * k, idesc1, (j | k) != 0);
-          umma_commit(&empty_bar[stage]);
-          if (j == 3) umma_commit(d1_full);
-        }
-        __syncwarp();
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-    };
-    auto mma2 = [&](int it, int s) {
-      const int b = s & 1;
-      const uint32_t n = 2u * it + (s >> 1);  // use counter of D2 buffer b
-      mbar_wait(&a2_full[s], it & 1, 43);
-      if (n > 0) mbar_wait(&d2_empty[b], (n - 1) & 1, 44);
-      tc_fence_after();
-      const uint64_t da = make_desc_sw128(smem_u32(smem + OFF_A2 + s * SUBA), 0, 1024);
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) umma_bf16(tmem_base + TM_D2 + b * 128, da + 2 * k, dw2 + 2 * k, idesc2, k != 0);
-        umma_commit(&d2_full[b]);
-        umma_commit(&a2_empty[s]);
-      }
-      __syncwarp();
-    };
-    if (n_items > 0) {
-      mbar_wait(w2_full, 0, 45);
-      mma1(0);
-      for (int it = 0; it < n_items; ++it) {
-        mma2(it, 0);
-        mma2(it, 1);
-        if (it + 1 < n_items) mma1(it + 1);  // overlaps E2 of this item
-        mma2(it, 2);
-        mma2(it, 3);
-      }
-    }
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------ epilogue warps
-    const int ew = warp - 4, quad = warp & 3, grp = ew >> 2, r = quad * 32 + lane;
-    const uint32_t tlane = tmem_base + ((uint32_t)(quad * 32) << 16);
-    const uint32_t a2row = smem_u32(smem + OFF_A2 + grp * SUBA) + r * 128;
-    const float inv64 = 1.0f / 64.0f;
-    for (int it = 0; it < n_items; ++it) {
-      const int item = it_begin + it, pp = item / TILES, rt = item % TILES;
-      // hyper-network vectors of this prompt -> private fp16x2 copy (read back as shared-memory broadcasts in E2)
-      __half2* hw = hyp_s + (ew * 2 + (it & 1)) * 64;
-      for (int i = lane; i < p.nm * 16; i += 32) {
-        const float2 v = __ldg(reinterpret_cast<const float2*>(p.hyper + ((size_t)pp * 4 + p.m0) * 32) + i);
-        hw[i] = __floats2half2_rn(v.x, v.y);
-      }
-      __syncwarp();
-
-      // ---- E1: (row r, sub-pixel grp): + bias, LayerNorm over 64 channels, GELU -> A2[grp] row r (fp16, K-major SW128)
-      mbar_wait(d1_full, it & 1, 46);
-      tc_fence_after();
-      float s4[4] = {0.f, 0.f, 0.f, 0.f}, q4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t v[32];
-        tmem_ld32(tlane + TM_D1 + 64 * grp + 32 * c, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const float x = __uint_as_float(v[j]) + b1_s[64 * grp + 32 * c + j];
-          s4[j & 3] += x;
-          q4[j & 3] = fmaf(x, x, q4[j & 3]);
-        }
-      }
-      const float sum = (s4[0] + s4[1]) + (s4[2] + s4[3]);
-      const float mean = sum * inv64;
-      const float var = fmaxf(((q4[0] + q4[1]) + (q4[2] + q4[3])) * inv64 - mean * mean, 0.f);
-      const float rstd = rsqrtf(var + p.eps);
-      const float shift = -mean * rstd;
-      if (it > 0) mbar_wait(&a2_empty[grp], (it - 1) & 1, 47);  // MMA2 of the previous item has read A2[grp]
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t v[32];
-        tmem_ld32(tlane + TM_D1 + 64 * grp + 32 * c, v);
-        tmem_ld_wait();
-        uint32_t o[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float x0 = __uint_as_float(v[2 * i]) + b1_s[64 * grp + 32 * c + 2 * i];
-          const float x1 = __uint_as_float(v[2 * i + 1]) + b1_s[64 * grp + 32 * c + 2 * i + 1];
-          const __half2 n2 = __floats2half2_rn(fmaf(x0, rstd, shift), fmaf(x1, rstd, shift));
-          o[i] = h2u(gelu_h2(__hfma2(n2, gb_s[16 * c + i], gb_s[32 + 16 * c + i])));
-        }
-#pragma unroll
-        for (int q = 0; q < 4; ++q)
-          st_shared_v4(a2row + (((4 * c + q) ^ (r & 7)) << 4), make_uint4(o[4 * q], o[4 * q + 1], o[4 * q + 2], o[4 * q + 3]));
-      }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) { mbar_arrive(&a2_full[grp]); mbar_arrive(d1_empty); }
-
-      // ---- E2: (row r, sub-pixel s, sub-sub-pixel grp): + bias, GELU, hyper product over the 32 channels -> low-res logits
-      const int tok = rt * 128 + r, ty = tok >> 6, tx = tok & 63;
-      float* obase = p.out + (size_t)pp * p.nm * 65536 + (size_t)(4 * ty + (grp >> 1)) * 256 + 4 * tx + (grp & 1);
-#pragma unroll 1
-      for (int s = 0; s < 4; ++s) {
-        const int b = s & 1;
-        const uint32_t n = 2u * it + (s >> 1);
-        mbar_wait(&d2_full[b], n & 1, 48);
-        tc_fence_after();
-        uint32_t v[32];
-        tmem_ld32(tlane + TM_D2 + b * 128 + 32 * grp, v);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&d2_empty[b]);
-        __half2 g[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i)
-          g[i] = gelu_h2(__hadd2(__floats2half2_rn(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1])), b2_s[grp * 16 + i]));
-        float* o = obase + (size_t)(2 * (s >> 1)) * 256 + 2 * (s & 1);
-        for (int mi = 0; mi < p.nm; ++mi) {
-          const __half2* hm = hw + mi * 16;
-          __half2 a0 = __floats2half2_rn(0.f, 0.f), a1 = a0;
-#pragma unroll
-          for (int i = 0; i < 16; i += 2) {
-            a0 = __hfma2(g[i], hm[i], a0);
-            a1 = __hfma2(g[i + 1], hm[i + 1], a1);
-          }
-          const float2 f0 = __half22float2(a0), f1 = __half22float2(a1);
-          o[(size_t)mi * 65536] = (f0.x + f0.y) + (f1.x + f1.y);
-        }
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
+  // ------------------------------------------------------------ warpgroup s = sub-pixel s.  Fragment element i of a thread:
+  // row 64 h + 16 wq + qr + 8 ((i >> 1) & 1) of the 64-row half h, column 8 (i >> 2) + qc + (i & 1).
+  const int sp = warp >> 2, wq = warp & 3, qr = lane >> 2, qc = 2 * (lane & 3);
+  const uint32_t a2 = smem_u32(smem + OFF_A2 + sp * SUBA), aw2 = smem_u32(smem + OFF_W2);
+  const float inv64 = 1.0f / 64.0f;
+  int stage = 0;
+  uint32_t phase = 0;
+  if (n_items > 0) mbar_wait(w2_full, 0, 45);
+  for (int it = 0; it < n_items; ++it) {
+    const int item = it_begin + it, pp = item / TILES, rt = item % TILES;
+    // ---- MMA1: D1[:, 64 sp .. 64 sp + 64) = keys tile . W1[64 sp .., :]^T
+    float d1[2][32];
+    for (int j = 0; j < 4; ++j) {
+      mbar_wait(&full_bar[stage], phase, 42);
+      const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
+      const uint64_t db = make_desc_sw128(sa + SUBA + sp * 8192, 0, 1024);
+      wg_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) wgmma<64>(d1[h], make_desc_sw128(sa + h * 8192, 0, 1024) + 2 * k, db + 2 * k, (j | k) != 0);
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc(d1[0]);
+      wg_fence_acc(d1[1]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    // ---- E1: (row, sub-pixel sp): + bias, LayerNorm over 64 channels, GELU -> A2_sp (fp16, K-major SW128)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int rs = 0; rs < 2; ++rs) {
+        const int r = 64 * h + 16 * wq + qr + 8 * rs;
+        float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float& x = d1[h][4 * j + 2 * rs + e];
+            x += b1_s[64 * sp + 8 * j + qc + e];
+            s1 += x;
+            s2 = fmaf(x, x, s2);
+          }
+        }
+        s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
+        s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
+        s2 += __shfl_xor_sync(0xffffffffu, s2, 1);
+        s2 += __shfl_xor_sync(0xffffffffu, s2, 2);
+        const float mean = s1 * inv64;
+        const float var = fmaxf(s2 * inv64 - mean * mean, 0.f);
+        const float rstd = rsqrtf(var + p.eps);
+        const float shift = -mean * rstd;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int c = 8 * j + qc;
+          const __half2 n2 = __floats2half2_rn(fmaf(d1[h][4 * j + 2 * rs], rstd, shift), fmaf(d1[h][4 * j + 2 * rs + 1], rstd, shift));
+          const uint32_t v = h2u(gelu_h2(__hfma2(n2, gb_s[c >> 1], gb_s[32 + (c >> 1)])));
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(a2 + (uint32_t)r * 128u + ((uint32_t)((c >> 3) ^ (r & 7)) << 4) + (uint32_t)(c & 7) * 2u),
+                       "r"(v) : "memory");
+        }
+      }
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(1 + sp, 128);   // the whole A2_sp tile is written before this warpgroup's MMA2 reads it
+    // ---- MMA2 + E2 per half of the conv-transpose-2 outputs (sub-sub-pixels ss = 2 hf, 2 hf + 1 = W2 rows [64 hf, +64)):
+    // + bias, GELU, hyper product over the 32 channels -> low-res logits
+    const int tok0 = rt * 128;
+#pragma unroll 1
+    for (int hf = 0; hf < 2; ++hf) {
+      float d2[2][32];
+      wg_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          wgmma<64, 0, 0, true>(d2[h], make_desc_sw128(a2 + h * 8192 + 32 * k, 0, 1024), make_desc_sw128(aw2 + hf * 8192 + 32 * k, 0, 1024), k != 0);
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc(d2[0]);
+      wg_fence_acc(d2[1]);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int rs = 0; rs < 2; ++rs) {
+          const int tok = tok0 + 64 * h + 16 * wq + qr + 8 * rs, ty = tok >> 6, tx = tok & 63;
+#pragma unroll
+          for (int sl = 0; sl < 2; ++sl) {
+            const int ss = 2 * hf + sl;
+            // this thread: channel pairs i = 4 jj + qc / 2 (jj < 4) of columns 32 sl + 8 jj + qc
+            __half2 gv[4];
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const int j = 4 * sl + jj, i = 4 * jj + (qc >> 1);
+              gv[jj] = gelu_h2(__hadd2(__floats2half2_rn(d2[h][4 * j + 2 * rs], d2[h][4 * j + 2 * rs + 1]), b2_s[ss * 16 + i]));
+            }
+            float* o = p.out + (size_t)pp * p.nm * 65536 + (size_t)(4 * ty + 2 * (sp >> 1) + (ss >> 1)) * 256 + 4 * tx + 2 * (sp & 1) + (ss & 1);
+            for (int mi = 0; mi < p.nm; ++mi) {
+              const float2* hv = reinterpret_cast<const float2*>(p.hyper + ((size_t)pp * 4 + p.m0 + mi) * 32);
+              __half2 acc = __floats2half2_rn(0.f, 0.f);
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj) {
+                const float2 w = __ldg(hv + 4 * jj + (qc >> 1));
+                acc = __hfma2(gv[jj], __floats2half2_rn(w.x, w.y), acc);
+              }
+              const float2 f = __half22float2(acc);
+              float v = f.x + f.y;
+              v += __shfl_xor_sync(0xffffffffu, v, 1);
+              v += __shfl_xor_sync(0xffffffffu, v, 2);
+              if ((lane & 3) == 0) o[(size_t)mi * 65536] = v;
+            }
+          }
+        }
+      }
+    }
   }
 }
 

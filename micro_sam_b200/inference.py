@@ -1,4 +1,4 @@
-"""micro_sam.inference.batched_inference (inference.py:155-286) on the B200 core.
+"""micro_sam.inference.batched_inference (inference.py:155-286) on the H100 core.
 
 `batched_tiled_inference` / `_stitch_segmentation` (inference.py:315-538) route prompts to tiles and call it per tile.
 

@@ -173,7 +173,27 @@ class AMGBase(ABC):
         return {"crop_list": self.crop_list, "crop_boxes": self.crop_boxes, "original_size": self.original_size}
 
     def set_state(self, state: Dict[str, Any]) -> None:
-        self._crop_list = state["crop_list"]
+        """A cached state (precompute_state.cache_amg_state) holds CPU tensors: what the kernels read goes back to the
+        predictor's device (`points` stay on the host, as `initialize` keeps them), except the low-res logits when they would
+        take more than half of the free device memory (then they stay in pinned host memory, the offloaded layout of
+        `initialize(offload_state=None)`)."""
+        dev = self._predictor.device
+        crops = state["crop_list"]
+        need = sum(d["low_res"].numel() * d["low_res"].element_size() for d in crops
+                   if "low_res" in d and torch.is_tensor(d["low_res"]))
+        offload = need > 0 and need > 0.5 * torch.cuda.mem_get_info(dev)[0]
+
+        def place(k, v):
+            if not torch.is_tensor(v) or k not in ("low_res", "iou_preds", "stability_score", "boxes", "area", "stats_done"):
+                return v
+            if k == "low_res" and offload:
+                return v if v.is_pinned() else v.cpu().pin_memory()
+            return v.to(dev)
+        self._crop_list = []
+        for d in crops:
+            data = amg_utils.MaskData()
+            data._stats.update({k: place(k, v) for k, v in d.items()})
+            self._crop_list.append(data)
         self._crop_boxes = state["crop_boxes"]
         self._original_size = state["original_size"]
         self._is_initialized = True
@@ -621,5 +641,5 @@ def get_instance_segmentation_generator(predictor, is_tiled: bool, decoder=None,
                                         **kwargs):
     """instance_segmentation.py:1631: only the AMG mode exists on this path (AIS/APG need the UNETR decoder, 8f-2)."""
     if decoder is not None or segmentation_mode not in (None, "amg"):
-        raise NotImplementedError("only segmentation_mode='amg' is available on the B200 path")
+        raise NotImplementedError("only segmentation_mode='amg' is available on the GPU path")
     return (TiledAutomaticMaskGenerator if is_tiled else AutomaticMaskGenerator)(predictor, **kwargs)

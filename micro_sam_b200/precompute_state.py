@@ -1,4 +1,4 @@
-"""micro_sam.precompute_state on the B200 core (micro_sam/precompute_state.py:27-279): precompute the image embeddings of a file /
+"""micro_sam.precompute_state on the H100 core (micro_sam/precompute_state.py:27-279): precompute the image embeddings of a file /
 folder into the reference's zarr layout and, optionally, the state of the automatic mask generator next to them
 (`<embeddings>.zarr/amg_state.pickle`, or `amg_state/state-<i>.pkl` per slice), so that a later session -- the annotator, a batch
 script -- loads instead of recomputing.  Same function names, arguments and file names as the reference.
@@ -85,7 +85,7 @@ def cache_amg_state(predictor, raw: np.ndarray, image_embeddings: util.ImageEmbe
 
 def cache_is_state(*args, **kwargs):
     """precompute_state.py:90-155 (AIS: UNETR decoder outputs)."""
-    raise NotImplementedError("the AIS decoder is not part of the B200 path (SURVEY.md 8f-2)")
+    raise NotImplementedError("the AIS decoder is not part of the GPU path (SURVEY.md 8f-2)")
 
 
 def _precompute_state_for_file(predictor, input_path, output_path, key, ndim, tile_shape, halo, precompute_amg_state, decoder, verbose):
@@ -121,12 +121,12 @@ def precompute_state(input_path: Union[os.PathLike, str], output_path: Union[os.
                      model_type: str = "vit_b", checkpoint_path: Optional[Union[os.PathLike, str]] = None, key: Optional[str] = None,
                      ndim: Optional[int] = None, tile_shape: Optional[Tuple[int, int]] = None, halo: Optional[Tuple[int, int]] = None,
                      precompute_amg_state: bool = False, predictor=None) -> None:
-    """precompute_state.py:224-279.  `predictor=` passes an already built B200 predictor (no download here: without it
+    """precompute_state.py:224-279.  `predictor=` passes an already built GPU predictor (no download here: without it
     `checkpoint_path` is required)."""
     if predictor is None:
         predictor, state = util.get_sam_model(model_type=model_type, checkpoint_path=checkpoint_path, return_state=True)
         if state is not None and "decoder_state" in state:
-            raise NotImplementedError("checkpoints with an AIS decoder: only the AMG state can be precomputed on the B200 path")
+            raise NotImplementedError("checkpoints with an AIS decoder: only the AMG state can be precomputed on the GPU path")
     if pattern is None:
         _precompute_state_for_file(predictor, input_path, output_path, key, ndim=ndim, tile_shape=tile_shape, halo=halo,
                                    precompute_amg_state=precompute_amg_state, decoder=None, verbose=True)

@@ -1,4 +1,4 @@
-"""Interactive (prompt-based) segmentation on the B200 predictor: `segment_from_points / _box / _box_and_points / _mask`
+"""Interactive (prompt-based) segmentation on the GPU predictor: `segment_from_points / _box / _box_and_points / _mask`
 with the reference's signatures (micro_sam/prompt_based_segmentation.py:251-506), including the tiled-embedding routing
 (`_initialize_predictor`, :209-231) and the mask -> (box, points, logits) prompt derivation (:28-113).
 

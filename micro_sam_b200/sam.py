@@ -4,7 +4,7 @@ micro-sam never touches SAM internals except through the predictor object that `
 (reference: micro_sam/util.py:460-476; attribute census in SURVEY.md 8b).  `B200SamPredictor` offers exactly that
 surface -- `set_image`, `set_torch_image`, `predict`, `predict_torch`, `get_image_embedding`, `reset_image`, the mutable
 `features / original_size / input_size / is_image_set` attributes, `transform`, `device`, `model` -- while every FLOP
-runs in the hand-written sm_100a kernels.  There is no PyTorch fallback: without the library / a B200 it raises.
+runs in the hand-written sm_90a kernels.  There is no PyTorch fallback: without the library / an H100 it raises.
 """
 from __future__ import annotations
 
@@ -302,7 +302,7 @@ class B200Sam:
             raise ValueError(f"unsupported model type {model_type!r} (have {sorted(ARCH)})")
         dev = torch.device(device)
         if dev.type != "cuda":
-            raise RuntimeError(f"micro_sam_b200 runs on a CUDA (sm_100a) device only; got device={device!r}")
+            raise RuntimeError(f"micro_sam_b200 runs on a CUDA (sm_90a) device only; got device={device!r}")
         if not torch.cuda.is_available():
             raise RuntimeError("micro_sam_b200: no CUDA device available and there is no CPU fallback")
         self.model_type = model_type
@@ -356,7 +356,7 @@ class B200Sam:
         return missing, unexpected
 
     def named_parameters(self):
-        """Host copies of the weights under their upstream names (frozen: the B200 core is an inference engine; the training
+        """Host copies of the weights under their upstream names (frozen: the H100 core is an inference engine; the training
         surface of cfg 5 is documented in DESIGN.md)."""
         for k, v in self._state.items():
             yield k, torch.nn.Parameter(v, requires_grad=False)

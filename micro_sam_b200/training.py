@@ -1,4 +1,4 @@
-"""Forward half of micro-sam's fine-tuning step on the B200 core (cfg 5; micro_sam/training/trainable_sam.py:24-114,
+"""Forward half of micro-sam's fine-tuning step on the H100 core (cfg 5; micro_sam/training/trainable_sam.py:24-114,
 micro_sam/training/sam_trainer.py:122-172).
 
 `TrainableSAM` keeps the reference's protocol -- `preprocess` (torch resize with antialias, normalise, pad),

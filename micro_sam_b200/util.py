@@ -1,4 +1,4 @@
-"""micro_sam.util's hot-path functions with their reference signatures, on the B200 core.
+"""micro_sam.util's hot-path functions with their reference signatures, on the H100 core.
 
 Mirrors (reference file:line): get_sam_model util.py:318-476, _to_image :618-651, _compute_embeddings_batched
 :654-681, tiled / 3-D drivers :765-1041, precompute_image_embeddings :1133-1212, set_precomputed :1215-1258,
@@ -29,12 +29,12 @@ ImageEmbeddings = Dict[str, Any]
 
 # ------------------------------------------------------------------------------------------------ model loading
 def get_device(device: Optional[Union[str, torch.device]] = None) -> torch.device:
-    """util.py:204-246 restricted to what this core can run on: a CUDA (sm_100a) device."""
+    """util.py:204-246 restricted to what this core can run on: a CUDA (sm_90a) device."""
     if device is None or str(device) == "auto":
         device = "cuda"
     dev = torch.device(device)
     if dev.type != "cuda":
-        raise RuntimeError(f"micro_sam_b200 only runs on CUDA sm_100a devices, not {device!r} (no CPU fallback).")
+        raise RuntimeError(f"micro_sam_b200 only runs on CUDA sm_90a devices, not {device!r} (no CPU fallback).")
     if not torch.cuda.is_available():
         raise RuntimeError("PyTorch CUDA backend is not available.")
     return dev
@@ -81,7 +81,7 @@ def get_sam_model(model_type: str = "vit_b", device: Optional[Union[str, torch.d
     checkpoint layouts) or from an in-memory upstream-keyed `state_dict`.  There is no download (no network)."""
     for k in ("peft_kwargs", "decoder_path"):
         if unsupported.get(k) is not None:
-            raise NotImplementedError(f"get_sam_model({k}=...) is outside the B200 hot path (SURVEY.md 8f)")
+            raise NotImplementedError(f"get_sam_model({k}=...) is outside the GPU hot path (SURVEY.md 8f)")
     device = get_device(device)
     state = None
     if state_dict is None:
@@ -210,7 +210,7 @@ def _needs_no_resize(predictor, image) -> bool:
 
 def _host_pool() -> futures.ThreadPoolExecutor:
     """Host threads for the per-tile numpy / PIL work (min-max normalisation, ResizeLongestSide): both release the GIL, and
-    at B200 encoder speeds (a few ms per tile) a single Python thread would be the bottleneck (SURVEY.md 8a, a4)."""
+    at H100 encoder speeds (a few ms per tile) a single Python thread would be the bottleneck (SURVEY.md 8a, a4)."""
     global _POOL
     if _POOL is None:
         _POOL = futures.ThreadPoolExecutor(max(1, min(32, (os.cpu_count() or 2) - 1)))

@@ -508,7 +508,7 @@ def test_model_level_prompt_encoder_and_mask_decoder(models):
 
 def test_trainable_sam_forward_and_loss(models):
     """a21 / a22 (forward half of cfg 5): TrainableSAM.preprocess / image_embeddings_oft / forward and SamTrainer._compute_loss
-    on the B200 kernels against the oracle restatement (oracle/train_ref.py): floats within the usual tolerances; the loss
+    on the GPU kernels against the oracle restatement (oracle/train_ref.py): floats within the usual tolerances; the loss
     statistics kernel is additionally checked against the oracle loss evaluated on the GPU's OWN logits (tight tolerance)."""
     from oracle import train_ref
     from micro_sam_b200 import training
