@@ -6,15 +6,23 @@
 // Algebra (exact up to bf16 rounding of the small per-prompt operands):
 //   scores[r, (h,t)] = (x_r + pe_r) . Mq[(h,t)] + c[(h,t)],  Mq[(h,t)] = 0.25 * Wq_h^T k_tok[t,h]   ([64, 256] per prompt)
 //   attn_out . Wo^T  = P[r, (h,t)] . V'[(h,t)],              V'[(h,t)] = Wo_h v_tok[t,h]            ([64, 256] per prompt)
-// so per 128-row tile the tensor core runs  S = X Mq^T (+ PE Mq^T),  O = X I (residual, exact) + P V'  and the CUDA cores
-// only do the 8-head x T softmax and the LayerNorm.  Mq / V'^T come from two small plain GEMMs (decoder.cu).
+// so per 128-row tile the tensor core runs  S = X Mq^T (+ PE Mq^T)  and  O = X + P V'  (the residual X is read from the
+// ring stage into registers, in fragment order, while the score MMAs run; it seeds the O accumulator, bf16 -> fp32 exactly,
+// before P V' accumulates onto it) and the CUDA cores only do the 8-head x T softmax and the LayerNorm.  Mq / V'^T come
+// from two small plain GEMMs (decoder.cu).
 //
-// CTA = 2 warpgroups + 1 TMA warp (64 rows of the tile each: wgmma chains, softmax and LayerNorm straight from the
-// accumulator fragments, P fed back from registers); persistent over a contiguous range of (prompt, row-tile) items so
-// Mq / V' stay resident while the prompt does not change.
-//   ring (3 stages x 32 KB): [a0_j | a1_j], j = 64-column slice of the 256 channels
-//     mode 1 (per-prompt keys): a0 = keys tile, a1 = pe tile:       S += a0 Mq_j^T + a1 Mq_j^T ; O[:, 64j..] = a0 I
-//     mode 0 (layer 0, shared): a0 = (src+pe) tile, a1 = src tile: S += a0 Mq_j^T             ; O[:, 64j..] = a1 I
+// CTA = 2 consumer warpgroups (64 rows of the tile each: wgmma chains, softmax and LayerNorm straight from the
+// accumulator fragments, P fed back from registers) + 1 warpgroup of which warp 8 issues the TMA loads and warps 9 / 10 the
+// TMA stores of consumer warpgroup 0 / 1; persistent over a contiguous range of (prompt, row-tile) items so Mq / V' stay
+// resident while the prompt does not change.
+//   ring (3 stages x 32 KB; 3 stages + 2 staging tiles per warpgroup measured faster than 4 stages + 1):
+//     [a0_j | a1_j], j = 64-column slice
+//     mode 1 (per-prompt keys): a0 = keys tile, a1 = pe tile:       S += a0 Mq_j^T + a1 Mq_j^T ; O[:, 64j..] = a0
+//     mode 0 (layer 0, shared): a0 = (src+pe) tile, a1 = src tile: S += a0 Mq_j^T             ; O[:, 64j..] = a1
+//   output: each warpgroup writes its normalised rows slice by slice into two [64 x 64] SW128 staging tiles (full / empty
+//   mbarriers with its store warp), which stores them with TMA, so the stores leave as whole 128-B rows.
+// Mode 1 writes `keys` in place.  That is safe because every item reads (TMA-loads, and L2-prefetches) only its own 128
+// rows, all four slices of them before its epilogue stores, and no other item reads those rows.
 #include "kernels.h"
 #include "ptx.cuh"
 #include "tensormap.h"
@@ -28,12 +36,14 @@ constexpr int SUB = 128 * 128;                 // [128 rows x 64 bf16] SWIZZLE_1
 constexpr int STAGE_BYTES = 2 * SUB;
 constexpr int OFF_M = STAGES * STAGE_BYTES;    // Mq[p]: 4 K-slices of [64 x 64]
 constexpr int OFF_V = OFF_M + 32768;           // V'^T[p]: [256 x 64]
-constexpr int OFF_I = OFF_V + 32768;           // identity [64 x 64]
-constexpr int OFF_BAR = OFF_I + 8192;
+constexpr int OBUF = 2;                        // output staging buffers per warpgroup
+constexpr int OFF_O = OFF_V + 32768;           // output staging: 2 warpgroups x OBUF x [64 x 64] bf16 SW128
+constexpr int OFF_BAR = OFF_O + 2 * OBUF * 8192;
 constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
-constexpr int THREADS = 256 + 128;             // 2 warpgroups, then a warpgroup whose first warp issues the TMA loads
+constexpr int THREADS = 256 + 128;             // 2 warpgroups, then a warpgroup: warp 8 issues the TMA loads, 9 / 10 the stores
 constexpr int TILES = 32;                      // 4096 image tokens / 128 rows
 constexpr int PF_AHEAD = 2;                    // L2 prefetch distance in work items
+static_assert(SMEM_BYTES + 768 * 4 <= 227 * 1024, "ring + operands + staging + rowp exceed the shared memory of an SM");
 }  // namespace i2t
 
 struct I2tParams {
@@ -51,8 +61,8 @@ __device__ __forceinline__ float ex2_approx(float x) {
 
 __global__ void __launch_bounds__(i2t::THREADS, 1)
 i2t_fused_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
-                 const __grid_constant__ CUtensorMap tmM, const __grid_constant__ CUtensorMap tmV, const I2tParams p,
-                 __nv_bfloat16* __restrict__ out) {
+                 const __grid_constant__ CUtensorMap tmM, const __grid_constant__ CUtensorMap tmV,
+                 const __grid_constant__ CUtensorMap tmO, const I2tParams p) {
   using namespace i2t;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -60,6 +70,8 @@ i2t_fused_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* mv_full = empty_bar + STAGES;
   uint64_t* mv_empty = mv_full + 1;
+  uint64_t* ofull = mv_empty + 1;      // [g * OBUF + b]: staging tile b of warpgroup g written (4 warps arrive)
+  uint64_t* oempty = ofull + 2 * OBUF;  // [g * OBUF + b]: its TMA store has read it
   __shared__ __align__(16) float rowp[768];  // out-proj bias | gamma | beta
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -67,23 +79,13 @@ i2t_fused_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
   const int it_begin = (int)(total * blockIdx.x / gridDim.x), it_end = (int)(total * (blockIdx.x + 1) / gridDim.x);
 
   if (warp == 8 && lane == 0) {
-    prefetch_tmap(&tmA0); prefetch_tmap(&tmA1); prefetch_tmap(&tmM); prefetch_tmap(&tmV);
+    prefetch_tmap(&tmA0); prefetch_tmap(&tmA1); prefetch_tmap(&tmM); prefetch_tmap(&tmV); prefetch_tmap(&tmO);
     for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 8); }
     mbar_init(mv_full, 1); mbar_init(mv_empty, 8);
+    for (int i = 0; i < 2 * OBUF; ++i) { mbar_init(&ofull[i], 4); mbar_init(&oempty[i], 1); }
     fence_barrier_init();
   }
   for (int i = threadIdx.x; i < 256; i += THREADS) { rowp[i] = p.bias[i]; rowp[256 + i] = p.gamma[i]; rowp[512 + i] = p.beta[i]; }
-  for (int i = threadIdx.x; i < 64 * 8; i += THREADS) {  // identity, K-major SW128: row n, 16-byte chunk c
-    const int n = i >> 3, c = i & 7;
-    uint4 v = make_uint4(0, 0, 0, 0);
-    if (c == (n >> 3)) {
-      const uint32_t one = (n & 1) ? 0x3F800000u : 0x00003F80u;  // bf16 1.0 in the high / low half
-      const int w = (n & 7) >> 1;
-      if (w == 0) v.x = one; else if (w == 1) v.y = one; else if (w == 2) v.z = one; else v.w = one;
-    }
-    st_shared_v4(smem_u32(smem + OFF_I) + n * 128 + ((c ^ (n & 7)) << 4), v);
-  }
-  fence_proxy_async_smem();
   __syncthreads();
 
   if (warp >= 8) {
@@ -119,6 +121,24 @@ i2t_fused_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
+    } else if ((warp == 9 || warp == 10) && lane == 0) {
+      // ---------------------------------------------------------- TMA stores of consumer warpgroup g (kept out of the
+      // consumers' code, where the store instructions cost ptxas the registers of the wgmma pipeline)
+      const int g = warp - 9;
+      int ob = 0;
+      uint32_t ophase = 0;
+      for (int item = it_begin; item < it_end; ++item) {
+        const int orow = (item / TILES) * 4096 + (item % TILES) * 128 + 64 * g;
+        for (int j = 0; j < 4; ++j) {
+          mbar_wait(&ofull[g * OBUF + ob], ophase, 14);
+          tma_store_2d(&tmO, smem + OFF_O + (g * OBUF + ob) * 8192, 64 * j, orow);
+          tma_store_commit();
+          tma_store_wait_read<0>();
+          mbar_arrive(&oempty[g * OBUF + ob]);
+          if (++ob == OBUF) { ob = 0; ophase ^= 1; }
+        }
+      }
+      tma_store_wait_all();
     }
     return;
   }
@@ -126,15 +146,17 @@ i2t_fused_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
 
   // ------------------------------------------------------------ warpgroup g: rows [64 g, 64 g + 64) of each tile.
   // Fragment element i of a thread: row 64 g + 16 wq + qr + 8 ((i >> 1) & 1), column 8 (i >> 2) + qc + (i & 1).
+  // In a [64 x 64] SW128 tile (the ring's residual half, the output staging) the bf16 pair (row r, columns 8 jj + qc, +1)
+  // sits at byte r * 128 + ((jj ^ (r & 7)) << 4) + 2 qc, and r & 7 = qr: the 8 rows of a warp hit 8 distinct 16-B chunks.
   const int g = warp >> 2, wq = warp & 3, qr = lane >> 2, qc = 2 * (lane & 3);
   const uint32_t own = (uint32_t)g * 8192u;
-  const uint64_t di = make_desc_sw128(smem_u32(smem + OFF_I), 0, 1024);
-  const uint32_t aV = smem_u32(smem + OFF_V);
+  const uint32_t frag = (uint32_t)(16 * wq + qr) * 128u + (uint32_t)qc * 2u;  // byte offset of rows rs = 0 (+1024: rs = 1)
+  const uint32_t aV = smem_u32(smem + OFF_V), ostage = smem_u32(smem + OFF_O) + (uint32_t)g * (OBUF * 8192u);
   const int T = p.T;
-  int stage = 0, cur_p = -1, nload = 0;
-  uint32_t phase = 0;
+  int stage = 0, cur_p = -1, nload = 0, ob = 0;
+  uint32_t phase = 0, ophase = 0;
   for (int item = it_begin; item < it_end; ++item) {
-    const int pp = item / TILES, rt = item % TILES;
+    const int pp = item / TILES;
     if (pp != cur_p) {
       mbar_wait(mv_full, nload & 1, 12);
       cur_p = pp; ++nload;
@@ -146,8 +168,6 @@ i2t_fused_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
       const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + own;
       const uint64_t d0 = make_desc_sw128(sa, 0, 1024), d1 = make_desc_sw128(sa + SUB, 0, 1024);
       const uint64_t dm = make_desc_sw128(smem_u32(smem + OFF_M + j * 8192), 0, 1024);
-      const uint64_t dr = p.mode ? d0 : d1;
-      float(&oj)[32] = *reinterpret_cast<float(*)[32]>(&o[32 * j]);   // columns [64 j, 64 j + 64) of O
       wg_fence();
 #pragma unroll
       for (int k = 0; k < 4; ++k) wgmma<64>(sacc, d0 + 2 * k, dm + 2 * k, (j | k) != 0);
@@ -155,12 +175,25 @@ i2t_fused_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
 #pragma unroll
         for (int k = 0; k < 4; ++k) wgmma<64>(sacc, d1 + 2 * k, dm + 2 * k, 1);
       }
-#pragma unroll
-      for (int k = 0; k < 4; ++k) wgmma<64>(oj, dr + 2 * k, di + 2 * k, k != 0);
       wg_commit();
+      // residual columns [64 j, 64 j + 64), read while the score MMAs run
+      const uint32_t res = (p.mode ? sa : sa + SUB) + frag;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+        for (int rs = 0; rs < 2; ++rs) {
+          uint32_t v;
+          asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(res + rs * 1024u + ((uint32_t)(jj ^ qr) << 4)));
+          o[32 * j + 4 * jj + 2 * rs] = __uint_as_float(v << 16);  // bf16 -> fp32 is exact
+          o[32 * j + 4 * jj + 2 * rs + 1] = __uint_as_float(v & 0xFFFF0000u);
+        }
+      }
       wg_wait<0>();
       wg_fence_acc(sacc);
-      wg_fence_acc(oj);
+      wg_fence_acc(*reinterpret_cast<float(*)[32]>(&o[32 * j]));
+      // The stage was read by the wgmma (async proxy, complete after the wait) and by the ld.shared above (generic proxy).
+      // Those loads have returned their values before the arrive, whose release semantics order them before the producer's
+      // acquire of the empty barrier and hence before the TMA that overwrites the stage.
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty_bar[stage]);
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -205,16 +238,20 @@ i2t_fused_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
       if (lane == 0) mbar_arrive(mv_empty);
     }
     // + out-proj bias, LayerNorm over the 256 channels of each row (this thread: 64 of them, the quad: all)
+    float sums[2] = {0.f, 0.f}, rstd[2], shift[2];
+#pragma unroll
+    for (int jj = 0; jj < 32; ++jj) {
+      const float2 b = *reinterpret_cast<const float2*>(&rowp[8 * jj + qc]);
+#pragma unroll
+      for (int rs = 0; rs < 2; ++rs) {
+        o[4 * jj + 2 * rs] += b.x;
+        o[4 * jj + 2 * rs + 1] += b.y;
+        sums[rs] += o[4 * jj + 2 * rs] + o[4 * jj + 2 * rs + 1];
+      }
+    }
 #pragma unroll
     for (int rs = 0; rs < 2; ++rs) {
-      float sum = 0.f;
-#pragma unroll
-      for (int jj = 0; jj < 32; ++jj) {
-        const int col = 8 * jj + qc;
-        o[4 * jj + 2 * rs] += rowp[col];
-        o[4 * jj + 2 * rs + 1] += rowp[col + 1];
-        sum += o[4 * jj + 2 * rs] + o[4 * jj + 2 * rs + 1];
-      }
+      float sum = sums[rs];
       sum += __shfl_xor_sync(0xffffffffu, sum, 1);
       sum += __shfl_xor_sync(0xffffffffu, sum, 2);
       const float mean = sum * (1.0f / 256);
@@ -226,16 +263,32 @@ i2t_fused_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
       }
       q += __shfl_xor_sync(0xffffffffu, q, 1);
       q += __shfl_xor_sync(0xffffffffu, q, 2);
-      const float rstd = rsqrtf(q * (1.0f / 256) + p.eps);
-      const float shift = -mean * rstd;
-      __nv_bfloat16* orow = out + ((size_t)pp * 4096 + rt * 128 + 64 * g + 16 * wq + qr + 8 * rs) * 256;
+      rstd[rs] = rsqrtf(q * (1.0f / 256) + p.eps);
+      shift[rs] = -mean * rstd[rs];
+    }
+    // normalised rows of slice j -> staging tile ob, stored by this warpgroup's store warp as the [64 x 64] block at
+    // (column 64 j, row of this warpgroup)
 #pragma unroll
-      for (int jj = 0; jj < 32; ++jj) {
-        const int col = 8 * jj + qc;
-        const float y0 = fmaf(fmaf(o[4 * jj + 2 * rs], rstd, shift), rowp[256 + col], rowp[512 + col]);
-        const float y1 = fmaf(fmaf(o[4 * jj + 2 * rs + 1], rstd, shift), rowp[256 + col + 1], rowp[512 + col + 1]);
-        *reinterpret_cast<uint32_t*>(orow + col) = pack_bf16(y0, y1);
+    for (int j = 0; j < 4; ++j) {
+      mbar_wait(&oempty[g * OBUF + ob], ophase ^ 1, 15);
+      const uint32_t buf = ostage + (uint32_t)ob * 8192u;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        const int col = 64 * j + 8 * jj + qc;
+        const float2 ga = *reinterpret_cast<const float2*>(&rowp[256 + col]);
+        const float2 be = *reinterpret_cast<const float2*>(&rowp[512 + col]);
+#pragma unroll
+        for (int rs = 0; rs < 2; ++rs) {
+          const float y0 = fmaf(fmaf(o[32 * j + 4 * jj + 2 * rs], rstd[rs], shift[rs]), ga.x, be.x);
+          const float y1 = fmaf(fmaf(o[32 * j + 4 * jj + 2 * rs + 1], rstd[rs], shift[rs]), ga.y, be.y);
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(buf + frag + rs * 1024u + ((uint32_t)(jj ^ qr) << 4)), "r"(pack_bf16(y0, y1))
+                       : "memory");
+        }
       }
+      fence_proxy_async_smem();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&ofull[g * OBUF + ob]);
+      if (++ob == OBUF) { ob = 0; ophase ^= 1; }
     }
   }
 }
@@ -249,19 +302,20 @@ int launch_i2t_fused(const I2tFusedArgs& a, int num_sms, cudaStream_t stream) {
     if (e != cudaSuccess) return set_error("i2t_fused: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
     attr_set = true;
   }
-  CUtensorMap tmA0, tmA1, tmM, tmV;
+  CUtensorMap tmA0, tmA1, tmM, tmV, tmO;
   const uint64_t xrows = a.mode ? (uint64_t)a.P * 4096 : 4096;
   if (make_tmap_bf16_2d(&tmA0, a.a0, xrows, 256, 256, 128)) return -1;
   if (make_tmap_bf16_2d(&tmA1, a.a1, 4096, 256, 256, 128)) return -1;
   if (make_tmap_bf16_2d(&tmM, a.mq, (uint64_t)a.P * 64, 256, 256, 64)) return -1;
   if (make_tmap_bf16_2d(&tmV, a.vt, 256, (uint64_t)a.P * 64, (uint64_t)a.P * 64, 256)) return -1;
+  if (make_tmap_bf16_2d(&tmO, a.out, (uint64_t)a.P * 4096, 256, 256, 64)) return -1;
   I2tParams p;
   p.P = a.P; p.T = a.T; p.mode = a.mode; p.sbias = a.sbias; p.bias = a.bias; p.gamma = a.gamma; p.beta = a.beta; p.eps = a.eps;
   const long total = (long)a.P * TILES;
   const int grid = total < num_sms ? (int)total : num_sms;
   const double bytes = (double)a.P * 4096 * 256 * 2 * (a.mode ? 2 : 1) + (double)a.P * 64 * 256 * 2 * 2;
   prof_begin(stream, a.mode ? "i2t_fused (own keys)" : "i2t_fused (shared image)", (double)a.P * 4096 * (2.0 * 256 * 64 * (a.mode ? 2 : 1) + 2.0 * 64 * 256), bytes);
-  i2t_fused_kernel<<<grid, THREADS, SMEM_BYTES, stream>>>(tmA0, tmA1, tmM, tmV, p, a.out);
+  i2t_fused_kernel<<<grid, THREADS, SMEM_BYTES, stream>>>(tmA0, tmA1, tmM, tmV, tmO, p);
   prof_end(stream);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error("i2t_fused launch failed: %s", cudaGetErrorString(e));
