@@ -85,7 +85,8 @@ int msam_decode_ex(msam_handle* h, const float* points, const float* labels, int
  * a mask prompt the dense embedding is the broadcast no_mask_embed and dense_out is not written);
  * sam.prompt_encoder.get_dense_pe() -> token-major [4096, 256] (the caller views it as (1, 256, 64, 64));
  * sam.mask_decoder(image_embeddings = the bound embedding, image_pe = get_dense_pe(), sparse, dense|NULL = no mask,
- * multimask_output) -> low_res [P, M, 256, 256], iou [P, M]. */
+ * multimask_output) -> low_res [P, M, 256, 256], iou [P, M].  n_sparse = 0 with dense = NULL (an empty prompt) decodes the 5
+ * output tokens alone, as upstream does. */
 int msam_prompt_encode(msam_handle* h, const float* points, const float* labels, int n_points, const float* boxes,
                        const float* mask_input, int P, float* sparse_out, float* dense_out, void* stream);
 int msam_get_dense_pe(msam_handle* h, float* out_4096x256, void* stream);
@@ -196,6 +197,23 @@ int msam_op_layernorm(const float* x, int rows, int D, const float* gamma, const
 /* Encoder attention on a packed qkv buffer (see csrc/attention.cu). rel_table: bf16 [NT, 64*ceil(hd/64)]. */
 int msam_op_attention(const void* qkv_bf16, const void* rel_table_bf16, void* out_bf16, int batch, int heads, int head_dim,
                       int window, float scale, void* stream);
+/* The three fused mask-decoder blocks, running the code msam_decode runs for them, on explicit bf16 inputs with the weights as
+ * loaded.  P <= max_prompts prompts of T tokens (5 <= T <= 16).  num_sms caps the grid of the persistent kernels (0 = the
+ * device's SM count): results must not depend on it.
+ * t2i: token -> image attention instance `which` (0 / 1 = cross_attn_token_to_image of layer 0 / 1, 2 =
+ * final_attn_token_to_image), q_pe = queries + query_pe [P*T, 256], keys [P*4096, 256] or NULL = the bound image embedding
+ * shared by every prompt -> out [P*T, 128]: the per-head attention output before out_proj. */
+int msam_op_dec_t2i(msam_handle* h, int which, const void* q_pe, const void* keys, int P, int T, void* out, int num_sms,
+                    void* stream);
+/* i2t: image -> token block of `layer`, keys <- norm4(keys + cross_attn_image_to_token(q = keys + pe, k = q_pe, v = queries)),
+ * queries / q_pe [P*T, 256]; keys [P*4096, 256] is updated in place.  shared = 1 (layer 0 only): the block's input is the bound
+ * image embedding (no mask prompt) and keys is only written. */
+int msam_op_dec_i2t(msam_handle* h, int layer, const void* queries, const void* q_pe, int shared, void* keys, int P, int T,
+                    int num_sms, void* stream);
+/* upscale: output_upscaling(keys [P*4096, 256] bf16) times hyper_in [P, 4, 32] fp32 -> low_res [P, M, 256, 256] fp32 (multimask:
+ * masks 1..3, M = 3; else mask 0, M = 1). */
+int msam_op_dec_upscale(msam_handle* h, const void* keys, const float* hyper_in, int P, int multimask, float* low_res,
+                        int num_sms, void* stream);
 
 /* ---- fine-tuning (BASELINE.json configs[4], micro_sam/training/sam_trainer.py:393: loss.backward() through the image encoder).
  * msam_encode_train = msam_encode_f32 that keeps the activations of B <= max_batch images (ViT encoders only);

@@ -44,6 +44,9 @@ def lib() -> ctypes.CDLL:
         L.msam_op_gemm_nn.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]
         L.msam_op_layernorm.argtypes = [c_void_p, c_int, c_int, c_void_p, c_void_p, c_float, c_void_p, c_int, c_void_p]
         L.msam_op_attention.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]
+        L.msam_op_dec_t2i.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p]
+        L.msam_op_dec_i2t.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p]
+        L.msam_op_dec_upscale.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p]
         L.msam_set_image_embedding.argtypes = [c_void_p, c_void_p, c_void_p]
         L.msam_decode.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]
         L.msam_decode_ex.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,

@@ -624,6 +624,84 @@ int Engine::set_image_embedding(const float* feat, cudaStream_t st) {
   return 0;
 }
 
+// ---- The three blocks that do most of a decode.  decode_chunk and the op-level entry points (msam_op_dec_*) both call these
+// functions, so the tests exercise the production launch sequence.
+
+// Token -> image attention of instance A: qpe = queries + query_pe [P*T, 256] -> per-head output before out_proj
+// [P*T, 128] (t2i_fused.cu).  keys [P*4096, 256], or nullptr: the bound image, shared by every prompt.
+static int t2i_block(Engine& E, cudaStream_t st, const AttnW& A, int P, int T, const __nv_bfloat16* qpe,
+                     const __nv_bfloat16* keys, __nv_bfloat16* out) {
+  DecoderState& d = *E.dec;
+  const int mode = keys ? 1 : 0;
+  if (gemm(E, st, qpe, DC, A.q, P * T, DI, DC, A.qb, d.t_q128, DI, 0)) return -1;
+  // T <= 8: 64 rows per prompt (row pp*64 + h*8 + t).  Shared image tokens (mode 0): two prompts per 128-row item;
+  // own keys (mode 1): one 64-row item per prompt (one warpgroup).  T > 8: 128 rows per prompt (h*16 + t).
+  const int small = T <= 8 ? 1 : 0;
+  const int prep_items = small ? (P + 1) / 2 : P;   // 128-row blocks of the Q' operand
+  if (launch_t2i_prep(d.t_q128, P, T, small, prep_items, d.qexp, st)) return -1;
+  if (gemm(E, st, d.qexp, DI, A.kT, prep_items * 128, DC, DI, nullptr, d.qp, DC, 0)) return -1;
+  T2iFusedArgs ta;
+  ta.mode = mode;
+  ta.rows = (small && mode) ? 64 : 128;
+  ta.n_items = (small && mode) ? P : prep_items;
+  ta.x = mode ? keys : d.src_bf;
+  ta.xs = mode ? d.pos_bf : d.src_pe_bf;
+  ta.qp = d.qp; ta.out = d.un;
+  if (launch_t2i_fused(ta, E.num_sms, st)) return -1;
+  return launch_t2i_head_proj(d.un, A.vT, A.vb, P, T, small, out, st);
+}
+
+// Image -> token attention block of layer l (TwoWayAttentionBlock step 4): keys <- norm4(keys + attn(q = keys + pe,
+// k = qpe, v = q)) for P prompts, q / qpe = queries / queries + query_pe [P*T, 256].  Own keys are updated in place;
+// shared (layer 0 without per-prompt keys) reads the bound image and only writes keys.
+static int i2t_block(Engine& E, cudaStream_t st, int l, int P, int T, const __nv_bfloat16* q, const __nv_bfloat16* qpe,
+                     bool shared, __nv_bfloat16* keys) {
+  DecoderState& d = *E.dec;
+  const DecLayer& L = d.layers[l];
+  const int NI = 4096, PN = P * NI;
+  const bool fused = T <= 8;
+  if (!shared && !fused) {  // q of the (unfused) image -> token attention: (keys + pe) Wq^T, pe term through the residual
+    if (gemm(E, st, keys, DC, L.i2t.q, PN, DI, DC, L.i2t.qb, d.img_kvq, DI, 0, 0, d.q_res[l], NI)) return -1;
+  }
+  if (gemm(E, st, qpe, DC, L.i2t.k, P * T, DI, DC, L.i2t.kb, d.t_k128, DI, 0)) return -1;
+  if (gemm(E, st, q, DC, L.i2t.v, P * T, DI, DC, L.i2t.vb, d.t_v128, DI, 0)) return -1;
+  if (fused) {
+    // keys = norm4(keys + out_proj(attn)) in one pass over the image tokens (i2t_fused.cu)
+    if (launch_i2t_prep(d.t_k128, d.t_v128, L.i2t.qb, P, T, d.kexp, d.vexp, d.sbias, st)) return -1;
+    if (gemm(E, st, d.kexp, DI, L.i2t_qT, P * 64, DC, DI, nullptr, d.mq, DC, 0)) return -1;
+    if (gemm(E, st, L.i2t.o, DI, d.vexp, DC, P * 64, DI, nullptr, d.vt, P * 64, 0)) return -1;
+    I2tFusedArgs fa;
+    fa.P = P; fa.T = T; fa.mode = shared ? 0 : 1;
+    fa.a0 = shared ? d.src_pe_bf : keys;
+    fa.a1 = shared ? d.src_bf : d.pos_bf;
+    fa.mq = d.mq; fa.vt = d.vt; fa.sbias = d.sbias;
+    fa.bias = L.i2t.ob; fa.gamma = L.n4g; fa.beta = L.n4b; fa.eps = 1e-5f;
+    fa.out = keys;
+    return launch_i2t_fused(fa, E.num_sms, st);
+  }
+  if (shared) {
+    i2t_attn_kernel<<<dim3(NI / 64, P), 256, 0, st>>>(d.q0, DI, 0, d.t_k128, d.t_v128, T, NI, d.img_att);
+  } else {
+    i2t_attn_kernel<<<dim3(NI / 64, P), 256, 0, st>>>(d.img_kvq, DI, NI, d.t_k128, d.t_v128, T, NI, d.img_att);
+  }
+  LAUNCH_CHECK("i2t_attn");
+  // LayerNorm fused into the out-projection GEMM epilogue (in place for own keys: every thread reads the residual of
+  // exactly the row segment it later overwrites)
+  if (shared) return gemm(E, st, d.img_att, DI, L.i2t.o, PN, DC, DI, L.i2t.ob, keys, DC, 0, 0, d.src_bf, NI, 1, 1, L.n4g, L.n4b, 1e-5f);
+  return gemm(E, st, d.img_att, DI, L.i2t.o, PN, DC, DI, L.i2t.ob, keys, DC, 0, 0, keys, PN, 1, 1, L.n4g, L.n4b, 1e-5f);
+}
+
+// Output upscaling + hyper product: convT(256->64) -> LN2d(64) -> GELU -> convT(64->32) -> GELU, dotted with hyper_in
+// [P, 4, 32]: one fused kernel (upscale_fused.cu); neither up-scaled embedding ever reaches HBM.
+static int upscale_block(Engine& E, cudaStream_t st, int P, int multimask, const __nv_bfloat16* keys, const float* hyper,
+                         float* low_res) {
+  DecoderState& d = *E.dec;
+  UpscaleFusedArgs ua;
+  ua.P = P; ua.nm = multimask ? 3 : 1; ua.m0 = multimask ? 1 : 0; ua.keys = keys; ua.w1 = d.ct1; ua.w2_f16 = d.ct2_f16;
+  ua.b1 = d.ct1b; ua.gamma = d.upln_g; ua.beta = d.upln_b; ua.eps = 1e-6f; ua.b2 = d.ct2b; ua.hyper = hyper; ua.out = low_res;
+  return launch_upscale_fused(ua, E.num_sms, st);
+}
+
 // One chunk of P <= max_prompts prompts.
 static int decode_chunk(Engine& E, cudaStream_t st, const float* points, const float* labels, int np, const float* boxes,
                         const float* mask_in, int P, int multimask, float* low_res, float* iou,
@@ -631,8 +709,10 @@ static int decode_chunk(Engine& E, cudaStream_t st, const float* points, const f
   DecoderState& d = *E.dec;
   const int NI = 4096;
   const int n_sparse = sparse ? n_sparse_given : (points ? np + (boxes ? 0 : 1) : 0) + (boxes ? 2 : 0);
-  const int T = 5 + n_sparse, PT = P * T, PN = P * NI;
-  if (n_sparse <= 0 && !mask_in && !dense) return set_error("decode: need points, boxes and/or mask prompts");
+  const int T = 5 + n_sparse, PT = P * T;
+  // Given embeddings with n_sparse = 0 and the no-mask dense embedding are what PromptEncoder returns for an empty prompt:
+  // upstream decodes the 5 output tokens alone (T = 5, shared image-side operands), and so does this path.
+  if (n_sparse <= 0 && !mask_in && !dense && n_sparse_given >= 0) return set_error("decode: need points, boxes and/or mask prompts");
   if (T > TMAX) return set_error("decode: %d tokens per prompt exceeds the supported %d", T, TMAX);
 
   if (sparse || n_sparse_given < 0) {  // given sparse embeddings (model-level mask_decoder call)
@@ -656,32 +736,9 @@ static int decode_chunk(Engine& E, cudaStream_t st, const float* points, const f
   }
   const bool own_keys = mask_in || dense;
 
-  // token -> image attention core: t_q128 -> t_att128 (t2i_fused.cu)
-  auto t2i = [&](const AttnW& A, int mode) -> int {
-    // T <= 8: 64 rows per prompt (row pp*64 + h*8 + t).  Shared image tokens (mode 0): two prompts per 128-row item;
-    // own keys (mode 1): one 64-row item per prompt (one warpgroup).  T > 8: 128 rows per prompt (h*16 + t).
-    const int small = T <= 8 ? 1 : 0;
-    const int prep_items = small ? (P + 1) / 2 : P;   // 128-row blocks of the Q' operand
-    if (launch_t2i_prep(d.t_q128, P, T, small, prep_items, d.qexp, st)) return -1;
-    if (gemm(E, st, d.qexp, DI, A.kT, prep_items * 128, DC, DI, nullptr, d.qp, DC, 0)) return -1;
-    T2iFusedArgs ta;
-    ta.mode = mode;
-    ta.rows = (small && mode) ? 64 : 128;
-    ta.n_items = (small && mode) ? P : prep_items;
-    ta.x = mode ? d.keys : d.src_bf;
-    ta.xs = mode ? d.pos_bf : d.src_pe_bf;
-    ta.qp = d.qp; ta.out = d.un;
-    if (launch_t2i_fused(ta, E.num_sms, st)) return -1;
-    return launch_t2i_head_proj(d.un, A.vT, A.vb, P, T, small, d.t_att128, st);
-  };
-
   for (int l = 0; l < 2; ++l) {
     const DecLayer& L = d.layers[l];
-    const bool fused_i2t = T <= 8;
     const bool shared = (l == 0) && !own_keys;  // image-side operands identical for every prompt
-    if (!shared && !fused_i2t) {  // q of the (unfused) image -> token attention: (keys + pe) Wq^T, pe term through the residual
-      if (gemm(E, st, d.keys, DC, L.i2t.q, PN, DI, DC, L.i2t.qb, d.img_kvq, DI, 0, 0, d.q_res[l], NI)) return -1;
-    }
     // ---- (1) token self attention
     if (l == 0) {
       if (gemm(E, st, d.tok0_bf, DC, L.self_attn.qkv, PT, 3 * DC, DC, L.self_attn.qkvb, d.t_qkv, 3 * DC, 0)) return -1;
@@ -700,8 +757,7 @@ static int decode_chunk(Engine& E, cudaStream_t st, const float* points, const f
     }
     if (ln(st, d.tok_f32, PT, DC, L.n1g, L.n1b, 1e-5f, d.q_bf, d.queries, d.tok0, PT, d.qpe_bf)) return -1;
     // ---- (2) token -> image cross attention
-    if (gemm(E, st, d.qpe_bf, DC, L.t2i.q, PT, DI, DC, L.t2i.qb, d.t_q128, DI, 0)) return -1;
-    if (t2i(L.t2i, shared ? 0 : 1)) return -1;
+    if (t2i_block(E, st, L.t2i, P, T, d.qpe_bf, shared ? nullptr : d.keys, d.t_att128)) return -1;
     if (gemm(E, st, d.t_att128, DI, L.t2i.o, PT, DC, DI, L.t2i.ob, d.tok_f32, DC, 1, 0, d.queries, PT)) return -1;
     if (ln(st, d.tok_f32, PT, DC, L.n2g, L.n2b, 1e-5f, d.q_bf, d.queries)) return -1;
     // ---- (3) MLP (ReLU)
@@ -709,42 +765,12 @@ static int decode_chunk(Engine& E, cudaStream_t st, const float* points, const f
     if (gemm(E, st, d.t_mlp, 2048, L.mlp2, PT, DC, 2048, L.mlp2b, d.tok_f32, DC, 1, 0, d.queries, PT)) return -1;
     if (ln(st, d.tok_f32, PT, DC, L.n3g, L.n3b, 1e-5f, d.q_bf, d.queries, d.tok0, PT, d.qpe_bf)) return -1;
     // ---- (4) image -> token cross attention (updates all image tokens of every prompt)
-    if (gemm(E, st, d.qpe_bf, DC, L.i2t.k, PT, DI, DC, L.i2t.kb, d.t_k128, DI, 0)) return -1;
-    if (gemm(E, st, d.q_bf, DC, L.i2t.v, PT, DI, DC, L.i2t.vb, d.t_v128, DI, 0)) return -1;
-    if (fused_i2t) {
-      // keys = norm4(keys + out_proj(attn)) in one pass over the image tokens (i2t_fused.cu)
-      if (launch_i2t_prep(d.t_k128, d.t_v128, L.i2t.qb, P, T, d.kexp, d.vexp, d.sbias, st)) return -1;
-      if (gemm(E, st, d.kexp, DI, L.i2t_qT, P * 64, DC, DI, nullptr, d.mq, DC, 0)) return -1;
-      if (gemm(E, st, L.i2t.o, DI, d.vexp, DC, P * 64, DI, nullptr, d.vt, P * 64, 0)) return -1;
-      I2tFusedArgs fa;
-      fa.P = P; fa.T = T; fa.mode = shared ? 0 : 1;
-      fa.a0 = shared ? d.src_pe_bf : d.keys;
-      fa.a1 = shared ? d.src_bf : d.pos_bf;
-      fa.mq = d.mq; fa.vt = d.vt; fa.sbias = d.sbias;
-      fa.bias = L.i2t.ob; fa.gamma = L.n4g; fa.beta = L.n4b; fa.eps = 1e-5f;
-      fa.out = d.keys;
-      if (launch_i2t_fused(fa, E.num_sms, st)) return -1;
-    } else {
-      if (shared) {
-        i2t_attn_kernel<<<dim3(NI / 64, P), 256, 0, st>>>(d.q0, DI, 0, d.t_k128, d.t_v128, T, NI, d.img_att);
-      } else {
-        i2t_attn_kernel<<<dim3(NI / 64, P), 256, 0, st>>>(d.img_kvq, DI, NI, d.t_k128, d.t_v128, T, NI, d.img_att);
-      }
-      LAUNCH_CHECK("i2t_attn");
-      // LayerNorm fused into the out-projection GEMM epilogue (in place for layer 1: every thread reads the residual of
-      // exactly the row segment it later overwrites)
-      if (shared) {
-        if (gemm(E, st, d.img_att, DI, L.i2t.o, PN, DC, DI, L.i2t.ob, d.keys, DC, 0, 0, d.src_bf, NI, 1, 1, L.n4g, L.n4b, 1e-5f)) return -1;
-      } else {
-        if (gemm(E, st, d.img_att, DI, L.i2t.o, PN, DC, DI, L.i2t.ob, d.keys, DC, 0, 0, d.keys, PN, 1, 1, L.n4g, L.n4b, 1e-5f)) return -1;
-      }
-    }
+    if (i2t_block(E, st, l, P, T, d.q_bf, d.qpe_bf, shared, d.keys)) return -1;
   }
   // ---- final token -> image attention
   {
     const AttnW& A = d.final_t2i;
-    if (gemm(E, st, d.qpe_bf, DC, A.q, PT, DI, DC, A.qb, d.t_q128, DI, 0)) return -1;
-    if (t2i(A, 1)) return -1;
+    if (t2i_block(E, st, A, P, T, d.qpe_bf, d.keys, d.t_att128)) return -1;
     if (gemm(E, st, d.t_att128, DI, A.o, PT, DC, DI, A.ob, d.tok_f32, DC, 1, 0, d.queries, PT)) return -1;
     if (ln(st, d.tok_f32, PT, DC, d.nfg, d.nfb, 1e-5f, d.q_bf)) return -1;
   }
@@ -761,15 +787,9 @@ static int decode_chunk(Engine& E, cudaStream_t st, const float* points, const f
       if (gemm(E, st, d.h2, DC, hm.w[2], P, 32, DC, hm.b[2], d.hyper_in + i * 32, 128, 1)) return -1;
     }
   }
-  // ---- output upscaling: convT(256->64) -> LN2d(64) -> GELU -> convT(64->32) -> GELU, then the hyper product: neither
-  // up-scaled embedding ever reaches HBM.
+  // ---- output upscaling + hyper product
   const int m0 = multimask ? 1 : 0, nm = multimask ? 3 : 1;
-  {  // convT1 + LN2d + GELU + convT2 + GELU + hyper product: one fused kernel (upscale_fused.cu)
-    UpscaleFusedArgs ua;
-    ua.P = P; ua.nm = nm; ua.m0 = m0; ua.keys = d.keys; ua.w1 = d.ct1; ua.w2_f16 = d.ct2_f16; ua.b1 = d.ct1b;
-    ua.gamma = d.upln_g; ua.beta = d.upln_b; ua.eps = 1e-6f; ua.b2 = d.ct2b; ua.hyper = d.hyper_in; ua.out = low_res;
-    if (launch_upscale_fused(ua, E.num_sms, st)) return -1;
-  }
+  if (upscale_block(E, st, P, multimask, d.keys, d.hyper_in, low_res)) return -1;
   gather_iou_kernel<<<(P * nm + 127) / 128, 128, 0, st>>>(d.iou_out, P, m0, nm, iou);
   LAUNCH_CHECK("gather_iou");
   return 0;
@@ -842,7 +862,6 @@ int Engine::mask_decode(const float* sparse, int n_sparse, const float* dense, i
   if (!dec->image_set) return set_error("mask_decode: no image embedding set");
   if (P <= 0) return set_error("mask_decode: empty prompt batch");
   if (n_sparse < 0 || (n_sparse > 0 && !sparse)) return set_error("mask_decode: bad sparse embeddings");
-  if (n_sparse == 0 && !dense) return set_error("mask_decode: need sparse and/or dense prompt embeddings");
   const int nm = multimask ? 3 : 1;
   for (int p0 = 0; p0 < P; p0 += cfg.max_prompts) {
     const int n = (P - p0 < cfg.max_prompts) ? (P - p0) : cfg.max_prompts;
@@ -852,6 +871,54 @@ int Engine::mask_decode(const float* sparse, int n_sparse, const float* dense, i
       return -1;
   }
   return 0;
+}
+
+// ---- op-level entry points of the three blocks (msam_op_dec_*): the functions decode_chunk calls, on explicit inputs.
+// The persistent kernels split their work items over min(items, num_sms) CTAs; num_sms > 0 overrides the device's count for
+// this call so that tests can vary the launch geometry.
+namespace {
+struct SmsOverride {
+  Engine& E;
+  int saved;
+  SmsOverride(Engine& e, int n) : E(e), saved(e.num_sms) { if (n > 0) e.num_sms = n; }
+  ~SmsOverride() { E.num_sms = saved; }
+};
+}  // namespace
+
+static int check_block(Engine& E, const char* name, int P, int T, int num_sms) {
+  if (!E.finalized || !E.dec) return set_error("%s: decoder weights not loaded", name);
+  if (P < 1 || P > E.cfg.max_prompts) return set_error("%s: P = %d outside [1, max_prompts = %d]", name, P, E.cfg.max_prompts);
+  if (T < 5 || T > TMAX) return set_error("%s: T = %d tokens per prompt outside [5, %d]", name, T, TMAX);
+  if (num_sms < 0) return set_error("%s: num_sms = %d < 0", name, num_sms);
+  return 0;
+}
+
+int Engine::op_dec_t2i(int which, const __nv_bfloat16* qpe, const __nv_bfloat16* keys, int P, int T, __nv_bfloat16* out,
+                       int sms, cudaStream_t st) {
+  if (check_block(*this, "op_dec_t2i", P, T, sms)) return -1;
+  if (!qpe || !out) return set_error("op_dec_t2i: null argument");
+  if (which < 0 || which > 2) return set_error("op_dec_t2i: attention instance %d (0, 1 = layers, 2 = final)", which);
+  if (!keys && !dec->image_set) return set_error("op_dec_t2i: the shared mode needs a bound image embedding");
+  SmsOverride o(*this, sms);
+  return t2i_block(*this, st, which == 2 ? dec->final_t2i : dec->layers[which].t2i, P, T, qpe, keys, out);
+}
+
+int Engine::op_dec_i2t(int layer, const __nv_bfloat16* q, const __nv_bfloat16* qpe, int shared, __nv_bfloat16* keys, int P,
+                       int T, int sms, cudaStream_t st) {
+  if (check_block(*this, "op_dec_i2t", P, T, sms)) return -1;
+  if (!q || !qpe || !keys) return set_error("op_dec_i2t: null argument");
+  if (layer < 0 || layer > 1) return set_error("op_dec_i2t: layer %d (0 or 1)", layer);
+  if (shared && (layer != 0 || !dec->image_set)) return set_error("op_dec_i2t: the shared mode is layer 0 on a bound image");
+  SmsOverride o(*this, sms);
+  return i2t_block(*this, st, layer, P, T, q, qpe, shared != 0, keys);
+}
+
+int Engine::op_dec_upscale(const __nv_bfloat16* keys, const float* hyper, int P, int multimask, float* low_res, int sms,
+                           cudaStream_t st) {
+  if (check_block(*this, "op_dec_upscale", P, 5, sms)) return -1;
+  if (!keys || !hyper || !low_res) return set_error("op_dec_upscale: null argument");
+  SmsOverride o(*this, sms);
+  return upscale_block(*this, st, P, multimask, keys, hyper, low_res);
 }
 
 int Engine::dense_pe(float* out_tokmajor, cudaStream_t st) {

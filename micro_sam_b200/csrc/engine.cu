@@ -647,6 +647,24 @@ int msam_op_attention(const void* qkv, const void* rel_table, void* out, int bat
   return launch_attention(a, (cudaStream_t)stream);
 }
 
+int msam_op_dec_t2i(msam_handle* h, int which, const void* q_pe, const void* keys, int P, int T, void* out, int num_sms,
+                    void* stream) {
+  if (!h) return set_error("msam_op_dec_t2i: null handle");
+  return h->eng.op_dec_t2i(which, (const __nv_bfloat16*)q_pe, (const __nv_bfloat16*)keys, P, T, (__nv_bfloat16*)out, num_sms,
+                           (cudaStream_t)stream);
+}
+int msam_op_dec_i2t(msam_handle* h, int layer, const void* queries, const void* q_pe, int shared, void* keys, int P, int T,
+                    int num_sms, void* stream) {
+  if (!h) return set_error("msam_op_dec_i2t: null handle");
+  return h->eng.op_dec_i2t(layer, (const __nv_bfloat16*)queries, (const __nv_bfloat16*)q_pe, shared, (__nv_bfloat16*)keys, P, T,
+                           num_sms, (cudaStream_t)stream);
+}
+int msam_op_dec_upscale(msam_handle* h, const void* keys, const float* hyper_in, int P, int multimask, float* low_res,
+                        int num_sms, void* stream) {
+  if (!h) return set_error("msam_op_dec_upscale: null handle");
+  return h->eng.op_dec_upscale((const __nv_bfloat16*)keys, hyper_in, P, multimask, low_res, num_sms, (cudaStream_t)stream);
+}
+
 int msam_encode_train(msam_handle* h, const float* nchw, int B, float* out, void* stream) {
   if (!h || !nchw || !out) return set_error("msam_encode_train: null argument");
   return h->eng.encode_train(nchw, B, out, (cudaStream_t)stream);

@@ -145,6 +145,13 @@ struct Engine {
   int mask_decode(const float* sparse, int n_sparse, const float* dense, int P, int multimask, float* low_res, float* iou,
                   cudaStream_t st);  // decoder.cu
   int dense_pe(float* out_tokmajor, cudaStream_t st);  // decoder.cu
+  // decoder.cu: the three fused decoder blocks on explicit inputs (msam_op_dec_*); sms > 0 overrides num_sms for the call
+  int op_dec_t2i(int which, const __nv_bfloat16* qpe, const __nv_bfloat16* keys, int P, int T, __nv_bfloat16* out, int sms,
+                 cudaStream_t st);
+  int op_dec_i2t(int layer, const __nv_bfloat16* q, const __nv_bfloat16* qpe, int shared, __nv_bfloat16* keys, int P, int T,
+                 int sms, cudaStream_t st);
+  int op_dec_upscale(const __nv_bfloat16* keys, const float* hyper, int P, int multimask, float* low_res, int sms,
+                     cudaStream_t st);
 };
 
 // postprocess.cu
