@@ -3,7 +3,9 @@ fp32 oracle encoder (oracle/sam_ref.py): op level (batched attention-backward GE
 backward) and model level (every parameter gradient of the image encoder for a random upstream gradient dL/d embedding).
 Tolerance: encoder alone (random upstream gradient) rel-L2 <= 3e-2 per gradient tensor (bf16 operands, fp32 accumulation; the forward
 tolerance is 2e-2); decoder and whole step: rel-L2 <= 1.5e-1 and cosine >= 0.99 per tensor = the measured bf16 noise floor of the
-decoder (see test_decoder_train_against_autograd); the loss-statistics adjoint is exact to 1e-6."""
+decoder (see test_decoder_train_against_autograd); the loss-statistics adjoint is exact to 1e-6.  The decoder is also compared with
+a float64 mirror that rounds to bf16 where the kernels do, over more prompt counts, token counts and backward paths, in
+tests/test_gpu_decoder_train.py."""
 import os
 import tempfile
 
