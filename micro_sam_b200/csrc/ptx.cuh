@@ -78,6 +78,12 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* s
                "r"(smem_u32(src)), "r"(c0), "r"(c1)
                : "memory");
 }
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // until at most N committed store groups still read their shared-memory source
 template <int N = 0>
