@@ -234,6 +234,19 @@ int msam_encoder_grad(msam_handle* h, const char* name, float* dst, int64_t n, v
 int msam_decoder_train_forward(msam_handle* h, int slot, const float* emb_nchw, const float* sparse, const int32_t* emb_index, int n_sparse,
                                int P, int multimask, float* low_res, float* iou, void* stream);
 int msam_decoder_train_backward(msam_handle* h, int slot, const float* d_low_res, const float* d_iou, float* d_emb_nchw, void* stream);
+/* msam_decoder_train_forward with mask prompts: mask_input [P, 1, 256, 256] fp32 low-res logits (PromptEncoder._embed_masks), or NULL
+ * (= msam_decoder_train_forward).  The dense prompt is then mask_downscaling(mask_input) instead of no_mask_embed.  The first call with
+ * masks adds the ten "prompt_encoder.mask_downscaling.*" tensors (upstream keys and layouts) to the gradient table and the optimizer;
+ * msam_decoder_train_backward of such a slot accumulates their gradients (none w.r.t. the mask) and none for no_mask_embed, and
+ * msam_optimizer_step updates them only when a masked backward has run since the last msam_decoder_zero_grads. */
+int msam_decoder_train_forward_ex(msam_handle* h, int slot, const float* emb_nchw, const float* sparse, const int32_t* emb_index,
+                                  int n_sparse, int P, const float* mask_input, int multimask, float* low_res, float* iou, void* stream);
+/* mask_downscaling alone, forward and backward, with the training masters (op-level tests): mask [P, 1, 256, 256] -> dense_out
+ * [P, 4096, 256] (token-major: the layout that is added to the image embedding); d_dense [P, 4096, 256] = upstream gradient ->
+ * grads_out [4684] = the gradients of the ten tensors, overwritten, concatenated in the order 0.weight, 0.bias, 1.weight, 1.bias,
+ * 3.weight, 3.bias, 4.weight, 4.bias, 6.weight, 6.bias (each in its upstream layout).  Leaves the engine's gradients alone. */
+int msam_op_mask_downscaling_train(msam_handle* h, const float* mask, int P, const float* d_dense, float* dense_out, float* grads_out,
+                                   void* stream);
 int msam_decoder_grad(msam_handle* h, const char* name, float* dst, int64_t n, void* stream);
 int msam_decoder_zero_grads(msam_handle* h, void* stream);
 /* torch.optim.AdamW semantics (micro_sam/training/training.py:train_sam's default optimizer) over every tensor that has received

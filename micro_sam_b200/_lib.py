@@ -97,6 +97,9 @@ def lib() -> ctypes.CDLL:
         L.msam_debug_attn_trace.argtypes = [c_void_p]
         L.msam_decoder_train_forward.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
                                                  c_void_p]
+        L.msam_decoder_train_forward_ex.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p,
+                                                    c_void_p, c_void_p]
+        L.msam_op_mask_downscaling_train.argtypes = [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
         L.msam_decoder_train_backward.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
         L.msam_decoder_grad.argtypes = [c_void_p, c_char_p, c_void_p, c_int64, c_void_p]
         L.msam_decoder_zero_grads.argtypes = [c_void_p, c_void_p]

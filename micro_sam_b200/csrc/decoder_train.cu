@@ -9,7 +9,8 @@
 // GEMMs (gemm.cu), the batched attention GEMM (bgemm.cu), LayerNorm -- allocates its output from a per-slot arena
 // and pushes its backward closure; backward() replays the closures in reverse.  Tensors carry an fp32 value, an fp32 gradient
 // (accumulated: every consumer ADDS) and a bf16 copy (the GEMM operand).  Parameter gradients accumulate across calls (images,
-// sub-iterations) until msam_decoder_zero_grads.  Supported prompts: points and / or boxes (dense prompt = no_mask_embed).
+// sub-iterations) until msam_decoder_zero_grads.  Prompts: points and / or boxes, with the dense prompt no_mask_embed or, for mask
+// prompts, mask_downscaling(mask) (md_* kernels: fp32, taped by keeping the mask; no gradient w.r.t. the mask itself).
 #include "engine.h"
 
 #include <algorithm>
@@ -201,6 +202,346 @@ __global__ void transpose_bf16_dk(const __nv_bfloat16* __restrict__ in, int rows
 
 inline unsigned nblk(long n, int per = 256) { return (unsigned)((n + per - 1) / per); }
 
+// ------------------------------------------------------------------------------------------------ mask prompts
+// PromptEncoder.mask_downscaling: conv 1->4 (k2 s2, 256^2 -> 128^2), LayerNorm2d(4), GELU, conv 4->16 (k2 s2 -> 64^2), LayerNorm2d(16),
+// GELU, conv 1x1 16->256, all fp32.  Output pixel (ty, tx) of the 64^2 grid depends on its own 4x4 input patch only.  The ten
+// parameters live in one packed fp32 buffer (masters and gradients alike) in upstream order and layout:
+constexpr int MD_W1 = 0, MD_B1 = 16, MD_G1 = 20, MD_BE1 = 24, MD_W2 = 28, MD_B2 = 284, MD_G2 = 300, MD_BE2 = 316, MD_W3 = 332,
+              MD_B3 = 4428, MD_N = 4684;
+constexpr int MD_SMALL = MD_W3;      // parameters of the two strided stages (reduced from md_param_grad_kernel's partials)
+constexpr int MD_BIG = MD_N - MD_W3; // W3 + b3 (reduced from md_keys_grad_kernel's partials)
+constexpr int MD_PIX_TILE = 128;     // pixels per tile of md_param_grad_kernel (= its block size)
+constexpr int MD_GRID2 = 256;        // most blocks of md_param_grad_kernel: partial rows to reduce, independent of the device
+
+__device__ __forceinline__ float md_gelu(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
+__device__ __forceinline__ float md_gelu_grad(float x) {   // d/dx [x Phi(x)] = Phi(x) + x phi(x), exact erf form
+  return 0.5f * (1.0f + erff(x * 0.70710678118654752440f)) + x * 0.39894228040143267794f * expf(-0.5f * x * x);
+}
+
+// Stages of one output pixel.  Index s = sy * 2 + sx is the stage-1 sub-pixel, k = dy * 2 + dx the position in a 2x2 conv window;
+// stage-1 channel c of sub-pixel s sits at c * 4 + s, the order of W2's input index (W2 [o][c][sy][sx]).  LayerNorm2d statistics are
+// two-pass (mean first, then the centred sum of squares): an almost constant mask makes the 4 stage-1 channels almost equal, and a
+// one-pass E[x^2] - E[x]^2 would cancel.
+// Stage 1 at sub-pixel s: m = the 2x2 input window, n = normalised, a = affine (pre-GELU) values of the 4 channels; returns rstd.
+__device__ __forceinline__ float md_stage1(const float* __restrict__ mask_p, int pix, int s, const float* W, float m[4], float n[4],
+                                           float a[4]) {
+  const float* mp = mask_p + (size_t)(4 * (pix >> 6) + 2 * (s >> 1)) * 256 + 4 * (pix & 63) + 2 * (s & 1);
+  m[0] = mp[0]; m[1] = mp[1]; m[2] = mp[256]; m[3] = mp[257];
+  float y[4], mean = 0.f;
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+    float acc = W[MD_B1 + c];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) acc += W[MD_W1 + c * 4 + k] * m[k];
+    y[c] = acc;
+    mean += acc;
+  }
+  mean *= 0.25f;
+  float var = 0.f;
+#pragma unroll
+  for (int c = 0; c < 4; ++c) var += (y[c] - mean) * (y[c] - mean);
+  const float rstd = rsqrtf(var * 0.25f + 1e-6f);
+#pragma unroll
+  for (int c = 0; c < 4; ++c) { n[c] = (y[c] - mean) * rstd; a[c] = n[c] * W[MD_G1 + c] + W[MD_BE1 + c]; }
+  return rstd;
+}
+// Stage 2 from the stage-1 GELU outputs h1[c * 4 + s]: n = normalised, a = affine (pre-GELU) values of the 16 channels; returns rstd.
+__device__ __forceinline__ float md_stage2(const float h1[16], const float* W, float n[16], float a[16]) {
+  float z[16], mean = 0.f;
+#pragma unroll
+  for (int o = 0; o < 16; ++o) {
+    float acc = W[MD_B2 + o];
+#pragma unroll
+    for (int k = 0; k < 16; ++k) acc += W[MD_W2 + o * 16 + k] * h1[k];
+    z[o] = acc;
+    mean += acc;
+  }
+  mean *= (1.0f / 16);
+  float var = 0.f;
+#pragma unroll
+  for (int o = 0; o < 16; ++o) var += (z[o] - mean) * (z[o] - mean);
+  const float rstd = rsqrtf(var * (1.0f / 16) + 1e-6f);
+#pragma unroll
+  for (int o = 0; o < 16; ++o) { n[o] = (z[o] - mean) * rstd; a[o] = n[o] * W[MD_G2 + o] + W[MD_BE2 + o]; }
+  return rstd;
+}
+// the stage-2 GELU outputs h2 of one pixel (forward)
+__device__ __forceinline__ void md_pixel(const float* __restrict__ mask_p, int pix, const float* W, float h2[16]) {
+  float h1[16];
+#pragma unroll
+  for (int s = 0; s < 4; ++s) {
+    float m[4], n[4], a[4];
+    md_stage1(mask_p, pix, s, W, m, n, a);
+#pragma unroll
+    for (int c = 0; c < 4; ++c) h1[c * 4 + s] = md_gelu(a[c]);
+  }
+  float n2[16], a2[16];
+  md_stage2(h1, W, n2, a2);
+#pragma unroll
+  for (int o = 0; o < 16; ++o) h2[o] = md_gelu(a2[o]);
+}
+
+// Forward: out[p, pix, c] = dense_p[c, pix] (+ emb_nchw[c, pix]); h2_out[p, pix, 0..15] = stage-2 output (the 1x1 conv's input,
+// kept for its weight gradient).  grid = (4096 / 16, P), block = 256 (thread = output channel; 16 pixels per block).
+__global__ void __launch_bounds__(256)
+md_forward_kernel(const float* __restrict__ mask, const float* __restrict__ W, const float* __restrict__ emb_nchw,
+                  float* __restrict__ out, __nv_bfloat16* __restrict__ out_bf, float* __restrict__ h2_out) {
+  __shared__ float sh[16][17];
+  const int p = blockIdx.y, pix0 = blockIdx.x * 16, tid = threadIdx.x;
+  if (tid < 16) {
+    float h2[16];
+    md_pixel(mask + (size_t)p * 65536, pix0 + tid, W, h2);
+#pragma unroll
+    for (int o = 0; o < 16; ++o) { sh[tid][o] = h2[o]; h2_out[((size_t)p * 4096 + pix0 + tid) * 16 + o] = h2[o]; }
+  }
+  __syncthreads();
+  float w[16];
+#pragma unroll
+  for (int o = 0; o < 16; ++o) w[o] = W[MD_W3 + tid * 16 + o];
+  const float b = W[MD_B3 + tid];
+  for (int i = 0; i < 16; ++i) {
+    float acc = b;
+#pragma unroll
+    for (int o = 0; o < 16; ++o) acc += w[o] * sh[i][o];
+    if (emb_nchw) acc += emb_nchw[(size_t)tid * 4096 + pix0 + i];
+    const size_t row = (size_t)p * 4096 + pix0 + i;
+    out[row * 256 + tid] = acc;
+    if (out_bf) out_bf[row * 256 + tid] = __float2bfloat16(acc);
+  }
+}
+
+// Backward, part 1: the one pass over g = dL/d keys0 [P, 4096, 256].  Per 16-pixel tile (grid = 256, block = 256, thread = channel):
+// d_emb_nchw[c, pix] = sum_p g[p, pix, c] (when non-null), d_h2[p, pix, :] = g[p, pix, :] W3, and this block's partial sums of
+// dW3 = sum g^T h2 and db3 = sum g -> part[blockIdx.x][MD_BIG] (reduced by md_reduce_kernel; no atomics).
+__global__ void __launch_bounds__(256)
+md_keys_grad_kernel(const float* __restrict__ g, const float* __restrict__ h2, const float* __restrict__ W, int P,
+                    float* __restrict__ d_emb_nchw, float* __restrict__ d_h2, float* __restrict__ part) {
+  __shared__ float gs[16][257];
+  __shared__ float hs[16][16];
+  __shared__ float w3s[256 * 16];
+  const int pix0 = blockIdx.x * 16, tid = threadIdx.x;
+  for (int i = tid; i < 256 * 16; i += 256) w3s[i] = W[MD_W3 + i];
+  float demb[16], dw[16], db = 0.f;
+#pragma unroll
+  for (int i = 0; i < 16; ++i) { demb[i] = 0.f; dw[i] = 0.f; }
+  for (int p = 0; p < P; ++p) {
+    __syncthreads();
+    const size_t row0 = (size_t)p * 4096 + pix0;
+#pragma unroll 4
+    for (int i = 0; i < 16; ++i) gs[i][tid] = g[(row0 + i) * 256 + tid];
+    hs[tid >> 4][tid & 15] = h2[row0 * 16 + tid];
+    __syncthreads();
+    {
+      const int i = tid >> 4, o = tid & 15;
+      float acc = 0.f;
+#pragma unroll 8
+      for (int c = 0; c < 256; ++c) acc += gs[i][c] * w3s[c * 16 + o];
+      d_h2[row0 * 16 + tid] = acc;
+    }
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const float v = gs[i][tid];
+      demb[i] += v;
+      db += v;
+#pragma unroll
+      for (int o = 0; o < 16; ++o) dw[o] += v * hs[i][o];
+    }
+  }
+  if (d_emb_nchw) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) d_emb_nchw[(size_t)tid * 4096 + pix0 + i] = demb[i];
+  }
+  float* pr = part + (size_t)blockIdx.x * MD_BIG;
+#pragma unroll
+  for (int o = 0; o < 16; ++o) pr[tid * 16 + o] = dw[o];
+  pr[4096 + tid] = db;
+}
+
+// Backward, part 2: pixel-local GELU', LayerNorm2d backward and the transposed k2s2 convs through both stages (stage values are
+// recomputed from the mask).  Block b (MD_PIX_TILE threads, thread = pixel) takes the tiles b, b + gridDim.x, ... of the P * 4096
+// pixels; per tile, phase A puts each pixel's terms in shared memory ([term][pixel], row pitch MD_LD so that phase B's reads of
+// different terms at one pixel fall in different banks) and phase B sums them over the tile's pixels into one accumulator per
+// parameter element and thread -> part[blockIdx.x][MD_SMALL].
+constexpr int MD_TERMS = 8 * 16;
+constexpr int MD_LD = MD_PIX_TILE + 1;
+__global__ void __launch_bounds__(MD_PIX_TILE)
+md_param_grad_kernel(const float* __restrict__ mask, const float* __restrict__ d_h2, const float* __restrict__ Wg, int P,
+                     float* __restrict__ part) {
+  extern __shared__ float sm[];      // [MD_TERMS][MD_LD]
+  float* s_m = sm;                   // m[s * 4 + k]
+  float* s_dy1 = sm + 16 * MD_LD;    // dL/d stage-1 conv output [c * 4 + s]
+  float* s_e1 = sm + 32 * MD_LD;     // dL/d a1 * n1
+  float* s_da1 = sm + 48 * MD_LD;    // dL/d a1 (holds a1 itself until the stage-1 backward)
+  float* s_h1 = sm + 64 * MD_LD;
+  float* s_dz = sm + 80 * MD_LD;     // dL/d stage-2 conv output
+  float* s_e2 = sm + 96 * MD_LD;
+  float* s_da2 = sm + 112 * MD_LD;
+  __shared__ float s_w[MD_SMALL];
+  const int tid = threadIdx.x;
+  for (int i = tid; i < MD_SMALL; i += MD_PIX_TILE) s_w[i] = Wg[i];
+  __syncthreads();
+  const float* W = s_w;
+  const int ntiles = P * (4096 / MD_PIX_TILE);
+  float acc[3] = {0.f, 0.f, 0.f};    // parameter elements tid, tid + 128, tid + 256 (< MD_SMALL)
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int p = tile / (4096 / MD_PIX_TILE), pix = (tile % (4096 / MD_PIX_TILE)) * MD_PIX_TILE + tid;
+    {
+      const float* mask_p = mask + (size_t)p * 65536;
+      float n1[16], rstd1[4], h1[16];
+#pragma unroll
+      for (int s = 0; s < 4; ++s) {
+        float m[4], n[4], a[4];
+        rstd1[s] = md_stage1(mask_p, pix, s, W, m, n, a);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) s_m[(s * 4 + k) * MD_LD + tid] = m[k];
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          const int j = c * 4 + s;
+          n1[j] = n[c];
+          h1[j] = md_gelu(a[c]);
+          s_h1[j * MD_LD + tid] = h1[j];
+          s_da1[j * MD_LD + tid] = a[c];
+        }
+      }
+      float dz[16];
+      {
+        float n2[16], a2[16];
+        const float rstd2 = md_stage2(h1, W, n2, a2);
+        const float* dh = d_h2 + ((size_t)p * 4096 + pix) * 16;
+        float mdn = 0.f, mdnn = 0.f;
+#pragma unroll
+        for (int o = 0; o < 16; ++o) {
+          const float da = dh[o] * md_gelu_grad(a2[o]);
+          s_da2[o * MD_LD + tid] = da;
+          s_e2[o * MD_LD + tid] = da * n2[o];
+          dz[o] = da * W[MD_G2 + o];          // dL/d n2, turned into dL/d z below
+          mdn += dz[o];
+          mdnn += dz[o] * n2[o];
+        }
+        mdn *= (1.0f / 16); mdnn *= (1.0f / 16);
+#pragma unroll
+        for (int o = 0; o < 16; ++o) {
+          dz[o] = rstd2 * (dz[o] - mdn - n2[o] * mdnn);
+          s_dz[o * MD_LD + tid] = dz[o];
+        }
+      }
+#pragma unroll 4   // fully unrolled, the 16 interleaved erf / exp evaluations need more than 255 registers
+      for (int k = 0; k < 16; ++k) {
+        float dh1 = 0.f;
+#pragma unroll
+        for (int o = 0; o < 16; ++o) dh1 += dz[o] * W[MD_W2 + o * 16 + k];
+        const float da = dh1 * md_gelu_grad(s_da1[k * MD_LD + tid]);
+        s_da1[k * MD_LD + tid] = da;
+        s_e1[k * MD_LD + tid] = da * n1[k];
+        s_dy1[k * MD_LD + tid] = da * W[MD_G1 + (k >> 2)];    // dL/d n1, turned into dL/d y1 below
+      }
+#pragma unroll
+      for (int s = 0; s < 4; ++s) {
+        float mdn1 = 0.f, mdnn1 = 0.f;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          const float dn = s_dy1[(c * 4 + s) * MD_LD + tid];
+          mdn1 += dn;
+          mdnn1 += dn * n1[c * 4 + s];
+        }
+        mdn1 *= 0.25f; mdnn1 *= 0.25f;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          float* d = s_dy1 + (c * 4 + s) * MD_LD + tid;
+          *d = rstd1[s] * (*d - mdn1 - n1[c * 4 + s] * mdnn1);
+        }
+      }
+    }
+    __syncthreads();
+#pragma unroll 1
+    for (int q = 0; q < 3; ++q) {
+      const int j = tid + q * MD_PIX_TILE;
+      if (j >= MD_SMALL) break;
+      float sum = 0.f;
+      if (j < MD_B1) {                       // W1[c][k] = sum_s dy1[c, s] m[s, k]
+        const int c = j >> 2, k = j & 3;
+#pragma unroll 4
+        for (int i = 0; i < MD_PIX_TILE; ++i)
+#pragma unroll
+          for (int s = 0; s < 4; ++s) sum += s_dy1[(c * 4 + s) * MD_LD + i] * s_m[(s * 4 + k) * MD_LD + i];
+      } else if (j < MD_W2) {                // b1 / gamma1 / beta1: sums over the 4 sub-pixels
+        const float* src = j < MD_G1 ? s_dy1 : j < MD_BE1 ? s_e1 : s_da1;
+        const int c = (j - MD_B1) & 3;
+#pragma unroll 4
+        for (int i = 0; i < MD_PIX_TILE; ++i)
+#pragma unroll
+          for (int s = 0; s < 4; ++s) sum += src[(c * 4 + s) * MD_LD + i];
+      } else if (j < MD_B2) {                // W2[o][k] = dz[o] h1[k]
+        const int o = (j - MD_W2) >> 4, k = (j - MD_W2) & 15;
+#pragma unroll 4
+        for (int i = 0; i < MD_PIX_TILE; ++i) sum += s_dz[o * MD_LD + i] * s_h1[k * MD_LD + i];
+      } else {                               // b2 / gamma2 / beta2
+        const float* src = j < MD_G2 ? s_dz : j < MD_BE2 ? s_e2 : s_da2;
+        const int o = (j - MD_B2) & 15;
+#pragma unroll 4
+        for (int i = 0; i < MD_PIX_TILE; ++i) sum += src[o * MD_LD + i];
+      }
+      acc[q] += sum;
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int q = 0; q < 3; ++q) {
+    const int j = tid + q * MD_PIX_TILE;
+    if (j < MD_SMALL) part[(size_t)blockIdx.x * MD_SMALL + j] = acc[q];
+  }
+}
+
+// grads[j] (+)= sum over the partial rows of element j, in a fixed order: one warp per element.
+__global__ void md_reduce_kernel(const float* __restrict__ part_small, int rows_small, const float* __restrict__ part_big, int rows_big,
+                                 float* __restrict__ grads, int accumulate) {
+  const int j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (j >= MD_N) return;
+  const bool small = j < MD_SMALL;
+  const float* src = small ? part_small + j : part_big + (j - MD_SMALL);
+  const int rows = small ? rows_small : rows_big;
+  const long pitch = small ? MD_SMALL : MD_BIG;
+  float s = 0.f;
+  for (int r = lane; r < rows; r += 32) s += src[(long)r * pitch];
+  s = dwarp_sum(s);
+  if (lane == 0) grads[j] = accumulate ? grads[j] + s : s;
+}
+
+inline int md_grid2(int P) { return std::min(P * (4096 / MD_PIX_TILE), MD_GRID2); }
+inline size_t md_scratch_floats(int P) {   // h2, d_h2, partials of both backward kernels
+  return (size_t)P * 4096 * 16 * 2 + (size_t)md_grid2(P) * MD_SMALL + (size_t)(4096 / 16) * MD_BIG;
+}
+struct MdScratch { float *h2, *d_h2, *part_small, *part_big; };
+inline MdScratch md_carve(float* base, int P) {
+  MdScratch s;
+  s.h2 = base;
+  s.d_h2 = s.h2 + (size_t)P * 4096 * 16;
+  s.part_small = s.d_h2 + (size_t)P * 4096 * 16;
+  s.part_big = s.part_small + (size_t)md_grid2(P) * MD_SMALL;
+  return s;
+}
+
+int md_forward(const float* mask, int P, const float* W, const float* emb_nchw, float* out, __nv_bfloat16* out_bf, const MdScratch& s,
+               cudaStream_t st) {
+  md_forward_kernel<<<dim3(4096 / 16, P), 256, 0, st>>>(mask, W, emb_nchw, out, out_bf, s.h2);
+  KCHECK("md_forward");
+  return 0;
+}
+// g = dL/d keys0 [P * 4096, 256] -> d_emb_nchw (if non-null) and the ten parameter gradients, added to (accumulate) or written over grads
+int md_backward(const float* g, const float* mask, int P, const float* W, float* d_emb_nchw, const MdScratch& s, float* grads,
+                int accumulate, cudaStream_t st) {
+  md_keys_grad_kernel<<<4096 / 16, 256, 0, st>>>(g, s.h2, W, P, d_emb_nchw, s.d_h2, s.part_big);
+  KCHECK("md_keys_grad");
+  const size_t smem = (size_t)MD_TERMS * MD_LD * 4;
+  if (cudaFuncSetAttribute(md_param_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+    return set_error("md_param_grad: shared-memory attribute failed");
+  md_param_grad_kernel<<<md_grid2(P), MD_PIX_TILE, smem, st>>>(mask, s.d_h2, W, P, s.part_small);
+  KCHECK("md_param_grad");
+  md_reduce_kernel<<<nblk((long)MD_N * 32), 256, 0, st>>>(s.part_small, md_grid2(P), s.part_big, 4096 / 16, grads, accumulate);
+  KCHECK("md_reduce");
+  return 0;
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------ data structures
@@ -225,6 +566,8 @@ struct DecSlot {
   Ten low4, iou32, keys0, tok;
   int* emb_index = nullptr;
   __nv_bfloat16* dmask8 = nullptr;
+  float* mask = nullptr;             // mask prompts [P, 256, 256] of the last forward, or null (dense prompt = no_mask_embed)
+  MdScratch md{};
   bool live = false;
 };
 
@@ -237,6 +580,11 @@ struct DecTrain {
   float *g_point_emb = nullptr, *g_nap = nullptr, *g_no_mask = nullptr, *g_out_tokens = nullptr;
   std::unordered_map<std::string, std::pair<float*, int64_t>> grads;
   DecSlot slot[8];
+  // mask_downscaling: packed fp32 masters / gradients (MD_* offsets), created by the first mask-prompt call; registered with the
+  // optimizer and the gradient table by the first masked training forward, so that runs without mask prompts never see them
+  float *md_w = nullptr, *md_g = nullptr;
+  bool md_registered = false;
+  bool md_written = false;           // a masked backward added to md_g since the last msam_decoder_zero_grads
 };
 
 namespace {
@@ -592,18 +940,83 @@ int Engine::dec_train_setup() {
   return rc;
 }
 
+namespace {
+struct MdTensor { const char* key; int off; std::initializer_list<int64_t> shape; };
+const MdTensor kMdTensors[10] = {
+    {"0.weight", MD_W1, {4, 1, 2, 2}},  {"0.bias", MD_B1, {4}},  {"1.weight", MD_G1, {4}},  {"1.bias", MD_BE1, {4}},
+    {"3.weight", MD_W2, {16, 4, 2, 2}}, {"3.bias", MD_B2, {16}}, {"4.weight", MD_G2, {16}}, {"4.bias", MD_BE2, {16}},
+    {"6.weight", MD_W3, {256, 16, 1, 1}}, {"6.bias", MD_B3, {256}}};
+const std::string kMdPrefix = "prompt_encoder.mask_downscaling.";
+int64_t md_numel(const MdTensor& t) { int64_t n = 1; for (int64_t d : t.shape) n *= d; return n; }
+}  // namespace
+
+// fp32 masters of mask_downscaling (from the host copies) and a zeroed gradient buffer; nothing is registered yet
+int Engine::md_setup() {
+  RUN(dec_train_setup());
+  DecTrain& d = *dtrain;
+  if (d.md_w) return 0;
+  std::vector<float> w(MD_N);
+  host_weights.swap(dec_host);
+  int rc = 0;
+  for (const MdTensor& t : kMdTensors) {
+    const auto* h = host(kMdPrefix + t.key, t.shape);
+    if (!h) { rc = -1; break; }
+    std::copy(h->begin(), h->end(), w.begin() + t.off);
+  }
+  host_weights.swap(dec_host);
+  if (rc) return rc;
+  CHK(d.md_w = upload_f32(w.data(), w.size()));
+  CHK(d.md_g = (float*)dalloc((size_t)MD_N * 4, true));
+  return 0;
+}
+
+// the ten tensors join the gradient table and the optimizer (after every tensor registered before); AdamW updates them only after a
+// masked backward has written their gradient since the last msam_decoder_zero_grads (torch.optim.AdamW skips a parameter whose grad
+// is None), with their own step count
+int Engine::md_register() {
+  RUN(md_setup());
+  DecTrain& d = *dtrain;
+  if (d.md_registered) return 0;
+  for (const MdTensor& t : kMdTensors) {
+    const std::string key = kMdPrefix + t.key;
+    d.grads[key] = {d.md_g + t.off, md_numel(t)};
+    OptParam p;
+    p.key = key; p.w = d.md_w + t.off; p.g = d.md_g + t.off; p.n = md_numel(t); p.written = &d.md_written;
+    opt_add(p);
+  }
+  d.md_registered = true;
+  return 0;
+}
+
+int Engine::op_mask_downscaling_train(const float* mask, int P, const float* d_dense, float* dense_out, float* grads_out,
+                                      cudaStream_t st) {
+  if (P <= 0) return set_error("msam_op_mask_downscaling_train: P = %d", P);
+  RUN(md_setup());
+  const float* W = dtrain->md_w;
+  float* scratch = nullptr;
+  if (cudaMallocAsync((void**)&scratch, md_scratch_floats(P) * 4, st) != cudaSuccess)
+    return set_error("msam_op_mask_downscaling_train: cudaMallocAsync failed");
+  const MdScratch s = md_carve(scratch, P);
+  int rc = md_forward(mask, P, W, nullptr, dense_out, nullptr, s, st);
+  if (!rc) rc = md_backward(d_dense, mask, P, W, nullptr, s, grads_out, 0, st);
+  cudaFreeAsync(scratch, st);
+  return rc;
+}
+
 // ------------------------------------------------------------------------------------------------ forward
-int Engine::decoder_train_forward(int slot, const float* emb_nchw, const float* sparse, const int* emb_index, int Ts, int P, int multimask,
-                                  float* low_res, float* iou, cudaStream_t st) {
+int Engine::decoder_train_forward(int slot, const float* emb_nchw, const float* sparse, const int* emb_index, int Ts, int P,
+                                  const float* mask_in, int multimask, float* low_res, float* iou, cudaStream_t st) {
   if (slot < 0 || slot >= 8) return set_error("decoder training: slot %d outside [0, 8)", slot);
   if (P <= 0 || Ts <= 0 || !sparse || !emb_index) return set_error("decoder training: needs sparse prompt embeddings (points and / or boxes)");
   RUN(dec_train_setup());
+  if (mask_in) RUN(md_register());
   DecTrain& d = *dtrain;
   DecSlot& s = d.slot[slot];
   const int T = 5 + Ts;
   const long Rt = (long)P * T, Ri = (long)P * 4096;
   {   // arena: ~ 110 fp32-equivalents of [P*4096, 256] cover the image-side tensors of both layers + the upscaling path
-    const size_t need = (size_t)Ri * 256 * 4 * 64 + ((size_t)64 << 20);
+    size_t need = (size_t)Ri * 256 * 4 * 64 + ((size_t)64 << 20);
+    if (mask_in) need += ((size_t)P * 65536 + md_scratch_floats(P)) * 4 + 1024;
     if (s.cap < need) {
       if (s.arena) cudaFree(s.arena);
       s.arena = nullptr; s.cap = 0;
@@ -611,7 +1024,7 @@ int Engine::decoder_train_forward(int slot, const float* emb_nchw, const float* 
       s.cap = need;
     }
   }
-  s.used = 0; s.tape.clear(); s.live = false;
+  s.used = 0; s.tape.clear(); s.live = false; s.mask = nullptr;
   s.P = P; s.T = T; s.Ts = Ts; s.nm = multimask ? 3 : 1; s.m0 = multimask ? 1 : 0;
   Ctx c{*this, d, s, st};
   s.emb_index = (int*)c.take((size_t)P * Ts * 4);
@@ -624,9 +1037,19 @@ int Engine::decoder_train_forward(int slot, const float* emb_nchw, const float* 
   assemble_tokens_kernel<<<nblk(Rt * 256), 256, 0, st>>>(d.out_tokens, sparse, P, T, Ts, tok.v);
   KCHECK("assemble_tokens");
   RUN(launch_cast_bf16(tok.v, tok.n(), tok.b, st));
-  src_broadcast_kernel<<<dim3(128, 8), dim3(32, 8), 0, st>>>(emb_nchw, d.no_mask, P, keys0.v);
-  KCHECK("src_broadcast");
-  RUN(launch_cast_bf16(keys0.v, keys0.n(), keys0.b, st));
+  if (mask_in) {   // dense prompt = mask_downscaling(mask); the mask is kept: the backward pass recomputes the stages from it
+    s.mask = (float*)c.take((size_t)P * 65536 * 4);
+    float* scratch = (float*)c.take(md_scratch_floats(P) * 4);
+    if (c.err) return -1;
+    s.md = md_carve(scratch, P);
+    if (cudaMemcpyAsync(s.mask, mask_in, (size_t)P * 65536 * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+      return set_error("decoder training: copy failed");
+    RUN(md_forward(s.mask, P, d.md_w, emb_nchw, keys0.v, keys0.b, s.md, st));
+  } else {
+    src_broadcast_kernel<<<dim3(128, 8), dim3(32, 8), 0, st>>>(emb_nchw, d.no_mask, P, keys0.v);
+    KCHECK("src_broadcast");
+    RUN(launch_cast_bf16(keys0.v, keys0.n(), keys0.b, st));
+  }
   s.tok = tok; s.keys0 = keys0;
   const float* pos = dec_pos();     // dense positional encoding, token-major [4096, 256] (no parameters)
   Ten Q = tok, K = keys0;
@@ -751,8 +1174,13 @@ int Engine::decoder_train_backward(int slot, const float* d_low_res, const float
   for (auto it = s.tape.rbegin(); it != s.tape.rend(); ++it) RUN((*it)(st));
   token_grads_kernel<<<s.T, 256, 0, st>>>(s.tok.g, s.emb_index, P, s.T, s.Ts, d.g_out_tokens, d.g_point_emb, d.g_nap);
   KCHECK("token_grads");
-  src_grad_kernel<<<dim3(128, 8), dim3(32, 8), 0, st>>>(s.keys0.g, P, d_emb_nchw, d.g_no_mask);
-  KCHECK("src_grad");
+  if (s.mask) {
+    RUN(md_backward(s.keys0.g, s.mask, P, d.md_w, d_emb_nchw, s.md, d.md_g, 1, st));
+    d.md_written = true;
+  } else {
+    src_grad_kernel<<<dim3(128, 8), dim3(32, 8), 0, st>>>(s.keys0.g, P, d_emb_nchw, d.g_no_mask);
+    KCHECK("src_grad");
+  }
   s.live = false;   // gradients of the activations are consumed: one backward per forward
   return 0;
 }
@@ -778,6 +1206,7 @@ int Engine::decoder_zero_grads(cudaStream_t st) {
   if (!dtrain) return 0;
   for (auto& kv : dtrain->grads)
     if (cudaMemsetAsync(kv.second.first, 0, (size_t)kv.second.second * 4, st) != cudaSuccess) return set_error("decoder training: memset failed");
+  dtrain->md_written = false;
   return 0;
 }
 

@@ -679,8 +679,18 @@ int msam_encoder_grad(msam_handle* h, const char* name, float* dst, int64_t n, v
 }
 int msam_decoder_train_forward(msam_handle* h, int slot, const float* emb_nchw, const float* sparse, const int32_t* emb_index, int n_sparse,
                                int P, int multimask, float* low_res, float* iou, void* stream) {
+  return msam_decoder_train_forward_ex(h, slot, emb_nchw, sparse, emb_index, n_sparse, P, nullptr, multimask, low_res, iou, stream);
+}
+int msam_decoder_train_forward_ex(msam_handle* h, int slot, const float* emb_nchw, const float* sparse, const int32_t* emb_index,
+                                  int n_sparse, int P, const float* mask_input, int multimask, float* low_res, float* iou, void* stream) {
   if (!h || !emb_nchw || !low_res || !iou) return set_error("msam_decoder_train_forward: null argument");
-  return h->eng.decoder_train_forward(slot, emb_nchw, sparse, emb_index, n_sparse, P, multimask, low_res, iou, (cudaStream_t)stream);
+  return h->eng.decoder_train_forward(slot, emb_nchw, sparse, emb_index, n_sparse, P, mask_input, multimask, low_res, iou,
+                                      (cudaStream_t)stream);
+}
+int msam_op_mask_downscaling_train(msam_handle* h, const float* mask, int P, const float* d_dense, float* dense_out, float* grads_out,
+                                   void* stream) {
+  if (!h || !mask || !d_dense || !dense_out || !grads_out) return set_error("msam_op_mask_downscaling_train: null argument");
+  return h->eng.op_mask_downscaling_train(mask, P, d_dense, dense_out, grads_out, (cudaStream_t)stream);
 }
 int msam_decoder_train_backward(msam_handle* h, int slot, const float* d_low_res, const float* d_iou, float* d_emb_nchw, void* stream) {
   if (!h || !d_emb_nchw) return set_error("msam_decoder_train_backward: null argument");

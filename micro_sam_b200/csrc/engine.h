@@ -71,6 +71,8 @@ struct OptParam {
   std::string key;              // gradient key: upstream name, or "<name>@gemm" / "@stack" for packed layouts
   float *w = nullptr, *g = nullptr, *m = nullptr, *v = nullptr;
   int64_t n = 0;
+  const bool* written = nullptr;  // non-null: AdamW skips the tensor while *written is false (no gradient since the last zeroing)
+  int64_t steps = 0;              // ... and counts its own steps for the bias correction (with written only)
   int refresh = 0;              // 0 none | 1 cast -> dst | 2 cast -> dst + transpose -> dstT | 3 rows of a rel-pos table | 4 neck 3x3 conv
                                 // relayout | 5 prompt-encoder tables of the inference decoder | 6 conv-transpose bias (fold the 4 tiles first)
   __nv_bfloat16 *dst = nullptr, *dstT = nullptr;
@@ -125,11 +127,14 @@ struct Engine {
   void dec_train_free();   // decoder_train.cu: per-slot arenas + host-side state
   // decoder_train.cu (cfg 5): mask decoder forward keeping activations (one image's prompts per call and slot) + backward
   int dec_train_setup();
-  int decoder_train_forward(int slot, const float* emb_nchw, const float* sparse, const int* emb_index, int Ts, int P, int multimask,
-                            float* low_res, float* iou, cudaStream_t st);
+  int decoder_train_forward(int slot, const float* emb_nchw, const float* sparse, const int* emb_index, int Ts, int P,
+                            const float* mask_in, int multimask, float* low_res, float* iou, cudaStream_t st);
   int decoder_train_backward(int slot, const float* d_low_res, const float* d_iou, float* d_emb_nchw, cudaStream_t st);
   int decoder_grad(const char* name, float* dst, int64_t n, cudaStream_t st);
   int decoder_zero_grads(cudaStream_t st);
+  int md_setup();      // mask_downscaling masters + gradient buffer
+  int md_register();   // ... joining the gradient table and the optimizer (first masked training forward)
+  int op_mask_downscaling_train(const float* mask, int P, const float* d_dense, float* dense_out, float* grads_out, cudaStream_t st);
   const float* dec_pos();   // decoder.cu: dense positional encoding, token-major [4096, 256] fp32
   int dec_set_prompt_tables(const float* point_emb_4x256, const float* not_a_point, cudaStream_t st);   // decoder.cu
   // train_opt.cu: AdamW over every registered tensor + refresh of the packed operands; read-out of the master weights

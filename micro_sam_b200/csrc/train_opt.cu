@@ -71,13 +71,19 @@ int Engine::optimizer_step(float lr, float b1, float b2, float eps, float wd, cu
   ++opt_step_count;
   const float c1 = 1.f - powf(b1, (float)opt_step_count), c2 = 1.f - powf(b2, (float)opt_step_count);
   for (OptParam& p : opt) {
+    float c1p = c1, c2p = c2;
+    if (p.written) {
+      if (!*p.written) continue;
+      ++p.steps;
+      c1p = 1.f - powf(b1, (float)p.steps); c2p = 1.f - powf(b2, (float)p.steps);
+    }
     if (!p.m) {
       p.m = (float*)dalloc((size_t)p.n * 4, true);
       p.v = (float*)dalloc((size_t)p.n * 4, true);
       if (!p.m || !p.v) return -1;
     }
     if (p.refresh == 6) fold4_kernel<<<(p.n / 4 + 127) / 128, 128, 0, st>>>(p.g, (int)(p.n / 4));
-    adamw_kernel<<<(unsigned)((p.n + 255) / 256), 256, 0, st>>>(p.w, p.g, p.m, p.v, p.n, lr, b1, b2, eps, wd, c1, c2);
+    adamw_kernel<<<(unsigned)((p.n + 255) / 256), 256, 0, st>>>(p.w, p.g, p.m, p.v, p.n, lr, b1, b2, eps, wd, c1p, c2p);
     count_launch();
     switch (p.refresh) {
       case 1:

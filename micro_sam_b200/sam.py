@@ -142,11 +142,12 @@ def _device_view(ptr: int, n: int, device) -> torch.Tensor:
 
 class _DecoderFn(torch.autograd.Function):
     """prompt encoder + mask decoder of ONE image with a backward pass (csrc/decoder_train.cu): (embedding [256,64,64], sparse prompt
-    embeddings [P,Ts,256]) -> (low-res logits [P,M,256,256], IoU predictions [P,M]).  backward fills / accumulates the decoder and
-    prompt-encoder parameter gradients inside the engine (`B200Sam.decoder_grads()`) and returns dL/d embedding."""
+    embeddings [P,Ts,256], mask prompts [P,1,256,256] or None) -> (low-res logits [P,M,256,256], IoU predictions [P,M]).  backward
+    fills / accumulates the decoder and prompt-encoder parameter gradients inside the engine (`B200Sam.decoder_grads()`) and returns
+    dL/d embedding (the mask prompts get no gradient)."""
 
     @staticmethod
-    def forward(ctx, emb, sparse, emb_index, sam, slot, multimask):
+    def forward(ctx, emb, sparse, emb_index, sam, slot, multimask, masks):
         emb = emb.to(device=sam.device, dtype=torch.float32).contiguous()
         sparse = sparse.to(device=sam.device, dtype=torch.float32).contiguous()
         emb_index = emb_index.to(device=sam.device, dtype=torch.int32).contiguous()
@@ -154,9 +155,10 @@ class _DecoderFn(torch.autograd.Function):
         M = 3 if multimask else 1
         low = torch.empty(P, M, 256, 256, device=sam.device, dtype=torch.float32)
         iou = torch.empty(P, M, device=sam.device, dtype=torch.float32)
-        _lib.check(_lib.lib().msam_decoder_train_forward(sam._h, slot, _lib.ptr(emb), _lib.ptr(sparse), _lib.ptr(emb_index), Ts, P,
-                                                         int(bool(multimask)), _lib.ptr(low), _lib.ptr(iou), _lib.cur_stream()))
-        ctx.sam, ctx.slot = sam, slot
+        _lib.check(_lib.lib().msam_decoder_train_forward_ex(sam._h, slot, _lib.ptr(emb), _lib.ptr(sparse), _lib.ptr(emb_index), Ts, P,
+                                                            _lib.ptr(masks), int(bool(multimask)), _lib.ptr(low), _lib.ptr(iou),
+                                                            _lib.cur_stream()))
+        ctx.sam, ctx.slot, ctx.masked = sam, slot, masks is not None
         return low, iou
 
     @staticmethod
@@ -167,7 +169,8 @@ class _DecoderFn(torch.autograd.Function):
         d_emb = torch.empty(256, 64, 64, device=sam.device, dtype=torch.float32)
         _lib.check(_lib.lib().msam_decoder_train_backward(sam._h, ctx.slot, _lib.ptr(d_low), _lib.ptr(d_iou), _lib.ptr(d_emb), _lib.cur_stream()))
         sam._decoder_grads_valid = True
-        return d_emb, None, None, None, None, None
+        sam._mask_grads_valid = sam._mask_grads_valid or ctx.masked
+        return d_emb, None, None, None, None, None, None
 
 
 class _ImageEncoder:
@@ -328,6 +331,7 @@ class B200Sam:
         self._h = ctypes.c_void_p()
         self._bound_key = self._bound_src = self._bound_tensor = None
         self._encoder_grads_valid = self._decoder_grads_valid = False   # a rebuilt engine has no training state yet
+        self._mask_grads_valid = False   # mask_downscaling joins the trained tensors with the first masked backward
         with torch.cuda.device(self.device):
             _lib.check(L.msam_create(ctypes.byref(self._cfg), self.device.index, ctypes.byref(self._h)))
             self._state = {}
@@ -373,30 +377,40 @@ class B200Sam:
 
     def train(self, mode: bool = True):
         """Training mode switches `image_encoder(x)` (under grad mode) to the activation-keeping forward with a backward pass
-        (csrc/encoder_train.cu).  The prompt encoder / mask decoder stay forward-only (DESIGN.md: decoder backward not built)."""
+        (csrc/encoder_train.cu); the prompt encoder / mask decoder are differentiated through `decoder_train`."""
         if mode and self.model_type == "vit_t":
             raise NotImplementedError("the TinyViT encoder has no backward pass")
         self.training = bool(mode)
         return self
 
-    def decoder_train(self, emb: torch.Tensor, points, boxes, multimask_output: bool, slot: int = 0):
-        """mask_decoder(prompt_encoder(points, boxes)) for ONE image in training mode: differentiable w.r.t. `emb` (256,64,64) and the
-        decoder / prompt-encoder parameters.  points = (coords (P,n,2), labels (P,n)) in the 1024 frame or None; boxes (P,4) or None."""
+    def decoder_train(self, emb: torch.Tensor, points, boxes, multimask_output: bool, slot: int = 0, masks=None):
+        """mask_decoder(prompt_encoder(points, boxes, masks)) for ONE image in training mode: differentiable w.r.t. `emb` (256,64,64)
+        and the decoder / prompt-encoder parameters.  points = (coords (P,n,2), labels (P,n)) in the 1024 frame or None; boxes (P,4)
+        or None; masks = (P,1,256,256) low-res logits used as mask prompts, or None.  The masks get no gradient, so a `masks` tensor
+        that requires grad is refused."""
         if not self.training:
             raise RuntimeError("decoder_train needs train() mode")
+        if masks is not None:
+            if masks.requires_grad:
+                raise ValueError("decoder_train: masks must not require grad (no gradient w.r.t. the mask prompts is computed)")
+            masks = masks.detach().to(self.device, torch.float32).contiguous()
         with torch.no_grad():
             sparse, _ = self.prompt_encoder(points=points, boxes=boxes, masks=None)
         P = sparse.shape[0]
+        if masks is not None and tuple(masks.shape) != (P, 1, 256, 256):
+            raise ValueError(f"decoder_train: masks must have shape ({P}, 1, 256, 256), got {tuple(masks.shape)}")
         emb_index = prompt_table_index(None if points is None else points[1], boxes is not None, P).to(self.device)
         assert emb_index.shape == sparse.shape[:2], (emb_index.shape, sparse.shape)
-        return _DecoderFn.apply(emb, sparse, emb_index, self, int(slot), bool(multimask_output))
+        return _DecoderFn.apply(emb, sparse, emb_index, self, int(slot), bool(multimask_output), masks)
 
     def zero_decoder_grads(self) -> None:
         _lib.check(_lib.lib().msam_decoder_zero_grads(self._h, _lib.cur_stream()))
+        self._decoder_zeroings = getattr(self, "_decoder_zeroings", 0) + 1
 
     def decoder_grads(self) -> Dict[str, torch.Tensor]:
         """fp32 gradients of the mask-decoder / prompt-encoder parameters accumulated since `zero_decoder_grads()`, keyed and shaped
-        like the upstream state dict (parameters the training path does not touch -- mask_downscaling, the PE matrix -- are absent)."""
+        like the upstream state dict.  The PE matrix is absent (it is not trained); mask_downscaling is present once a backward pass
+        with mask prompts has run."""
         if not getattr(self, "_decoder_grads_valid", False):
             raise RuntimeError("no decoder gradients: run decoder_train(...) and backward() first")
         return self._decoder_tensors(_lib.lib().msam_decoder_grad)
@@ -411,7 +425,7 @@ class B200Sam:
         for k, v in self._state.items():
             if not (k.startswith("mask_decoder.") or k.startswith("prompt_encoder.")):
                 continue
-            if "mask_downscaling" in k or k.endswith("positional_encoding_gaussian_matrix"):
+            if k.endswith("positional_encoding_gaussian_matrix") or ("mask_downscaling" in k and not self._mask_grads_valid):
                 continue
             if "output_upscaling.0" in k or "output_upscaling.3" in k:       # ConvTranspose2d [ci, co, 2, 2] <- GEMM layout [(dy,dx,co), ci]
                 ci, co = self._state[k.rsplit(".", 1)[0] + ".weight"].shape[:2]

@@ -8,11 +8,14 @@ minimum over the 1 / 3 predicted masks, + MSE between predicted and true IoU) fr
 `msam_mask_loss_stats` accumulates straight from the low-res logits, so the (n_obj, M, H, W) logits are only materialised
 when the caller asks for `masks`.
 
-Backward: the image encoder has one (csrc/encoder_train.cu): with `sam.train()` the embeddings returned by
-`image_embeddings_oft` are part of the autograd graph, `embeddings.backward(dL/d embeddings)` runs the encoder backward pass on
-the device and `sam.encoder_grads()` hands out one fp32 gradient per encoder parameter (upstream keys / shapes).  The prompt
-encoder / mask decoder are forward-only: `forward` runs under no_grad and the loss is a number, so dL/d embeddings has to come
-from elsewhere (DESIGN.md section 7: decoder backward not built).
+Backward: with `sam.train()` and grad mode on, every stage is differentiable.  The embeddings returned by `image_embeddings_oft`
+are part of the autograd graph (encoder backward: csrc/encoder_train.cu); `forward` runs the prompt encoder and mask decoder of
+image i in decoder slot i (csrc/decoder_train.cu; point, box and mask prompts) and `compute_loss` has an adjoint, so
+`loss.backward()` fills `sam.encoder_grads()` and `sam.decoder_grads()` (fp32, upstream keys / shapes).
+
+`compute_iterative_loss` restates `SamTrainer._compute_iterative_loss` (sam_trainer.py:243-289): several decoder passes per step,
+the later ones prompted with the previous predictions (points and / or mask logits).  Each pass is back-propagated as soon as its
+loss exists, so any number of passes fits in the one decoder slot per image.
 """
 from __future__ import annotations
 
@@ -50,7 +53,8 @@ class TrainableSAM:
                 return_masks: bool = True) -> List[Dict[str, Any]]:
         """trainable_sam.py:62-114.  `return_masks=False` skips the (n_obj, M, H, W) up-sampled logits (the loss does not need
         them: `compute_loss` works from `low_res_masks`).  In train() mode with grad enabled the outputs are part of the autograd
-        graph (point / box prompts; mask prompts are forward-only): image i of the batch uses decoder slot i."""
+        graph (point, box and `mask_inputs` prompts; the mask inputs get no gradient): image i of the batch uses decoder slot i,
+        which holds its activations until its backward pass has run."""
         if getattr(self.sam, "training", False) and torch.is_grad_enabled():
             return self._forward_train(batched_inputs, image_embeddings, multimask_output, return_masks)
         with torch.no_grad():
@@ -62,11 +66,10 @@ class TrainableSAM:
             raise ValueError("training forward: at most 8 images per call (one decoder slot per image until its backward pass has run)")
         outputs = []
         for i, (rec, emb) in enumerate(zip(batched_inputs, image_embeddings)):
-            if "mask_inputs" in rec:
-                raise NotImplementedError("mask prompts have no backward pass (DESIGN.md): train with point / box prompts")
             points = (rec["point_coords"].to(dev), rec["point_labels"].to(dev)) if "point_coords" in rec else None
             boxes = rec["boxes"].to(dev) if "boxes" in rec else None
-            low, iou = sam.decoder_train(emb, points, boxes, multimask_output, slot=i % 8)
+            masks = rec["mask_inputs"].to(dev) if "mask_inputs" in rec else None
+            low, iou = sam.decoder_train(emb, points, boxes, multimask_output, slot=i % 8, masks=masks)
             out = {"low_res_masks": low, "iou_predictions": iou, "input_size": tuple(rec["input_size"]),
                    "original_size": tuple(rec["original_size"])}
             if return_masks:
@@ -159,3 +162,74 @@ def get_best_masks(batched_outputs: List[Dict[str, Any]]):
         logits.append(low)
         masks.append(None if full is None else (full > 0.0).float())
     return (None if masks[0] is None else torch.stack(masks)), torch.stack(logits)
+
+
+class _IterativeLossFn(torch.autograd.Function):
+    """Ties the loss of `compute_iterative_loss` to the image embeddings: its backward hands the dL/d embeddings accumulated over the
+    sub-iterations to the encoder's backward pass once.  The decoder gradients were accumulated at scale 1 while the passes ran, so
+    only an upstream gradient of 1 (`loss.backward()`) keeps the two consistent, and zeroing them in between would lose them."""
+
+    @staticmethod
+    def forward(ctx, loss, image_embeddings, d_embeddings, sam, zeroings):
+        ctx.save_for_backward(d_embeddings)
+        ctx.sam, ctx.zeroings = sam, zeroings
+        return loss.clone()
+
+    @staticmethod
+    def backward(ctx, grad):
+        if float(grad) != 1.0:
+            raise ValueError(f"compute_iterative_loss: upstream gradient {float(grad)} != 1; the decoder gradients were already "
+                             "accumulated for the loss itself (scale the learning rate instead)")
+        if getattr(ctx.sam, "_decoder_zeroings", 0) != ctx.zeroings:
+            raise RuntimeError("compute_iterative_loss: zero_decoder_grads() ran after the passes and discarded their decoder "
+                               "gradients; zero them before compute_iterative_loss, not between it and loss.backward()")
+        d_emb, = ctx.saved_tensors
+        return None, d_emb, None, None, None
+
+
+def compute_iterative_loss(model: TrainableSAM, batched_inputs: List[Dict[str, Any]], y_one_hot, num_subiter: int,
+                           multimask_output: bool, update_prompts):
+    """SamTrainer._compute_iterative_loss (sam_trainer.py:243-289) -> (loss, mask_loss, iou_regression_loss, mean_model_iou),
+    each averaged over the `num_subiter` passes.  Pass 0 uses `multimask_output`, the later ones a single mask.  Between passes
+    `update_prompts(batched_inputs, masks, logits)` runs under no_grad with the best mask per object (binary full-size (B, n_obj,
+    1, H, W) and low-res logits (B, n_obj, 1, 256, 256), `get_best_masks`) and returns the records of the next pass, e.g. with
+    more points and the logits as "mask_inputs".
+
+    Training (`sam.train()` and grad mode): every pass runs the decoder on a detached copy of the embeddings and back-propagates
+    its loss / num_subiter at once, which accumulates the decoder gradients and dL/d embeddings and frees the image's decoder slot.
+    So the decoder gradients exist when this returns: call `sam.zero_decoder_grads()` BEFORE it (where the reference trainer calls
+    `optimizer.zero_grad()`), never between it and `loss.backward()` -- that backward raises if it happened.  `loss.backward()`
+    carries the summed dL/d embeddings into the encoder's backward pass, once.  The passes share nothing but the embeddings, so
+    these are the gradients of the reference's single backward through all passes.
+
+    Otherwise (validation: eval() mode or no_grad) the passes only run forward and the returned values carry no graph."""
+    sam = model.sam
+    train = bool(getattr(sam, "training", False)) and torch.is_grad_enabled()
+    image_embeddings, batched_inputs = model.image_embeddings_oft(batched_inputs)
+    d_emb = torch.zeros_like(image_embeddings, dtype=torch.float32) if train else None
+    loss = mask_loss = iou_loss = mean_iou = 0.0
+    for i in range(num_subiter):
+        last = i == num_subiter - 1
+        multimask = multimask_output if i == 0 else False
+        if train:
+            emb = image_embeddings.detach().requires_grad_(True)
+            outputs = model(batched_inputs, emb, multimask_output=multimask, return_masks=not last)
+            net_loss, net_mask_loss, net_iou_loss = compute_loss(outputs, y_one_hot)
+            (net_loss / num_subiter).backward()
+            d_emb += emb.grad
+        else:
+            with torch.no_grad():
+                outputs = model(batched_inputs, image_embeddings, multimask_output=multimask, return_masks=not last)
+                net_loss, net_mask_loss, net_iou_loss = compute_loss(outputs, y_one_hot)
+        with torch.no_grad():
+            loss = loss + net_loss.detach()
+            mask_loss = mask_loss + net_mask_loss.detach()
+            iou_loss = iou_loss + net_iou_loss.detach()
+            mean_iou = mean_iou + torch.stack([o["iou_predictions"] for o in outputs]).mean()
+            if not last:
+                masks, logits = get_best_masks(outputs)
+                batched_inputs = update_prompts(batched_inputs, masks, logits)
+    loss = loss / num_subiter
+    if train:
+        loss = _IterativeLossFn.apply(loss, image_embeddings, d_emb, sam, getattr(sam, "_decoder_zeroings", 0))
+    return loss, mask_loss / num_subiter, iou_loss / num_subiter, mean_iou / num_subiter
