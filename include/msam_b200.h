@@ -271,6 +271,30 @@ int msam_op_bgemm(const void* A, const void* B, int a_mn, int b_mn, int M, int N
 /* LayerNorm backward over fp32 rows (csrc/backward.cu); dgamma / dbeta are ACCUMULATED into (zero them first). */
 int msam_op_layernorm_bwd(const float* x, int rows, int D, const float* gamma, float eps, const float* dy, int window_mode,
                           int accumulate, float* dx, float* dgamma, float* dbeta, void* stream);
+/* Training prompts (csrc/prompts.cu).  Random draws come from Philox4x32-10 keyed by `seed`, counter (image, object, draw): the
+ * result depends on the seed and the inputs only.
+ *
+ * ConvertToSamInputs._get_prompt_lists minus the host-side id sampling (micro_sam/training/util.py:174-211,
+ * segmentation_to_one_hot and get_centers_and_bounding_boxes(mode="p")): label images [B, H, W] (label_dtype 0 int32,
+ * 1 int64), sorted ids [B, n_obj] int64 of which the first n_ids[b] (int32 [B]) are used -> uint8 one-hot targets
+ * [B, n_obj, H, W], int32 pixel counts [B, n_obj] and int32 boxes [B, n_obj, 4] (min_row, min_col, max_row + 1, max_col + 1;
+ * 0 for unused slots).  box_distortion >= 0 applies _distort_boxes with that factor; < 0 leaves the boxes as they are. */
+int msam_prompt_targets(const void* labels, int label_dtype, int B, int H, int W, const int64_t* ids, const int32_t* n_ids, int n_obj,
+                        double box_distortion, uint64_t seed, uint8_t* targets, int32_t* counts, int32_t* boxes, void* stream);
+/* PointAndBoxPromptGenerator._sample_points (micro_sam/prompt_generators.py:105-205): n = n_img * n_per_img objects, uint8 masks
+ * [n, H, W], pixel counts [n], boxes [n, 4] (row / col, exclusive max, as passed by the caller), optional int32 centres [n, 2]
+ * (row, col; NULL = none) -> int32 coords [n, n_pos + n_neg, 2] (x, y) and labels [n, n_pos + n_neg].  n_pos + n_neg <= 64.
+ * scratch: 2 * n * H * W bytes when n_neg > 0 and dilation > 0, else NULL. */
+int msam_prompt_sample_points(const uint8_t* targets, const int32_t* counts, const int32_t* boxes, const int32_t* centers, int n,
+                              int n_per_img, int H, int W, int n_pos, int n_neg, int dilation, uint64_t seed, uint8_t* scratch,
+                              int32_t* coords, int32_t* labels, void* stream);
+/* IterativePromptGenerator.__call__ for 2-D objects (micro_sam/prompt_generators.py:252-377) with SamTrainer._get_best_masks
+ * (sam_trainer.py:178-204): uint8 targets [n, H, W] and EITHER low_res [n, M, 256, 256] logits with iou [n, M] (argmax, NULL
+ * when M == 1; the prediction is Sam.postprocess_masks(low_res) > 0 for input_size (in_h, in_w), evaluated per pixel) OR a
+ * binary prediction pred [n, H, W] uint8 -> int32 coords [n, 2, 2] (x, y; positive then negative) and labels [n, 2]. */
+int msam_prompt_iterative(const uint8_t* targets, const float* low_res, const float* iou, int M, const uint8_t* pred, int n,
+                          int n_per_img, int in_h, int in_w, int orig_h, int orig_w, uint64_t seed, int32_t* coords, int32_t* labels,
+                          void* stream);
 /* debug: device buffer of 64 x 16 uint64 %globaltimer stamps written by the window-attention kernels, NULL = off */
 int msam_debug_attn_trace(void* dev_buf);
 

@@ -4,7 +4,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, c_char_p, c_float, c_int, c_int32, c_int64, c_void_p
+from ctypes import POINTER, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_uint64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libmsam_b200.so")
@@ -108,6 +108,12 @@ def lib() -> ctypes.CDLL:
         L.msam_train_tensor_count.argtypes = [c_void_p]
         L.msam_train_tensor_info.argtypes = [c_void_p, c_int, ctypes.c_char_p, c_int, POINTER(c_void_p), POINTER(c_void_p), POINTER(c_int64)]
         L.msam_mask_loss_backward.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
+        L.msam_prompt_targets.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_double, c_uint64, c_void_p,
+                                          c_void_p, c_void_p, c_void_p]
+        L.msam_prompt_sample_points.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                                c_uint64, c_void_p, c_void_p, c_void_p, c_void_p]
+        L.msam_prompt_iterative.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_uint64,
+                                            c_void_p, c_void_p, c_void_p]
         _lib = L
     return _lib
 

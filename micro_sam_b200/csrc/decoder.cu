@@ -9,6 +9,7 @@
 // image in set_image_embedding (SURVEY.md 8d).
 #include "engine.h"
 
+#include <algorithm>
 #include <cmath>
 #include <cstdlib>
 
@@ -18,6 +19,7 @@ constexpr int DC = 256;     // transformer dim
 constexpr int DI = 128;     // cross-attention internal dim
 constexpr int NHEAD = 8;
 constexpr int TMAX = 16;    // max tokens per prompt (5 output tokens + sparse prompt tokens)
+constexpr int TMAX_TRAIN = 64;   // max tokens per prompt of the prompt encoder feeding the training decoder (decoder_train.cu)
 
 struct AttnW {  // one SamAttention: q,k,v [inner, 256], out [256, inner]
   __nv_bfloat16 *q = nullptr, *k = nullptr, *v = nullptr, *o = nullptr, *qk = nullptr, *qkv = nullptr;
@@ -828,9 +830,14 @@ int Engine::prompt_encode(const float* points, const float* labels, int np, cons
   if (!finalized || !dec) return set_error("prompt_encode: decoder weights not loaded");
   DecoderState& d = *dec;
   const int n_sparse = (points ? np + (boxes ? 0 : 1) : 0) + (boxes ? 2 : 0), T = 5 + n_sparse;
-  if (T > TMAX) return set_error("prompt_encode: %d tokens per prompt exceeds the supported %d", T, TMAX);
-  for (int p0 = 0; p0 < P; p0 += cfg.max_prompts) {
-    const int n = (P - p0 < cfg.max_prompts) ? (P - p0) : cfg.max_prompts;
+  // The encoder itself has no token limit: prompts with more than TMAX tokens (the limit of the inference decoder; the training
+  // decoder takes up to TMAX_TRAIN) are encoded in chunks of fewer prompts so that chunk * T tokens fit the max_prompts * TMAX
+  // token workspace.
+  if (T > TMAX_TRAIN || T > cfg.max_prompts * TMAX)
+    return set_error("prompt_encode: %d tokens per prompt exceeds the supported %d", T, std::min(TMAX_TRAIN, cfg.max_prompts * TMAX));
+  const int chunk = T <= TMAX ? cfg.max_prompts : cfg.max_prompts * TMAX / T;
+  for (int p0 = 0; p0 < P; p0 += chunk) {
+    const int n = (P - p0 < chunk) ? (P - p0) : chunk;
     if (n_sparse > 0) {
       if (!sparse_out) return set_error("prompt_encode: sparse_out is null");
       prompt_tokens_kernel<<<dim3(n_sparse, n), 128, 0, st>>>(points ? points + (size_t)p0 * np * 2 : nullptr,

@@ -1008,6 +1008,7 @@ int Engine::decoder_train_forward(int slot, const float* emb_nchw, const float* 
                                   const float* mask_in, int multimask, float* low_res, float* iou, cudaStream_t st) {
   if (slot < 0 || slot >= 8) return set_error("decoder training: slot %d outside [0, 8)", slot);
   if (P <= 0 || Ts <= 0 || !sparse || !emb_index) return set_error("decoder training: needs sparse prompt embeddings (points and / or boxes)");
+  if (5 + Ts > 64) return set_error("decoder training: %d tokens per prompt exceeds the supported 64", 5 + Ts);
   RUN(dec_train_setup());
   if (mask_in) RUN(md_register());
   DecTrain& d = *dtrain;

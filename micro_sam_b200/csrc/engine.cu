@@ -572,6 +572,25 @@ int msam_mask_loss_stats(const float* low_res, const uint8_t* targets, int n_obj
   if (!low_res || !targets || !out5) return set_error("msam_mask_loss_stats: null argument");
   return post_mask_loss_stats(low_res, targets, n_obj, M, in_h, in_w, orig_h, orig_w, out5, (cudaStream_t)stream);
 }
+int msam_prompt_targets(const void* labels, int label_dtype, int B, int H, int W, const int64_t* ids, const int32_t* n_ids, int n_obj,
+                        double box_distortion, uint64_t seed, uint8_t* targets, int32_t* counts, int32_t* boxes, void* stream) {
+  if (!labels || !ids || !n_ids || !targets || !counts || !boxes) return set_error("msam_prompt_targets: null argument");
+  return prompt_targets(labels, label_dtype, B, H, W, ids, n_ids, n_obj, box_distortion, seed, targets, counts, boxes, (cudaStream_t)stream);
+}
+int msam_prompt_sample_points(const uint8_t* targets, const int32_t* counts, const int32_t* boxes, const int32_t* centers, int n,
+                              int n_per_img, int H, int W, int n_pos, int n_neg, int dilation, uint64_t seed, uint8_t* scratch,
+                              int32_t* coords, int32_t* labels, void* stream) {
+  if (!targets || !counts || !boxes || !coords || !labels) return set_error("msam_prompt_sample_points: null argument");
+  return prompt_sample_points(targets, counts, boxes, centers, n, n_per_img, H, W, n_pos, n_neg, dilation, seed, scratch, coords, labels,
+                              (cudaStream_t)stream);
+}
+int msam_prompt_iterative(const uint8_t* targets, const float* low_res, const float* iou, int M, const uint8_t* pred, int n,
+                          int n_per_img, int in_h, int in_w, int orig_h, int orig_w, uint64_t seed, int32_t* coords, int32_t* labels,
+                          void* stream) {
+  if (!targets || !coords || !labels) return set_error("msam_prompt_iterative: null argument");
+  return prompt_iterative(targets, low_res, iou, M, pred, n, n_per_img, in_h, in_w, orig_h, orig_w, seed, coords, labels,
+                          (cudaStream_t)stream);
+}
 int msam_to_image(const void* src, int dtype, int h, int w, int c, uint8_t* out_hwc3, uint32_t* scratch6, void* stream) {
   return post_to_image(src, dtype, h, w, c, out_hwc3, scratch6, (cudaStream_t)stream);
 }

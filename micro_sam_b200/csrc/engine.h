@@ -194,4 +194,13 @@ int post_filter_nms(const int32_t* boxes, const float* scores, const float* stab
                     float stab_thresh, float nms_thresh, const int32_t* crop_box, const int32_t* orig_box, int32_t* keep,
                     int32_t* n_keep, cudaStream_t st);
 
+// ---- prompts.cu: training prompts from label images and predictions (micro_sam/prompt_generators.py)
+int prompt_targets(const void* labels, int label_dtype, int B, int H, int W, const int64_t* ids, const int32_t* n_ids, int n_obj,
+                   double box_distortion, uint64_t seed, uint8_t* targets, int32_t* counts, int32_t* boxes, cudaStream_t st);
+int prompt_sample_points(const uint8_t* targets, const int32_t* counts, const int32_t* boxes, const int32_t* centers, int n, int n_per_img,
+                         int H, int W, int n_pos, int n_neg, int dilation, uint64_t seed, uint8_t* scratch, int32_t* coords,
+                         int32_t* labels, cudaStream_t st);
+int prompt_iterative(const uint8_t* targets, const float* low_res, const float* iou, int M, const uint8_t* pred, int n, int n_per_img,
+                     int in_h, int in_w, int H, int W, uint64_t seed, int32_t* coords, int32_t* labels, cudaStream_t st);
+
 }  // namespace msam

@@ -9,6 +9,7 @@ runs in the hand-written sm_90a kernels.  There is no PyTorch fallback: without 
 from __future__ import annotations
 
 import ctypes
+import types
 from typing import Dict, Optional, Tuple
 
 import numpy as np
@@ -402,6 +403,17 @@ class B200Sam:
         emb_index = prompt_table_index(None if points is None else points[1], boxes is not None, P).to(self.device)
         assert emb_index.shape == sparse.shape[:2], (emb_index.shape, sparse.shape)
         return _DecoderFn.apply(emb, sparse, emb_index, self, int(slot), bool(multimask_output), masks)
+
+    def decode_with_training_decoder(self, emb: torch.Tensor, points, boxes, multimask_output: bool, slot: int = 0, masks=None):
+        """Forward pass only of `decoder_train` (no autograd record, any mode): the inference decoder takes at most 16 tokens per
+        prompt, the training decoder up to 64, so prompts with more tokens (e.g. the later passes of iterative prompting) are decoded
+        here.  Uses decoder slot `slot` like `decoder_train` (a pending backward pass of that slot is lost)."""
+        with torch.no_grad():
+            if masks is not None:
+                masks = masks.detach().to(self.device, torch.float32).contiguous()
+            sparse, _ = self.prompt_encoder(points=points, boxes=boxes, masks=None)
+            emb_index = prompt_table_index(None if points is None else points[1], boxes is not None, sparse.shape[0]).to(self.device)
+            return _DecoderFn.forward(types.SimpleNamespace(), emb.detach(), sparse, emb_index, self, int(slot), bool(multimask_output), masks)
 
     def zero_decoder_grads(self) -> None:
         _lib.check(_lib.lib().msam_decoder_zero_grads(self._h, _lib.cur_stream()))
