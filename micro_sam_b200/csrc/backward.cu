@@ -329,6 +329,17 @@ __global__ void cast_f32_kernel(const uint2* __restrict__ x, long n4, float4* __
   out[i] = make_float4(blo(u.x), bhi(u.x), blo(u.y), bhi(u.y));
 }
 
+// out [cols, rows] = in [rows, cols]^T in 32 x 32 tiles through shared memory; block = (32, 8)
+__global__ void transpose_bf16_kernel(const __nv_bfloat16* __restrict__ in, int rows, int cols, __nv_bfloat16* __restrict__ out) {
+  __shared__ __nv_bfloat16 tile[32][34];
+  const int r0 = blockIdx.y * 32, c0 = blockIdx.x * 32;
+  for (int i = threadIdx.y; i < 32; i += blockDim.y)
+    if (r0 + i < rows && c0 + threadIdx.x < cols) tile[i][threadIdx.x] = in[(long)(r0 + i) * cols + c0 + threadIdx.x];
+  __syncthreads();
+  for (int i = threadIdx.y; i < 32; i += blockDim.y)
+    if (c0 + i < cols && r0 + threadIdx.x < rows) out[(long)(c0 + i) * rows + r0 + threadIdx.x] = tile[threadIdx.x][i];
+}
+
 }  // namespace
 
 int launch_layernorm_bwd(const float* x, int rows, int D, const float* gamma, float eps, const float* dy, int window_mode, int grid,
@@ -417,6 +428,11 @@ int launch_cast_f32(const __nv_bfloat16* x, long n, float* out, cudaStream_t str
   if (n % 4) return set_error("cast: n must be a multiple of 4");
   cast_f32_kernel<<<(unsigned)((n / 4 + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const uint2*>(x), n / 4, reinterpret_cast<float4*>(out));
   BWD_CHECK("cast_f32");
+  return 0;
+}
+int launch_transpose_bf16(const __nv_bfloat16* in, int rows, int cols, __nv_bfloat16* out, cudaStream_t stream) {
+  transpose_bf16_kernel<<<dim3((cols + 31) / 32, (rows + 31) / 32), dim3(32, 8), 0, stream>>>(in, rows, cols, out);
+  BWD_CHECK("transpose");
   return 0;
 }
 

@@ -190,15 +190,6 @@ __global__ void masks_grad_kernel(const float* __restrict__ d_low, int P, int nm
   for (int m = 0; m < nm; ++m) v[m0 + m] = d_low[((p * nm + m) * 256 + Y) * 256 + X];
   *reinterpret_cast<uint4*>(out8 + (p * 65536 + up_row(Y, X)) * 8) = make_uint4(dpk2(v[0], v[1]), dpk2(v[2], v[3]), dpk2(v[4], v[5]), dpk2(v[6], v[7]));
 }
-__global__ void transpose_bf16_dk(const __nv_bfloat16* __restrict__ in, int rows, int cols, __nv_bfloat16* __restrict__ out) {
-  __shared__ __nv_bfloat16 tile[32][34];
-  const int r0 = blockIdx.y * 32, c0 = blockIdx.x * 32;
-  for (int i = threadIdx.y; i < 32; i += blockDim.y)
-    if (r0 + i < rows && c0 + threadIdx.x < cols) tile[i][threadIdx.x] = in[(long)(r0 + i) * cols + c0 + threadIdx.x];
-  __syncthreads();
-  for (int i = threadIdx.y; i < 32; i += blockDim.y)
-    if (c0 + i < cols && r0 + threadIdx.x < rows) out[(long)(c0 + i) * rows + r0 + threadIdx.x] = tile[threadIdx.x][i];
-}
 
 inline unsigned nblk(long n, int per = 256) { return (unsigned)((n + per - 1) / per); }
 
@@ -806,7 +797,7 @@ static int dt_lin(Engine& e, DecTrain& d, const std::string& key, int out, int i
   L->out = op; L->in = in;
   CHK(L->w = e.upload_bf16(wp.data(), wp.size()));
   CHK(L->wT = (__nv_bfloat16*)e.dalloc((size_t)op * in * 2));
-  transpose_bf16_dk<<<dim3((in + 31) / 32, (op + 31) / 32), dim3(32, 8)>>>(L->w, op, in, L->wT);
+  RUN(launch_transpose_bf16(L->w, op, in, L->wT, 0));
   CHK(L->bias = e.upload_f32(bp.data(), bp.size()));
   CHK(L->gw = (float*)e.dalloc((size_t)op * in * 4, true));
   CHK(L->gb = (float*)e.dalloc((size_t)op * 4, true));
@@ -814,7 +805,7 @@ static int dt_lin(Engine& e, DecTrain& d, const std::string& key, int out, int i
   d.grads[key + ".bias"] = {L->gb, op};
   OptParam pw, pb;
   pw.key = key + ".weight"; CHK(pw.w = e.upload_f32(wp.data(), wp.size())); pw.g = L->gw; pw.n = (int64_t)op * in;
-  pw.refresh = 2; pw.dst = L->w; pw.dstT = L->wT; pw.rows = op; pw.cols = in;
+  pw.refresh = 1; pw.dst = L->w; pw.dstT = L->wT; pw.rows = op; pw.cols = in;
   pb.key = key + ".bias"; pb.w = L->bias; pb.g = L->gb; pb.n = op;
   e.opt_add(pw); e.opt_add(pb);
   return 0;
@@ -855,7 +846,7 @@ static int dt_convT(Engine& e, DecTrain& d, const std::string& key, int ci, int 
   L->out = 4 * co; L->in = ci;
   CHK(L->w = e.upload_bf16(wg.data(), wg.size()));
   CHK(L->wT = (__nv_bfloat16*)e.dalloc(wg.size() * 2));
-  transpose_bf16_dk<<<dim3((ci + 31) / 32, (4 * co + 31) / 32), dim3(32, 8)>>>(L->w, 4 * co, ci, L->wT);
+  RUN(launch_transpose_bf16(L->w, 4 * co, ci, L->wT, 0));
   CHK(L->bias = e.upload_f32(bg.data(), bg.size()));
   CHK(L->gw = (float*)e.dalloc(wg.size() * 4, true));
   CHK(L->gb = (float*)e.dalloc(bg.size() * 4, true));
@@ -863,7 +854,7 @@ static int dt_convT(Engine& e, DecTrain& d, const std::string& key, int ci, int 
   d.grads[key + ".bias@gemm"] = {L->gb, (int64_t)bg.size()};
   OptParam pw, pb;
   pw.key = key + ".weight@gemm"; CHK(pw.w = e.upload_f32(wg.data(), wg.size())); pw.g = L->gw; pw.n = (int64_t)wg.size();
-  pw.refresh = 2; pw.dst = L->w; pw.dstT = L->wT; pw.rows = 4 * co; pw.cols = ci;
+  pw.refresh = 1; pw.dst = L->w; pw.dstT = L->wT; pw.rows = 4 * co; pw.cols = ci;
   pb.key = key + ".bias@gemm"; pb.w = L->bias; pb.g = L->gb; pb.n = (int64_t)bg.size(); pb.refresh = 6;
   e.opt_add(pw); e.opt_add(pb);
   return 0;

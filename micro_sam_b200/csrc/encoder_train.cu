@@ -7,8 +7,9 @@
 // GELU(fc1) are recomputed (HBM-bound, cheaper than keeping them).  Per block, in reverse:
 //   MLP    dW2 = dy^T h | dh = dy W2 | dpre = dh o gelu'(pre) | dW1 = dpre^T LN2(x_mid) | dxn = dpre W1 | dx += LN2'(dxn)
 //   attn   dWp = dy^T a | da = dy Wp | (dq, dk, dv, drel) = attention'(qkv, da) | dWqkv = dqkv^T LN1(x_in) | dxn = dqkv Wqkv | dx += LN1'(dxn)
+// The forward pass is Engine::vit_forward (engine.cu), the inference forward with those activations kept.
 // dgrad products use the forward wgmma GEMMs on weights transposed once per weight update (W^T as the K-major operand: the
-// GEMM of gemm.cu and its epilogues apply), wgrad products the MN-major GEMM of gemm_tn.cu, the five attention products the batched
+// GEMM of gemm.cu and its epilogues apply; built here at setup and rebuilt by optimizer_step), wgrad products the MN-major GEMM of gemm_tn.cu, the five attention products the batched
 // GEMM of bgemm.cu (one launch per product for all windows / images and heads), with S / P / dS materialised in HBM per block
 // (window blocks: 0.1 GB, global blocks: 0.07 GB per image and head).  Gradients are fp32, operands bf16.
 #include "engine.h"
@@ -23,23 +24,6 @@ namespace msam {
 
 namespace {
 
-__global__ void transpose_bf16_kernel(const __nv_bfloat16* __restrict__ in, int rows, int cols, __nv_bfloat16* __restrict__ out) {
-  __shared__ __nv_bfloat16 tile[32][34];
-  const int r0 = blockIdx.y * 32, c0 = blockIdx.x * 32;
-  for (int i = threadIdx.y; i < 32; i += blockDim.y)
-    if (r0 + i < rows && c0 + threadIdx.x < cols) tile[i][threadIdx.x] = in[(long)(r0 + i) * cols + c0 + threadIdx.x];
-  __syncthreads();
-  for (int i = threadIdx.y; i < 32; i += blockDim.y)
-    if (c0 + i < cols && r0 + threadIdx.x < rows) out[(long)(c0 + i) * rows + r0 + threadIdx.x] = tile[threadIdx.x][i];
-}
-
-int transpose_bf16(const __nv_bfloat16* in, int rows, int cols, __nv_bfloat16* out, cudaStream_t st) {
-  transpose_bf16_kernel<<<dim3((cols + 31) / 32, (rows + 31) / 32), dim3(32, 8), 0, st>>>(in, rows, cols, out);
-  if (cudaGetLastError() != cudaSuccess) return set_error("transpose launch failed");
-  count_launch();
-  return 0;
-}
-
 // [o][k][c] (GEMM operand of the 3x3 neck conv) gradient -> upstream [o][c][k]
 __global__ void neck2_grad_relayout_kernel(const float* __restrict__ g, int C, float* __restrict__ out) {
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -51,8 +35,6 @@ __global__ void neck2_grad_relayout_kernel(const float* __restrict__ g, int C, f
 }  // namespace
 
 struct TrainSave {
-  float *x_in = nullptr, *x_mid = nullptr;
-  __nv_bfloat16 *qkv = nullptr, *attn = nullptr, *pre = nullptr;
   __nv_bfloat16 *qkv_wT = nullptr, *proj_wT = nullptr, *fc1_wT = nullptr, *fc2_wT = nullptr;
   float *g_ln1_g = nullptr, *g_ln1_b = nullptr, *g_ln2_g = nullptr, *g_ln2_b = nullptr, *g_qkv_w = nullptr, *g_qkv_b = nullptr,
         *g_proj_w = nullptr, *g_proj_b = nullptr, *g_fc1_w = nullptr, *g_fc1_b = nullptr, *g_fc2_w = nullptr, *g_fc2_b = nullptr,
@@ -61,7 +43,7 @@ struct TrainSave {
 
 struct TrainState {
   int B = 0;                 // batch of the saved forward pass (0 = none)
-  bool transposed = false;
+  std::vector<VitBlockActs> acts;
   std::vector<TrainSave> blk;
   __nv_bfloat16 *neck1_wT = nullptr, *neck2_wT = nullptr;
   float *g_patch_w = nullptr, *g_patch_b = nullptr, *g_pos = nullptr, *g_neck1_w = nullptr, *g_neck_ln1_g = nullptr, *g_neck_ln1_b = nullptr,
@@ -81,7 +63,7 @@ static float* galloc(Engine& e, TrainState& t, const std::string& name, int64_t 
   return p;
 }
 
-int Engine::train_setup() {
+int Engine::train_setup(cudaStream_t st) {
   if (train) return 0;
   if (is_tinyvit()) return set_error("training mode: the TinyViT encoder has no backward pass");
   train = new TrainState();
@@ -90,17 +72,28 @@ int Engine::train_setup() {
   const int wpr = (g + cfg.window_size - 1) / cfg.window_size;
   const size_t Tw = (size_t)wpr * wpr * cfg.window_size * cfg.window_size, M = (size_t)B * T, Mq = (size_t)B * Tw;
   const std::string e = "image_encoder.";
+  t.acts.resize(cfg.depth);
   t.blk.resize(cfg.depth);
+  // optimizer registry (train_opt.cu): fp32 parameters are updated in place, bf16 operands (and their W^T) from fp32 masters
+  auto inplace = [&](const std::string& k, float* w, float* g, int64_t n) { OptParam q; q.key = k; q.w = w; q.g = g; q.n = n; opt_add(q); };
+  auto casted = [&](const std::string& k, float* g, __nv_bfloat16* dst, int rows, int cols, __nv_bfloat16* dstT, int refresh = 1) -> int {
+    OptParam q; q.key = k; q.g = g; q.n = (int64_t)rows * cols; q.refresh = refresh; q.dst = dst; q.dstT = dstT; q.rows = rows; q.cols = cols;
+    CHK(q.w = opt_master_from_host(k, q.n));
+    opt_add(q);
+    return dstT ? launch_transpose_bf16(dst, rows, cols, dstT, st) : 0;
+  };
   for (int i = 0; i < cfg.depth; ++i) {
+    VitBlockActs& a = t.acts[i];
     TrainSave& s = t.blk[i];
     const bool glob = enc.blocks[i].global;
-    const int S = glob ? g : cfg.window_size;
+    const AttnBwdGeom geo = rel_table_geom(glob, cfg.window_size, g);
+    const int S = geo.side;
     const std::string p = e + "blocks." + std::to_string(i) + ".";
-    CHK(s.x_in = (float*)dalloc(M * D * 4));
-    CHK(s.x_mid = (float*)dalloc(M * D * 4));
-    CHK(s.qkv = (__nv_bfloat16*)dalloc((glob ? M : Mq) * 3 * D * 2));
-    CHK(s.attn = (__nv_bfloat16*)dalloc(M * D * 2));
-    CHK(s.pre = (__nv_bfloat16*)dalloc(M * 4 * D * 2));
+    CHK(a.x_in = (float*)dalloc(M * D * 4));
+    CHK(a.x_mid = (float*)dalloc(M * D * 4));
+    CHK(a.qkv = (__nv_bfloat16*)dalloc((glob ? M : Mq) * 3 * D * 2));
+    CHK(a.attn = (__nv_bfloat16*)dalloc(M * D * 2));
+    CHK(a.pre = (__nv_bfloat16*)dalloc(M * 4 * D * 2));
     CHK(s.qkv_wT = (__nv_bfloat16*)dalloc((size_t)3 * D * D * 2));
     CHK(s.proj_wT = (__nv_bfloat16*)dalloc((size_t)D * D * 2));
     CHK(s.fc1_wT = (__nv_bfloat16*)dalloc((size_t)4 * D * D * 2));
@@ -119,25 +112,17 @@ int Engine::train_setup() {
     CHK(s.g_fc2_b = galloc(*this, t, p + "mlp.lin2.bias", D));
     CHK(s.g_rel_h = galloc(*this, t, p + "attn.rel_pos_h", (int64_t)(2 * S - 1) * hd));
     CHK(s.g_rel_w = galloc(*this, t, p + "attn.rel_pos_w", (int64_t)(2 * S - 1) * hd));
-    // optimizer registry (train_opt.cu): fp32 parameters are updated in place, bf16 operands from fp32 masters
     EncBlock& b = enc.blocks[i];
-    auto inplace = [&](const std::string& k, float* w, float* g, int64_t n) { OptParam q; q.key = k; q.w = w; q.g = g; q.n = n; opt_add(q); };
-    auto casted = [&](const std::string& k, float* g, int64_t n, __nv_bfloat16* dst) -> int {
-      OptParam q; q.key = k; q.g = g; q.n = n; q.refresh = 1; q.dst = dst;
-      CHK(q.w = opt_master_from_host(k, n));
-      opt_add(q);
-      return 0;
-    };
     inplace(p + "norm1.weight", b.ln1_g, s.g_ln1_g, D); inplace(p + "norm1.bias", b.ln1_b, s.g_ln1_b, D);
     inplace(p + "norm2.weight", b.ln2_g, s.g_ln2_g, D); inplace(p + "norm2.bias", b.ln2_b, s.g_ln2_b, D);
-    RUN(casted(p + "attn.qkv.weight", s.g_qkv_w, (int64_t)3 * D * D, b.qkv_w)); inplace(p + "attn.qkv.bias", b.qkv_b, s.g_qkv_b, 3 * D);
-    RUN(casted(p + "attn.proj.weight", s.g_proj_w, (int64_t)D * D, b.proj_w)); inplace(p + "attn.proj.bias", b.proj_b, s.g_proj_b, D);
-    RUN(casted(p + "mlp.lin1.weight", s.g_fc1_w, (int64_t)4 * D * D, b.fc1_w)); inplace(p + "mlp.lin1.bias", b.fc1_b, s.g_fc1_b, 4 * D);
-    RUN(casted(p + "mlp.lin2.weight", s.g_fc2_w, (int64_t)4 * D * D, b.fc2_w)); inplace(p + "mlp.lin2.bias", b.fc2_b, s.g_fc2_b, D);
+    RUN(casted(p + "attn.qkv.weight", s.g_qkv_w, b.qkv_w, 3 * D, D, s.qkv_wT)); inplace(p + "attn.qkv.bias", b.qkv_b, s.g_qkv_b, 3 * D);
+    RUN(casted(p + "attn.proj.weight", s.g_proj_w, b.proj_w, D, D, s.proj_wT)); inplace(p + "attn.proj.bias", b.proj_b, s.g_proj_b, D);
+    RUN(casted(p + "mlp.lin1.weight", s.g_fc1_w, b.fc1_w, 4 * D, D, s.fc1_wT)); inplace(p + "mlp.lin1.bias", b.fc1_b, s.g_fc1_b, 4 * D);
+    RUN(casted(p + "mlp.lin2.weight", s.g_fc2_w, b.fc2_w, D, 4 * D, s.fc2_wT)); inplace(p + "mlp.lin2.bias", b.fc2_b, s.g_fc2_b, D);
     for (int hw = 0; hw < 2; ++hw) {
       OptParam q;
       q.key = p + (hw ? "attn.rel_pos_w" : "attn.rel_pos_h"); q.g = hw ? s.g_rel_w : s.g_rel_h; q.n = (int64_t)(2 * S - 1) * hd;
-      q.refresh = 3; q.dst = b.rel_table; q.rows = 2 * S - 1; q.cols = hd; q.cols_pad = ((hd + 63) / 64) * 64; q.row_off = hw ? (glob ? 128 : 32) : 0;
+      q.refresh = 3; q.dst = b.rel_table; q.rows = 2 * S - 1; q.cols = hd; q.cols_pad = rel_table_cols(hd); q.row_off = hw ? geo.woff : 0;
       CHK(q.w = opt_master_from_host(q.key, q.n));
       opt_add(q);
     }
@@ -154,20 +139,13 @@ int Engine::train_setup() {
   CHK(t.g_neck2_w_up = galloc(*this, t, e + "neck.2.weight", (int64_t)9 * C * C));
   CHK(t.g_neck_ln2_g = galloc(*this, t, e + "neck.3.weight", C));
   CHK(t.g_neck_ln2_b = galloc(*this, t, e + "neck.3.bias", C));
-  {
-    auto inplace = [&](const std::string& k, float* w, float* g, int64_t n) { OptParam q; q.key = k; q.w = w; q.g = g; q.n = n; opt_add(q); };
-    OptParam q;
-    q.key = e + "patch_embed.proj.weight"; q.g = t.g_patch_w; q.n = (int64_t)D * 768; q.refresh = 1; q.dst = enc.patch_w;
-    CHK(q.w = opt_master_from_host(q.key, q.n)); opt_add(q);
-    inplace(e + "patch_embed.proj.bias", enc.patch_b, t.g_patch_b, D);
-    inplace(e + "pos_embed", enc.pos_embed, t.g_pos, (int64_t)T * D);
-    q = OptParam(); q.key = e + "neck.0.weight"; q.g = t.g_neck1_w; q.n = (int64_t)C * D; q.refresh = 1; q.dst = enc.neck_conv1;
-    CHK(q.w = opt_master_from_host(q.key, q.n)); opt_add(q);
-    inplace(e + "neck.1.weight", enc.neck_ln1_g, t.g_neck_ln1_g, C); inplace(e + "neck.1.bias", enc.neck_ln1_b, t.g_neck_ln1_b, C);
-    q = OptParam(); q.key = e + "neck.2.weight"; q.g = t.g_neck2_w_up; q.n = (int64_t)9 * C * C; q.refresh = 4; q.dst = enc.neck_conv2; q.rows = C;
-    CHK(q.w = opt_master_from_host(q.key, q.n)); opt_add(q);
-    inplace(e + "neck.3.weight", enc.neck_ln2_g, t.g_neck_ln2_g, C); inplace(e + "neck.3.bias", enc.neck_ln2_b, t.g_neck_ln2_b, C);
-  }
+  RUN(casted(e + "patch_embed.proj.weight", t.g_patch_w, enc.patch_w, D, 768, nullptr));
+  inplace(e + "patch_embed.proj.bias", enc.patch_b, t.g_patch_b, D);
+  inplace(e + "pos_embed", enc.pos_embed, t.g_pos, (int64_t)T * D);
+  RUN(casted(e + "neck.0.weight", t.g_neck1_w, enc.neck_conv1, C, D, t.neck1_wT));
+  inplace(e + "neck.1.weight", enc.neck_ln1_g, t.g_neck_ln1_g, C); inplace(e + "neck.1.bias", enc.neck_ln1_b, t.g_neck_ln1_b, C);
+  RUN(casted(e + "neck.2.weight", t.g_neck2_w_up, enc.neck_conv2, C, 9 * C, t.neck2_wT, 4));   // refresh 4 reads rows = C
+  inplace(e + "neck.3.weight", enc.neck_ln2_g, t.g_neck_ln2_g, C); inplace(e + "neck.3.bias", enc.neck_ln2_b, t.g_neck_ln2_b, C);
   // scratch
   const size_t Dm = D > C ? D : C;
   CHK(t.dx = (float*)dalloc(M * Dm * 4));
@@ -201,97 +179,9 @@ int Engine::train_setup() {
 int Engine::encode_train(const float* f32, int B, float* out, cudaStream_t st) {
   if (!finalized) return set_error("msam_encode_train: weights not finalized");
   if (B <= 0 || B > cfg.max_batch) return set_error("msam_encode_train: batch %d outside [1, max_batch = %d]", B, cfg.max_batch);
-  RUN(train_setup());
-  TrainState& t = *train;
-  const int D = cfg.embed_dim, hd = D / cfg.num_heads, g = cfg.image_size / cfg.patch_size, T = g * g, C = cfg.out_chans;
-  const int wpr = (g + cfg.window_size - 1) / cfg.window_size;
-  const int Tw = wpr * wpr * cfg.window_size * cfg.window_size;
-  const int M = B * T;
-  static const float mean[3] = {123.675f, 116.28f, 103.53f}, stdv[3] = {58.395f, 57.12f, 57.375f};
-  if (!t.transposed) {   // W^T operands of the dgrad GEMMs (again after every weight update: msam_finalize_weights resets this)
-    for (int i = 0; i < cfg.depth; ++i) {
-      const EncBlock& b = enc.blocks[i];
-      TrainSave& s = t.blk[i];
-      RUN(transpose_bf16(b.qkv_w, 3 * D, D, s.qkv_wT, st));
-      RUN(transpose_bf16(b.proj_w, D, D, s.proj_wT, st));
-      RUN(transpose_bf16(b.fc1_w, 4 * D, D, s.fc1_wT, st));
-      RUN(transpose_bf16(b.fc2_w, D, 4 * D, s.fc2_wT, st));
-    }
-    RUN(transpose_bf16(enc.neck_conv1, C, D, t.neck1_wT, st));
-    RUN(transpose_bf16(enc.neck_conv2, C, 9 * C, t.neck2_wT, st));
-    t.transposed = true;
-  }
-  RUN(launch_patchify(nullptr, f32, B, cfg.image_size, cfg.image_size, cfg.image_size, mean, stdv, ws.patches, st));
-  {
-    GemmArgs a;
-    a.A = ws.patches; a.W = enc.patch_w; a.M = M; a.N = D; a.K = 768; a.lda = 768; a.ldw = 768;
-    a.bias = enc.patch_b; a.residual = enc.pos_embed; a.res_rows = T; a.out = ws.x; a.out_fp32 = 1;
-    RUN(launch_gemm(a, num_sms, st));
-  }
-  for (int i = 0; i < cfg.depth; ++i) {
-    const EncBlock& b = enc.blocks[i];
-    TrainSave& s = t.blk[i];
-    if (cudaMemcpyAsync(s.x_in, ws.x, (size_t)M * D * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess) return set_error("encode_train: copy failed");
-    LnArgs l;
-    l.x = ws.x; l.rows = M; l.D = D; l.gamma = b.ln1_g; l.beta = b.ln1_b; l.eps = 1e-6f; l.grid = g; l.ws = cfg.window_size;
-    if (b.global) { l.out = ws.xn; } else { l.out = ws.xn_win; l.window_mode = 1; }
-    RUN(launch_layernorm(l, st));
-    const int Mq = b.global ? M : B * Tw;
-    {
-      GemmArgs a;
-      a.A = b.global ? ws.xn : ws.xn_win; a.W = b.qkv_w; a.M = Mq; a.N = 3 * D; a.K = D; a.lda = D; a.ldw = D;
-      a.bias = b.qkv_b; a.out = s.qkv;
-      RUN(launch_gemm(a, num_sms, st));
-    }
-    {
-      AttnArgs a;
-      a.qkv = s.qkv; a.rel_table = b.rel_table; a.out = s.attn; a.batch = B; a.heads = cfg.num_heads;
-      a.head_dim = hd; a.grid = g; a.window = b.global ? 0 : cfg.window_size; a.scale = 1.0f / sqrtf((float)hd);
-      RUN(launch_attention(a, st));
-    }
-    {
-      GemmArgs a;
-      a.A = s.attn; a.W = b.proj_w; a.M = M; a.N = D; a.K = D; a.lda = D; a.ldw = D;
-      a.bias = b.proj_b; a.residual = ws.x; a.out = ws.x; a.out_fp32 = 1;
-      RUN(launch_gemm(a, num_sms, st));
-    }
-    if (cudaMemcpyAsync(s.x_mid, ws.x, (size_t)M * D * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess) return set_error("encode_train: copy failed");
-    l = LnArgs();
-    l.x = ws.x; l.rows = M; l.D = D; l.gamma = b.ln2_g; l.beta = b.ln2_b; l.eps = 1e-6f; l.out = ws.xn;
-    RUN(launch_layernorm(l, st));
-    {
-      GemmArgs a;   // pre-activation kept; GELU as its own pass
-      a.A = ws.xn; a.W = b.fc1_w; a.M = M; a.N = 4 * D; a.K = D; a.lda = D; a.ldw = D; a.bias = b.fc1_b; a.out = s.pre;
-      RUN(launch_gemm(a, num_sms, st));
-    }
-    RUN(launch_gelu_fwd(s.pre, (long)M * 4 * D, ws.hidden, st));
-    {
-      GemmArgs a;
-      a.A = ws.hidden; a.W = b.fc2_w; a.M = M; a.N = D; a.K = 4 * D; a.lda = 4 * D; a.ldw = 4 * D;
-      a.bias = b.fc2_b; a.residual = ws.x; a.out = ws.x; a.out_fp32 = 1;
-      RUN(launch_gemm(a, num_sms, st));
-    }
-  }
-  // neck (every intermediate stays in the workspace for the backward pass)
-  RUN(launch_cast_bf16(ws.x, (long)M * D, ws.xn, st));
-  {
-    GemmArgs a;
-    a.A = ws.xn; a.W = enc.neck_conv1; a.M = M; a.N = C; a.K = D; a.lda = D; a.ldw = D; a.out = ws.neck1; a.out_fp32 = 1;
-    RUN(launch_gemm(a, num_sms, st));
-  }
-  {
-    LnArgs l;
-    l.x = ws.neck1; l.rows = M; l.D = C; l.gamma = enc.neck_ln1_g; l.beta = enc.neck_ln1_b; l.eps = 1e-6f; l.out = ws.neck1b;
-    RUN(launch_layernorm(l, st));
-  }
-  RUN(launch_im2col3x3(ws.neck1b, B, g, C, ws.neck_col, st));
-  {
-    GemmArgs a;
-    a.A = ws.neck_col; a.W = enc.neck_conv2; a.M = M; a.N = C; a.K = 9 * C; a.lda = 9 * C; a.ldw = 9 * C; a.out = ws.neck2; a.out_fp32 = 1;
-    RUN(launch_gemm(a, num_sms, st));
-  }
-  RUN(launch_layernorm2d_nchw(ws.neck2, B, T, enc.neck_ln2_g, enc.neck_ln2_b, 1e-6f, out, st));
-  t.B = B;
+  RUN(train_setup(st));
+  RUN(vit_forward(nullptr, f32, B, cfg.image_size, cfg.image_size, train->acts.data(), out, st));
+  train->B = B;
   return 0;
 }
 
@@ -314,18 +204,17 @@ static int linear_dgrad(Engine& e, const __nv_bfloat16* dy, const __nv_bfloat16*
 }
 
 // (dq, dk, dv) and the rel-pos table gradients of one block; qkv / do in the block's row order (window-partitioned or image)
-static int attention_backward(Engine& e, TrainState& t, const EncBlock& b, TrainSave& s, const __nv_bfloat16* d_out, int B, cudaStream_t st) {
+static int attention_backward(Engine& e, TrainState& t, const EncBlock& b, const VitBlockActs& acts, TrainSave& s, const __nv_bfloat16* d_out,
+                              int B, cudaStream_t st) {
   const msam_config& cfg = e.cfg;
   const int D = cfg.embed_dim, H = cfg.num_heads, hd = D / H, g = cfg.image_size / cfg.patch_size;
   const int wpr = (g + cfg.window_size - 1) / cfg.window_size;
-  AttnBwdGeom geo;
-  int outer;
-  if (b.global) { geo.side = g; geo.n_tok = g * g; geo.nt = 256; geo.woff = 128; outer = B; }
-  else { geo.side = cfg.window_size; geo.n_tok = geo.side * geo.side; geo.nt = 64; geo.woff = 32; outer = B * wpr * wpr; }
-  const int Tk = geo.n_tok, pitch = (Tk + 7) & ~7, rt_cols = ((hd + 63) / 64) * 64;
+  const AttnBwdGeom geo = rel_table_geom(b.global, cfg.window_size, g);
+  const int outer = b.global ? B : B * wpr * wpr;
+  const int Tk = geo.n_tok, pitch = (Tk + 7) & ~7, rt_cols = rel_table_cols(hd);
   const long nb = (long)outer * H;
   const float scale = 1.0f / sqrtf((float)hd);
-  const __nv_bfloat16 *Q = s.qkv, *K = s.qkv + D, *V = s.qkv + 2 * D;
+  const __nv_bfloat16 *Q = acts.qkv, *K = acts.qkv + D, *V = acts.qkv + 2 * D;
   const long row_w = (long)Tk * 3 * D;     // elements between consecutive outer entries of qkv
   BGemmArgs a;
   // S = Q K^T
@@ -408,43 +297,44 @@ int Engine::encode_backward(const float* d_out, cudaStream_t st) {
   // ---- blocks, in reverse
   for (int i = cfg.depth - 1; i >= 0; --i) {
     const EncBlock& b = enc.blocks[i];
+    const VitBlockActs& a = t.acts[i];
     TrainSave& s = t.blk[i];
     const int Mq = b.global ? M : B * Tw;
     // MLP
     RUN(launch_cast_bf16(t.dx, (long)M * D, t.gb, st));
-    RUN(launch_gelu_fwd(s.pre, (long)M * 4 * D, t.hid, st));
+    RUN(launch_gelu_fwd(a.pre, (long)M * 4 * D, t.hid, st));
     RUN(linear_wgrad(t.gb, t.hid, M, D, 4 * D, s.g_fc2_w, s.g_fc2_b, st));
     RUN(linear_dgrad(*this, t.gb, s.fc2_wT, M, D, 4 * D, t.dhid, 0, st));
-    RUN(launch_gelu_bwd(t.dhid, s.pre, (long)M * 4 * D, t.dhid, st));
+    RUN(launch_gelu_bwd(t.dhid, a.pre, (long)M * 4 * D, t.dhid, st));
     {
       LnArgs l;
-      l.x = s.x_mid; l.rows = M; l.D = D; l.gamma = b.ln2_g; l.beta = b.ln2_b; l.eps = 1e-6f; l.out = t.xn;
+      l.x = a.x_mid; l.rows = M; l.D = D; l.gamma = b.ln2_g; l.beta = b.ln2_b; l.eps = 1e-6f; l.out = t.xn;
       RUN(launch_layernorm(l, st));
     }
     RUN(linear_wgrad(t.dhid, t.xn, M, 4 * D, D, s.g_fc1_w, s.g_fc1_b, st));
     RUN(linear_dgrad(*this, t.dhid, s.fc1_wT, M, 4 * D, D, t.dxn, 1, st));
     RUN(zero(s.g_ln2_g, D)); RUN(zero(s.g_ln2_b, D));
-    RUN(launch_layernorm_bwd(s.x_mid, M, D, b.ln2_g, 1e-6f, t.dxn, 0, g, cfg.window_size, 1, t.dx, s.g_ln2_g, s.g_ln2_b, st));
+    RUN(launch_layernorm_bwd(a.x_mid, M, D, b.ln2_g, 1e-6f, t.dxn, 0, g, cfg.window_size, 1, t.dx, s.g_ln2_g, s.g_ln2_b, st));
     // attention
     RUN(launch_cast_bf16(t.dx, (long)M * D, t.gb, st));
-    RUN(linear_wgrad(t.gb, s.attn, M, D, D, s.g_proj_w, s.g_proj_b, st));
+    RUN(linear_wgrad(t.gb, a.attn, M, D, D, s.g_proj_w, s.g_proj_b, st));
     RUN(linear_dgrad(*this, t.gb, s.proj_wT, M, D, D, t.xn, 0, st));       // d(attention output), image order, over the xn scratch
     const __nv_bfloat16* d_attn = t.xn;
     if (!b.global) {
       RUN(launch_window_gather(t.xn, B, g, cfg.window_size, D, t.do_win, st));
       d_attn = t.do_win;
     }
-    RUN(attention_backward(*this, t, b, s, d_attn, B, st));
+    RUN(attention_backward(*this, t, b, a, s, d_attn, B, st));
     {
       LnArgs l;
-      l.x = s.x_in; l.rows = M; l.D = D; l.gamma = b.ln1_g; l.beta = b.ln1_b; l.eps = 1e-6f; l.grid = g; l.ws = cfg.window_size;
+      l.x = a.x_in; l.rows = M; l.D = D; l.gamma = b.ln1_g; l.beta = b.ln1_b; l.eps = 1e-6f; l.grid = g; l.ws = cfg.window_size;
       if (b.global) { l.out = t.xn; } else { l.out = t.xn_win; l.window_mode = 1; }
       RUN(launch_layernorm(l, st));
     }
     RUN(linear_wgrad(t.dqkv, b.global ? t.xn : t.xn_win, Mq, 3 * D, D, s.g_qkv_w, s.g_qkv_b, st));
     RUN(linear_dgrad(*this, t.dqkv, s.qkv_wT, Mq, 3 * D, D, t.dxn, 1, st));
     RUN(zero(s.g_ln1_g, D)); RUN(zero(s.g_ln1_b, D));
-    RUN(launch_layernorm_bwd(s.x_in, M, D, b.ln1_g, 1e-6f, t.dxn, b.global ? 0 : 1, g, cfg.window_size, 1, t.dx, s.g_ln1_g, s.g_ln1_b, st));
+    RUN(launch_layernorm_bwd(a.x_in, M, D, b.ln1_g, 1e-6f, t.dxn, b.global ? 0 : 1, g, cfg.window_size, 1, t.dx, s.g_ln1_g, s.g_ln1_b, st));
   }
   // ---- patch embedding + positional embedding: x0 = patches W^T + b + pos
   RUN(launch_sum_batch(t.dx, B, (long)T * D, t.g_pos, 0, st));
@@ -469,7 +359,7 @@ void Engine::train_free() {
 }
 
 void Engine::train_invalidate() {
-  if (train) { train->transposed = false; train->B = 0; }
+  if (train) train->B = 0;
 }
 
 }  // namespace msam

@@ -179,7 +179,8 @@ int Engine::finalize_encoder() {
     const std::string p = e + "blocks." + std::to_string(i) + ".";
     b.global = false;
     for (int k = 0; k < 8 && cfg.global_attn[k] >= 0; ++k) b.global |= (cfg.global_attn[k] == i);
-    const int S = b.global ? g : cfg.window_size;
+    const AttnBwdGeom geo = rel_table_geom(b.global, cfg.window_size, g);
+    const int S = geo.side;
     CHK(b.ln1_g = up_f32(p + "norm1.weight", {D}));
     CHK(b.ln1_b = up_f32(p + "norm1.bias", {D}));
     CHK(b.qkv_w = up_bf16(p + "attn.qkv.weight", {3 * D, D}));
@@ -192,18 +193,17 @@ int Engine::finalize_encoder() {
     CHK(b.fc1_b = up_f32(p + "mlp.lin1.bias", {4 * D}));
     CHK(b.fc2_w = up_bf16(p + "mlp.lin2.weight", {D, 4 * D}));
     CHK(b.fc2_b = up_f32(p + "mlp.lin2.bias", {D}));
-    // relative-position table tile: rows [0,2S-1) = rel_pos_h, rows [WOFF, WOFF+2S-1) = rel_pos_w, zero elsewhere;
-    // columns padded to a multiple of 64 (csrc/attention.cu).  get_rel_pos's interpolation branch (table length
+    // relative-position table tile in the layout of rel_table_geom (kernels.h).  get_rel_pos's interpolation branch (table length
     // != 2S-1, only hit when image_size != 1024) is not supported.
     const auto* rh = host(p + "attn.rel_pos_h", {2 * S - 1, hd});
     const auto* rw = host(p + "attn.rel_pos_w", {2 * S - 1, hd});
     CHK(rh && rw);
-    const int NT = b.global ? 256 : 64, WOFF = b.global ? 128 : 32, cols = ((hd + 63) / 64) * 64;
-    std::vector<float> tab((size_t)NT * cols, 0.f);
+    const int cols = rel_table_cols(hd);
+    std::vector<float> tab((size_t)geo.nt * cols, 0.f);
     for (int r = 0; r < 2 * S - 1; ++r)
       for (int c = 0; c < hd; ++c) {
         tab[(size_t)r * cols + c] = (*rh)[(size_t)r * hd + c];
-        tab[(size_t)(WOFF + r) * cols + c] = (*rw)[(size_t)r * hd + c];
+        tab[(size_t)(geo.woff + r) * cols + c] = (*rw)[(size_t)r * hd + c];
       }
     CHK(b.rel_table = upload_bf16(tab.data(), tab.size()));
   }
@@ -249,95 +249,108 @@ int Engine::encode(const uint8_t* u8, const float* f32, int B, int hh, int ww, f
   if (is_tinyvit()) return encode_tinyvit(u8, f32, B, hh, ww, out, st, stop_after, x_out);
   if (!finalized) return set_error("msam_encode: weights not finalized");
   if (B <= 0) return set_error("msam_encode: empty batch");
+  const int D = cfg.embed_dim, g = cfg.image_size / cfg.patch_size, T = g * g, C = cfg.out_chans;
+  if (u8 && (hh > cfg.image_size || ww > cfg.image_size || hh <= 0 || ww <= 0))
+    return set_error("msam_encode_u8: image %dx%d exceeds %d", hh, ww, cfg.image_size);
+  for (int b0 = 0; b0 < B; b0 += cfg.max_batch) {
+    const int nb = (B - b0 < cfg.max_batch) ? (B - b0) : cfg.max_batch;
+    const uint8_t* u8p = u8 ? u8 + (size_t)b0 * hh * ww * 3 : nullptr;
+    const float* f32p = f32 ? f32 + (size_t)b0 * 3 * cfg.image_size * cfg.image_size : nullptr;
+    if (vit_forward(u8p, f32p, nb, hh, ww, nullptr, stop_after >= 0 ? nullptr : out + (size_t)b0 * C * T, st, stop_after)) return -1;
+    if (stop_after >= 0 &&   // debug / parity localisation: the fp32 residual stream after `stop_after` blocks
+        cudaMemcpyAsync(x_out + (size_t)b0 * T * D, ws.x, (size_t)nb * T * D * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+      return set_error("encode_blocks: copy failed");
+  }
+  return 0;
+}
+
+int Engine::vit_forward(const uint8_t* u8, const float* f32, int nb, int hh, int ww, const VitBlockActs* keep, float* out,
+                        cudaStream_t st, int stop_after) {
   const int D = cfg.embed_dim, hd = D / cfg.num_heads, g = cfg.image_size / cfg.patch_size, T = g * g, C = cfg.out_chans;
   const int wpr = (g + cfg.window_size - 1) / cfg.window_size;
   const int Tw = wpr * wpr * cfg.window_size * cfg.window_size;
-  if (u8 && (hh > cfg.image_size || ww > cfg.image_size || hh <= 0 || ww <= 0))
-    return set_error("msam_encode_u8: image %dx%d exceeds %d", hh, ww, cfg.image_size);
+  const int M = nb * T;
   static const float mean[3] = {123.675f, 116.28f, 103.53f}, stdv[3] = {58.395f, 57.12f, 57.375f};
-  for (int b0 = 0; b0 < B; b0 += cfg.max_batch) {
-    const int nb = (B - b0 < cfg.max_batch) ? (B - b0) : cfg.max_batch;
-    const int M = nb * T;
-    const uint8_t* u8p = u8 ? u8 + (size_t)b0 * hh * ww * 3 : nullptr;
-    const float* f32p = f32 ? f32 + (size_t)b0 * 3 * cfg.image_size * cfg.image_size : nullptr;
-    if (launch_patchify(u8p, f32p, nb, hh, ww, cfg.image_size, mean, stdv, ws.patches, st)) return -1;
-    {  // patch embed: conv 16x16/16 == GEMM, + bias + pos_embed (row % T)
-      GemmArgs a;
-      a.A = ws.patches; a.W = enc.patch_w; a.M = M; a.N = D; a.K = 768; a.lda = 768; a.ldw = 768;
-      a.bias = enc.patch_b; a.residual = enc.pos_embed; a.res_rows = T; a.out = ws.x; a.out_fp32 = 1;
-      if (launch_gemm(a, num_sms, st)) return -1;
-    }
-    int blk_idx = 0;
-    for (const EncBlock& b : enc.blocks) {
-      if (stop_after >= 0 && blk_idx++ >= stop_after) break;
-      LnArgs l;
-      l.x = ws.x; l.rows = M; l.D = D; l.gamma = b.ln1_g; l.beta = b.ln1_b; l.eps = 1e-6f;
-      l.grid = g; l.ws = cfg.window_size;
-      if (b.global) { l.out = ws.xn; } else { l.out = ws.xn_win; l.window_mode = 1; }
-      if (launch_layernorm(l, st)) return -1;
-      const int Mq = b.global ? M : nb * Tw;
-      {
-        GemmArgs a;
-        a.A = b.global ? ws.xn : ws.xn_win; a.W = b.qkv_w; a.M = Mq; a.N = 3 * D; a.K = D; a.lda = D; a.ldw = D;
-        a.bias = b.qkv_b; a.out = ws.qkv;
-        if (launch_gemm(a, num_sms, st)) return -1;
-      }
-      {
-        AttnArgs a;
-        a.qkv = ws.qkv; a.rel_table = b.rel_table; a.out = ws.attn; a.batch = nb; a.heads = cfg.num_heads;
-        a.head_dim = hd; a.grid = g; a.window = b.global ? 0 : cfg.window_size; a.scale = 1.0f / sqrtf((float)hd);
-        if (launch_attention(a, st)) return -1;
-      }
-      {
-        GemmArgs a;
-        a.A = ws.attn; a.W = b.proj_w; a.M = M; a.N = D; a.K = D; a.lda = D; a.ldw = D;
-        a.bias = b.proj_b; a.residual = ws.x; a.out = ws.x; a.out_fp32 = 1;
-        if (launch_gemm(a, num_sms, st)) return -1;
-      }
-      l = LnArgs();
-      l.x = ws.x; l.rows = M; l.D = D; l.gamma = b.ln2_g; l.beta = b.ln2_b; l.eps = 1e-6f; l.out = ws.xn;
-      if (launch_layernorm(l, st)) return -1;
-      {
-        GemmArgs a;
-        a.A = ws.xn; a.W = b.fc1_w; a.M = M; a.N = 4 * D; a.K = D; a.lda = D; a.ldw = D;
-        a.bias = b.fc1_b; a.act = 1; a.out = ws.hidden;
-        if (launch_gemm(a, num_sms, st)) return -1;
-      }
-      {
-        GemmArgs a;
-        a.A = ws.hidden; a.W = b.fc2_w; a.M = M; a.N = D; a.K = 4 * D; a.lda = 4 * D; a.ldw = 4 * D;
-        a.bias = b.fc2_b; a.residual = ws.x; a.out = ws.x; a.out_fp32 = 1;
-        if (launch_gemm(a, num_sms, st)) return -1;
-      }
-    }
-    if (stop_after >= 0) {  // debug / parity localisation: the fp32 residual stream after `stop_after` blocks
-      if (cudaMemcpyAsync(x_out + (size_t)b0 * T * D, ws.x, (size_t)M * D * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
-        return set_error("encode_blocks: copy failed");
-      continue;
-    }
-    // neck: conv1x1 -> LN2d -> conv3x3 (im2col GEMM) -> LN2d (NCHW out)
-    if (launch_cast_bf16(ws.x, (long)M * D, ws.xn, st)) return -1;
-    {
-      GemmArgs a;
-      a.A = ws.xn; a.W = enc.neck_conv1; a.M = M; a.N = C; a.K = D; a.lda = D; a.ldw = D; a.out = ws.neck1; a.out_fp32 = 1;
-      if (launch_gemm(a, num_sms, st)) return -1;
-    }
-    {
-      LnArgs l;
-      l.x = ws.neck1; l.rows = M; l.D = C; l.gamma = enc.neck_ln1_g; l.beta = enc.neck_ln1_b; l.eps = 1e-6f; l.out = ws.neck1b;
-      if (launch_layernorm(l, st)) return -1;
-    }
-    if (launch_im2col3x3(ws.neck1b, nb, g, C, ws.neck_col, st)) return -1;
-    {
-      GemmArgs a;
-      a.A = ws.neck_col; a.W = enc.neck_conv2; a.M = M; a.N = C; a.K = 9 * C; a.lda = 9 * C; a.ldw = 9 * C;
-      a.out = ws.neck2; a.out_fp32 = 1;
-      if (launch_gemm(a, num_sms, st)) return -1;
-    }
-    if (launch_layernorm2d_nchw(ws.neck2, nb, T, enc.neck_ln2_g, enc.neck_ln2_b, 1e-6f, out + (size_t)b0 * C * T, st))
-      return -1;
+  auto keep_copy = [&](float* dst) {   // training: a copy of the fp32 residual stream for the backward pass
+    if (cudaMemcpyAsync(dst, ws.x, (size_t)M * D * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess) return set_error("encode_train: copy failed");
+    return 0;
+  };
+  if (launch_patchify(u8, f32, nb, hh, ww, cfg.image_size, mean, stdv, ws.patches, st)) return -1;
+  {  // patch embed: conv 16x16/16 == GEMM, + bias + pos_embed (row % T)
+    GemmArgs a;
+    a.A = ws.patches; a.W = enc.patch_w; a.M = M; a.N = D; a.K = 768; a.lda = 768; a.ldw = 768;
+    a.bias = enc.patch_b; a.residual = enc.pos_embed; a.res_rows = T; a.out = ws.x; a.out_fp32 = 1;
+    if (launch_gemm(a, num_sms, st)) return -1;
   }
-  return 0;
+  const int n_blocks = stop_after >= 0 && stop_after < cfg.depth ? stop_after : cfg.depth;
+  for (int i = 0; i < n_blocks; ++i) {
+    const EncBlock& b = enc.blocks[i];
+    __nv_bfloat16* qkv = keep ? keep[i].qkv : ws.qkv;
+    __nv_bfloat16* attn = keep ? keep[i].attn : ws.attn;
+    if (keep && keep_copy(keep[i].x_in)) return -1;
+    LnArgs l;
+    l.x = ws.x; l.rows = M; l.D = D; l.gamma = b.ln1_g; l.beta = b.ln1_b; l.eps = 1e-6f;
+    l.grid = g; l.ws = cfg.window_size;
+    if (b.global) { l.out = ws.xn; } else { l.out = ws.xn_win; l.window_mode = 1; }
+    if (launch_layernorm(l, st)) return -1;
+    const int Mq = b.global ? M : nb * Tw;
+    {
+      GemmArgs a;
+      a.A = b.global ? ws.xn : ws.xn_win; a.W = b.qkv_w; a.M = Mq; a.N = 3 * D; a.K = D; a.lda = D; a.ldw = D;
+      a.bias = b.qkv_b; a.out = qkv;
+      if (launch_gemm(a, num_sms, st)) return -1;
+    }
+    {
+      AttnArgs a;
+      a.qkv = qkv; a.rel_table = b.rel_table; a.out = attn; a.batch = nb; a.heads = cfg.num_heads;
+      a.head_dim = hd; a.grid = g; a.window = b.global ? 0 : cfg.window_size; a.scale = 1.0f / sqrtf((float)hd);
+      if (launch_attention(a, st)) return -1;
+    }
+    {
+      GemmArgs a;
+      a.A = attn; a.W = b.proj_w; a.M = M; a.N = D; a.K = D; a.lda = D; a.ldw = D;
+      a.bias = b.proj_b; a.residual = ws.x; a.out = ws.x; a.out_fp32 = 1;
+      if (launch_gemm(a, num_sms, st)) return -1;
+    }
+    if (keep && keep_copy(keep[i].x_mid)) return -1;
+    l = LnArgs();
+    l.x = ws.x; l.rows = M; l.D = D; l.gamma = b.ln2_g; l.beta = b.ln2_b; l.eps = 1e-6f; l.out = ws.xn;
+    if (launch_layernorm(l, st)) return -1;
+    {
+      GemmArgs a;
+      a.A = ws.xn; a.W = b.fc1_w; a.M = M; a.N = 4 * D; a.K = D; a.lda = D; a.ldw = D; a.bias = b.fc1_b;
+      if (keep) { a.out = keep[i].pre; } else { a.act = 1; a.out = ws.hidden; }   // training keeps the pre-activation for GELU'
+      if (launch_gemm(a, num_sms, st)) return -1;
+    }
+    if (keep && launch_gelu_fwd(keep[i].pre, (long)M * 4 * D, ws.hidden, st)) return -1;
+    {
+      GemmArgs a;
+      a.A = ws.hidden; a.W = b.fc2_w; a.M = M; a.N = D; a.K = 4 * D; a.lda = 4 * D; a.ldw = 4 * D;
+      a.bias = b.fc2_b; a.residual = ws.x; a.out = ws.x; a.out_fp32 = 1;
+      if (launch_gemm(a, num_sms, st)) return -1;
+    }
+  }
+  if (stop_after >= 0) return 0;
+  // neck: conv1x1 -> LN2d -> conv3x3 (im2col GEMM) -> LN2d (NCHW out); the training backward reads its intermediates from ws
+  if (launch_cast_bf16(ws.x, (long)M * D, ws.xn, st)) return -1;
+  {
+    GemmArgs a;
+    a.A = ws.xn; a.W = enc.neck_conv1; a.M = M; a.N = C; a.K = D; a.lda = D; a.ldw = D; a.out = ws.neck1; a.out_fp32 = 1;
+    if (launch_gemm(a, num_sms, st)) return -1;
+  }
+  {
+    LnArgs l;
+    l.x = ws.neck1; l.rows = M; l.D = C; l.gamma = enc.neck_ln1_g; l.beta = enc.neck_ln1_b; l.eps = 1e-6f; l.out = ws.neck1b;
+    if (launch_layernorm(l, st)) return -1;
+  }
+  if (launch_im2col3x3(ws.neck1b, nb, g, C, ws.neck_col, st)) return -1;
+  {
+    GemmArgs a;
+    a.A = ws.neck_col; a.W = enc.neck_conv2; a.M = M; a.N = C; a.K = 9 * C; a.lda = 9 * C; a.ldw = 9 * C;
+    a.out = ws.neck2; a.out_fp32 = 1;
+    if (launch_gemm(a, num_sms, st)) return -1;
+  }
+  return launch_layernorm2d_nchw(ws.neck2, nb, T, enc.neck_ln2_g, enc.neck_ln2_b, 1e-6f, out, st);
 }
 
 }  // namespace msam

@@ -40,6 +40,13 @@ struct EncoderWorkspace {
   __nv_bfloat16 *neck1b = nullptr, *neck_col = nullptr;
 };
 
+// Activations of one ViT block that the training forward keeps for the backward pass (encoder_train.cu): the fp32 residual stream
+// before the block (x_in) and before the MLP (x_mid), qkv, the attention output and the fc1 pre-activation (bf16).
+struct VitBlockActs {
+  float *x_in = nullptr, *x_mid = nullptr;
+  __nv_bfloat16 *qkv = nullptr, *attn = nullptr, *pre = nullptr;
+};
+
 // ---- TinyViT (vit_t) encoder, tinyvit.cu
 struct TvConv {                       // Conv2d_BN with the BatchNorm folded in
   __nv_bfloat16* w = nullptr;         // dense / 1x1: GEMM operand [out, in * k * k]
@@ -73,9 +80,10 @@ struct OptParam {
   int64_t n = 0;
   const bool* written = nullptr;  // non-null: AdamW skips the tensor while *written is false (no gradient since the last zeroing)
   int64_t steps = 0;              // ... and counts its own steps for the bias correction (with written only)
-  int refresh = 0;              // 0 none | 1 cast -> dst | 2 cast -> dst + transpose -> dstT | 3 rows of a rel-pos table | 4 neck 3x3 conv
-                                // relayout | 5 prompt-encoder tables of the inference decoder | 6 conv-transpose bias (fold the 4 tiles first)
-  __nv_bfloat16 *dst = nullptr, *dstT = nullptr;
+  int refresh = 0;              // 0 none | 1 cast -> dst | 3 rows of a rel-pos table | 4 neck 3x3 conv relayout | 5 prompt-encoder
+                                // tables of the inference decoder | 6 conv-transpose bias (fold the 4 tiles first)
+  __nv_bfloat16 *dst = nullptr;
+  __nv_bfloat16* dstT = nullptr;  // non-null: after the refresh, dstT [cols, rows] = dst [rows, cols]^T (W^T of the dgrad GEMMs)
   int rows = 0, cols = 0, cols_pad = 0, row_off = 0;
 };
 
@@ -117,8 +125,12 @@ struct Engine {
                      float* x_out = nullptr);
   int encode(const uint8_t* u8, const float* f32, int B, int hh, int ww, float* out, cudaStream_t st, int stop_after = -1,
              float* x_out = nullptr);
+  // ViT forward of nb <= max_batch images: patch embedding, blocks, neck -> out (NCHW).  stop_after >= 0: only the first stop_after
+  // blocks, no neck (the fp32 residual stream is left in ws.x).  keep: null for inference, else one VitBlockActs per block.
+  int vit_forward(const uint8_t* u8, const float* f32, int nb, int hh, int ww, const VitBlockActs* keep, float* out, cudaStream_t st,
+                  int stop_after = -1);
   // encoder_train.cu (cfg 5): forward keeping activations, backward, gradient read-out by upstream key name
-  int train_setup();
+  int train_setup(cudaStream_t st);
   int encode_train(const float* f32, int B, float* out, cudaStream_t st);
   int encode_backward(const float* d_out, cudaStream_t st);
   int encoder_grad(const char* name, float* dst, int64_t n, cudaStream_t st);

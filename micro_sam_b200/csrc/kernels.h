@@ -86,6 +86,17 @@ int launch_gelu_bwd(const __nv_bfloat16* dh, const __nv_bfloat16* pre, long n, _
 int launch_colsum(const __nv_bfloat16* x, long rows, int N, float* out, cudaStream_t stream);   // out[N] += column sums
 int launch_window_gather(const __nv_bfloat16* x, int B, int grid, int ws, int D, __nv_bfloat16* out_win, cudaStream_t stream);
 struct AttnBwdGeom { int side = 14, n_tok = 196, nt = 64, woff = 32; };   // window: 14 / 196 / 64 / 32; global: 64 / 4096 / 256 / 128
+// Packed rel-pos table of one encoder block, bf16 [nt, rel_table_cols(head_dim)]: rows [0, 2 side - 1) = rel_pos_h, rows
+// [woff, woff + 2 side - 1) = rel_pos_w, zero elsewhere.  The attention kernels (forward and backward) read this layout.
+inline AttnBwdGeom rel_table_geom(bool global, int window, int grid) {
+  AttnBwdGeom g;
+  g.side = global ? grid : window;
+  g.n_tok = g.side * g.side;
+  g.nt = global ? 256 : 64;
+  g.woff = global ? 128 : 32;
+  return g;
+}
+inline int rel_table_cols(int head_dim) { return ((head_dim + 63) / 64) * 64; }
 int launch_attn_probs(const float* S, const float* T, long n_batch, AttnBwdGeom g, int pitch_s, int pitch_p, float scale,
                       __nv_bfloat16* P, cudaStream_t stream);
 int launch_attn_ds(const __nv_bfloat16* P, const float* dP, long n_batch, AttnBwdGeom g, int pitch_s, int pitch_p,
@@ -96,6 +107,8 @@ int launch_sum_batch(const float* x, long n_batch, long n, float* out, int accum
 int launch_nchw_to_tok(const float* nchw, int B, int C, int T, float* tok, cudaStream_t stream);
 int launch_col2im3x3(const __nv_bfloat16* dcol, int B, int g, int C, float* out, cudaStream_t stream);
 int launch_cast_f32(const __nv_bfloat16* x, long n, float* out, cudaStream_t stream);
+// out [cols, rows] = in [rows, cols]^T (the W^T operands of the dgrad GEMMs)
+int launch_transpose_bf16(const __nv_bfloat16* in, int rows, int cols, __nv_bfloat16* out, cudaStream_t stream);
 
 // ---- upscale_fused.cu : conv-transpose 1 + LayerNorm2d + GELU + conv-transpose 2 + GELU + hyper-network product in one pass
 struct UpscaleFusedArgs {

@@ -32,15 +32,6 @@ __global__ void fold4_kernel(float* __restrict__ g, int co) {
   const float s = g[o] + g[co + o] + g[2 * co + o] + g[3 * co + o];
   g[o] = s; g[co + o] = s; g[2 * co + o] = s; g[3 * co + o] = s;
 }
-__global__ void transpose_bf16_opt(const __nv_bfloat16* __restrict__ in, int rows, int cols, __nv_bfloat16* __restrict__ out) {
-  __shared__ __nv_bfloat16 tile[32][34];
-  const int r0 = blockIdx.y * 32, c0 = blockIdx.x * 32;
-  for (int i = threadIdx.y; i < 32; i += blockDim.y)
-    if (r0 + i < rows && c0 + threadIdx.x < cols) tile[i][threadIdx.x] = in[(long)(r0 + i) * cols + c0 + threadIdx.x];
-  __syncthreads();
-  for (int i = threadIdx.y; i < 32; i += blockDim.y)
-    if (c0 + i < cols && r0 + threadIdx.x < rows) out[(long)(c0 + i) * rows + r0 + threadIdx.x] = tile[threadIdx.x][i];
-}
 // rows [row_off, row_off + rows) of a rel-pos table tile [NT, cols_pad] <- fp32 [rows, cols]
 __global__ void rel_rows_kernel(const float* __restrict__ w, int rows, int cols, int cols_pad, int row_off, __nv_bfloat16* __restrict__ tab) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -89,10 +80,6 @@ int Engine::optimizer_step(float lr, float b1, float b2, float eps, float wd, cu
       case 1:
         RUN(launch_cast_bf16(p.w, p.n, p.dst, st));
         break;
-      case 2:
-        RUN(launch_cast_bf16(p.w, p.n, p.dst, st));
-        transpose_bf16_opt<<<dim3((p.cols + 31) / 32, (p.rows + 31) / 32), dim3(32, 8), 0, st>>>(p.dst, p.rows, p.cols, p.dstT);
-        break;
       case 3:
         rel_rows_kernel<<<(unsigned)((p.n + 255) / 256), 256, 0, st>>>(p.w, p.rows, p.cols, p.cols_pad, p.row_off, p.dst);
         break;
@@ -102,13 +89,14 @@ int Engine::optimizer_step(float lr, float b1, float b2, float eps, float wd, cu
       default:
         break;
     }
+    if (p.dstT) RUN(launch_transpose_bf16(p.dst, p.rows, p.cols, p.dstT, st));
   }
   // embedding tables shared with the inference prompt encoder (it produces the sparse tokens of the training path as well)
   const float *pe = nullptr, *nap = nullptr;
   for (const OptParam& p : opt)
     if (p.refresh == 5) { if (p.n == 4 * 256) pe = p.w; else nap = p.w; }
   if (pe || nap) RUN(dec_set_prompt_tables(pe, nap, st));
-  train_invalidate();   // W^T operands of the encoder dgrad GEMMs are rebuilt by the next msam_encode_train
+  train_invalidate();   // the saved encoder forward pass belongs to the old weights
   if (cudaGetLastError() != cudaSuccess) return set_error("optimizer step: kernel launch failed");
   return 0;
 }
