@@ -215,28 +215,25 @@ int msam_op_dec_i2t(msam_handle* h, int layer, const void* queries, const void* 
 int msam_op_dec_upscale(msam_handle* h, const void* keys, const float* hyper_in, int P, int multimask, float* low_res,
                         int num_sms, void* stream);
 
-/* ---- fine-tuning (BASELINE.json configs[4], micro_sam/training/sam_trainer.py:393: loss.backward() through the image encoder).
+/* ---- fine-tuning (BASELINE.json configs[4], micro_sam/training/sam_trainer.py:393: loss.backward() through the image encoder and
+ * the mask decoder).  Every trainable tensor has one fp32 gradient buffer and one fp32 master buffer in the engine, listed by
+ * msam_train_tensor_count / _info (below); that list is the only way to read gradients and master weights.
  * msam_encode_train = msam_encode_f32 that keeps the activations of B <= max_batch images (ViT encoders only);
- * msam_encode_backward takes dL/d(embedding) (B,256,64,64) fp32 NCHW and fills one fp32 gradient per encoder parameter;
- * msam_encoder_grad copies the gradient of the parameter with upstream key `name` (e.g. "image_encoder.blocks.0.attn.qkv.weight",
- * n = its element count, upstream layout) into a device buffer.  The decoder-side backward (dL/d embedding from the mask loss) is
- * not part of this library yet (DESIGN.md). */
+ * msam_encode_backward takes dL/d(embedding) (B,256,64,64) fp32 NCHW and overwrites the gradient of every encoder parameter. */
 int msam_encode_train(msam_handle* h, const float* nchw, int B, float* out, void* stream);
 int msam_encode_backward(msam_handle* h, const float* d_out_nchw, void* stream);
-int msam_encoder_grad(msam_handle* h, const char* name, float* dst, int64_t n, void* stream);
 /* Mask decoder + prompt encoder in training mode (micro_sam/training/trainable_sam.py:62-114): MaskDecoder.forward for the P prompts of
  * ONE image keeping the activations in `slot` (0..7), and its backward pass.  sparse = prompt_encoder's sparse embeddings
  * [P, n_sparse, 256] (msam_prompt_encode), emb_index [P, n_sparse] int32 = the embedding-table row behind each sparse token (0..3 =
  * point_embeddings.{0..3}, 4 = not_a_point_embed) so that their gradients can be formed; the dense prompt is no_mask_embed.
  * backward: d_low_res [P, M, 256, 256] / d_iou [P, M] (either may be NULL) -> parameter gradients ACCUMULATE (msam_decoder_zero_grads),
- * d_emb_nchw [256, 64, 64] = dL/d(image embedding) is overwritten.  msam_decoder_grad reads a gradient by upstream key
- * ("....weight@gemm" / "@stack" keys carry packed layouts that micro_sam_b200/sam.py:decoder_grads folds back). */
+ * d_emb_nchw [256, 64, 64] = dL/d(image embedding) is overwritten. */
 int msam_decoder_train_forward(msam_handle* h, int slot, const float* emb_nchw, const float* sparse, const int32_t* emb_index, int n_sparse,
                                int P, int multimask, float* low_res, float* iou, void* stream);
 int msam_decoder_train_backward(msam_handle* h, int slot, const float* d_low_res, const float* d_iou, float* d_emb_nchw, void* stream);
 /* msam_decoder_train_forward with mask prompts: mask_input [P, 1, 256, 256] fp32 low-res logits (PromptEncoder._embed_masks), or NULL
  * (= msam_decoder_train_forward).  The dense prompt is then mask_downscaling(mask_input) instead of no_mask_embed.  The first call with
- * masks adds the ten "prompt_encoder.mask_downscaling.*" tensors (upstream keys and layouts) to the gradient table and the optimizer;
+ * masks adds the ten "prompt_encoder.mask_downscaling.*" tensors (upstream keys and layouts) to the trainable tensors;
  * msam_decoder_train_backward of such a slot accumulates their gradients (none w.r.t. the mask) and none for no_mask_embed, and
  * msam_optimizer_step updates them only when a masked backward has run since the last msam_decoder_zero_grads. */
 int msam_decoder_train_forward_ex(msam_handle* h, int slot, const float* emb_nchw, const float* sparse, const int32_t* emb_index,
@@ -247,17 +244,20 @@ int msam_decoder_train_forward_ex(msam_handle* h, int slot, const float* emb_nch
  * 3.weight, 3.bias, 4.weight, 4.bias, 6.weight, 6.bias (each in its upstream layout).  Leaves the engine's gradients alone. */
 int msam_op_mask_downscaling_train(msam_handle* h, const float* mask, int P, const float* d_dense, float* dense_out, float* grads_out,
                                    void* stream);
-int msam_decoder_grad(msam_handle* h, const char* name, float* dst, int64_t n, void* stream);
+/* Zeroes the gradients of the prompt-encoder and mask-decoder tensors (the encoder's are overwritten by each backward). */
 int msam_decoder_zero_grads(msam_handle* h, void* stream);
 /* torch.optim.AdamW semantics (micro_sam/training/training.py:train_sam's default optimizer) over every tensor that has received
  * gradients through msam_encode_backward / msam_decoder_train_backward: fp32 master weights, moments and decoupled weight decay on the
- * device, then the bf16 / transposed / packed operands of the training paths are refreshed.  msam_train_param reads a master tensor
- * (same keys and layouts as the gradient read-outs).  The packed operands of the INFERENCE decoder are refreshed by load_state_dict. */
+ * device, then the bf16 / transposed / tiled operands of the training paths are refreshed.  No gradient buffer is written, so a
+ * second step without a new backward applies the same gradients again, as torch.optim.AdamW does.  The packed operands of the
+ * INFERENCE decoder are refreshed by load_state_dict. */
 int msam_optimizer_step(msam_handle* h, float lr, float beta1, float beta2, float eps, float weight_decay, void* stream);
-int msam_train_param(msam_handle* h, const char* key, float* dst, int64_t n, void* stream);
 /* Enumeration of the trainable tensors (after the first training forward passes): key, DEVICE pointers of the fp32 gradient and master
- * buffers, element count -- so that a data-parallel driver can all-reduce the gradients in place (torch.distributed / NCCL on views of
- * these buffers) before msam_optimizer_step. */
+ * buffers, element count -- to read gradients and weights, and so that a data-parallel driver can all-reduce (or clip) the gradients in
+ * place before msam_optimizer_step.  Each tensor is an upstream one with its upstream element count.  The key is its upstream name,
+ * except for the three convolution weights kept in the layout of their GEMM, a permutation of the upstream layout:
+ * "mask_decoder.output_upscaling.{0,3}.weight@gemm" (ConvTranspose2d [ci, co, 2, 2] as [(dy * 2 + dx) * co + o][ci]) and
+ * "image_encoder.neck.2.weight@gemm" (Conv2d [o, c, 3, 3] as [o][ky * 3 + kx][c]). */
 int msam_train_tensor_count(msam_handle* h);
 int msam_train_tensor_info(msam_handle* h, int i, char* key_buf, int cap, void** grad, void** master, int64_t* n);
 /* Adjoint of msam_mask_loss_stats w.r.t. the low-res logits: d_stats [n_obj*M, 5] (only columns 0, 1 = dL/d sum(p t), dL/d sum(p^2)

@@ -89,7 +89,6 @@ def lib() -> ctypes.CDLL:
         L.msam_encode_u8_blocks.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
         L.msam_encode_train.argtypes = [c_void_p, c_void_p, c_int, c_void_p, c_void_p]
         L.msam_encode_backward.argtypes = [c_void_p, c_void_p, c_void_p]
-        L.msam_encoder_grad.argtypes = [c_void_p, c_char_p, c_void_p, c_int64, c_void_p]
         L.msam_op_bgemm.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_int64, c_int64,
                                     c_int64, c_int, c_int, c_void_p, c_int, c_int64, c_int64, c_float, c_int, c_void_p]
         L.msam_op_layernorm_bwd.argtypes = [c_void_p, c_int, c_int, c_void_p, c_float, c_void_p, c_int, c_int, c_void_p, c_void_p,
@@ -101,10 +100,8 @@ def lib() -> ctypes.CDLL:
                                                     c_void_p, c_void_p]
         L.msam_op_mask_downscaling_train.argtypes = [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
         L.msam_decoder_train_backward.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
-        L.msam_decoder_grad.argtypes = [c_void_p, c_char_p, c_void_p, c_int64, c_void_p]
         L.msam_decoder_zero_grads.argtypes = [c_void_p, c_void_p]
         L.msam_optimizer_step.argtypes = [c_void_p, c_float, c_float, c_float, c_float, c_float, c_void_p]
-        L.msam_train_param.argtypes = [c_void_p, c_char_p, c_void_p, c_int64, c_void_p]
         L.msam_train_tensor_count.argtypes = [c_void_p]
         L.msam_train_tensor_info.argtypes = [c_void_p, c_int, ctypes.c_char_p, c_int, POINTER(c_void_p), POINTER(c_void_p), POINTER(c_int64)]
         L.msam_mask_loss_backward.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]

@@ -544,7 +544,9 @@ struct Ten {
   int cols = 0;
   long n() const { return rows * cols; }
 };
-struct DLin { int out = 0, in = 0; __nv_bfloat16 *w = nullptr, *wT = nullptr; float *bias = nullptr, *gw = nullptr, *gb = nullptr; };
+// tiles > 1: a conv-transpose as a linear layer over sub-pixel tiles, out = tiles * co columns; bias [out] holds the bias [co] once per
+// tile, its gradient gb [co] sums over the tiles
+struct DLin { int out = 0, in = 0, tiles = 1; __nv_bfloat16 *w = nullptr, *wT = nullptr; float *bias = nullptr, *gw = nullptr, *gb = nullptr; };
 struct DLn { int D = 0; float eps = 1e-5f; float *g = nullptr, *b = nullptr, *gg = nullptr, *gb = nullptr; };
 struct DAttn { DLin q, k, v, o; int inner = 0; };
 struct DLayer { DAttn self, t2i, i2t; DLn n1, n2, n3, n4; DLin mlp1, mlp2; };
@@ -569,10 +571,9 @@ struct DecTrain {
   DLin ct1, ct2, hyper[4][3], iou[3];
   float *point_emb = nullptr, *not_a_point = nullptr, *no_mask = nullptr, *out_tokens = nullptr;
   float *g_point_emb = nullptr, *g_nap = nullptr, *g_no_mask = nullptr, *g_out_tokens = nullptr;
-  std::unordered_map<std::string, std::pair<float*, int64_t>> grads;
   DecSlot slot[8];
-  // mask_downscaling: packed fp32 masters / gradients (MD_* offsets), created by the first mask-prompt call; registered with the
-  // optimizer and the gradient table by the first masked training forward, so that runs without mask prompts never see them
+  // mask_downscaling: packed fp32 masters / gradients (MD_* offsets), created by the first mask-prompt call; registered by the first
+  // masked training forward, so that runs without mask prompts never see them
   float *md_w = nullptr, *md_g = nullptr;
   bool md_registered = false;
   bool md_written = false;           // a masked backward added to md_g since the last msam_decoder_zero_grads
@@ -634,7 +635,7 @@ int op_linear(Ctx& c, const Ten& x, DLin& L, Ten& y, int act, const Ten* residua
   c.s.tape.push_back([=](cudaStream_t st) -> int {
     RUN(cast_grad(yout.g, relu ? yout.b : nullptr, yout.n(), scratch, st));
     RUN(launch_gemm_tn(scratch, xin.b, Lp->out, Lp->in, (int)xin.rows, Lp->out, Lp->in, Lp->gw, Lp->in, st, 1));
-    RUN(launch_colsum(scratch, xin.rows, Lp->out, Lp->gb, st));
+    RUN(launch_colsum(scratch, xin.rows * Lp->tiles, Lp->out / Lp->tiles, Lp->gb, st));   // [rows, tiles * co] read as [tiles * rows, co]
     if (xin.g) {
       GemmArgs a;
       a.A = scratch; a.W = Lp->wT; a.M = (int)xin.rows; a.N = Lp->in; a.K = Lp->out; a.lda = Lp->out; a.ldw = Lp->out;
@@ -786,7 +787,9 @@ int attn_module(Ctx& c, DAttn& A, const Ten& q_in, const Ten& k_in, const Ten& v
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------ setup
-static int dt_lin(Engine& e, DecTrain& d, const std::string& key, int out, int in, DLin* L, int out_pad = 0) {
+// registered with the upstream element counts; out_pad > out: the GEMM operands have out_pad rows, the rows beyond out stay zero (their
+// gradient rows are sums of zeros)
+static int dt_lin(Engine& e, const std::string& key, int out, int in, DLin* L, int out_pad = 0) {
   const auto* w = e.host(key + ".weight", {out, in});
   const auto* b = e.host(key + ".bias", {out});
   if (!w || !b) return -1;
@@ -801,39 +804,33 @@ static int dt_lin(Engine& e, DecTrain& d, const std::string& key, int out, int i
   CHK(L->bias = e.upload_f32(bp.data(), bp.size()));
   CHK(L->gw = (float*)e.dalloc((size_t)op * in * 4, true));
   CHK(L->gb = (float*)e.dalloc((size_t)op * 4, true));
-  d.grads[key + ".weight"] = {L->gw, (int64_t)op * in};
-  d.grads[key + ".bias"] = {L->gb, op};
   OptParam pw, pb;
-  pw.key = key + ".weight"; CHK(pw.w = e.upload_f32(wp.data(), wp.size())); pw.g = L->gw; pw.n = (int64_t)op * in;
-  pw.refresh = 1; pw.dst = L->w; pw.dstT = L->wT; pw.rows = op; pw.cols = in;
-  pb.key = key + ".bias"; pb.w = L->bias; pb.g = L->gb; pb.n = op;
-  e.opt_add(pw); e.opt_add(pb);
+  pw.key = key + ".weight"; pw.g = L->gw; pw.n = (int64_t)out * in; pw.decoder = true;
+  pw.refresh = Refresh::Cast; pw.dst = L->w; pw.dstT = L->wT; pw.rows = op; pw.cols = in;
+  pb.key = key + ".bias"; pb.w = L->bias; pb.g = L->gb; pb.n = out; pb.decoder = true;
+  CHK(e.train_add(pw, w->data()) && e.train_add(pb));
   return 0;
 }
-static int dt_ln(Engine& e, DecTrain& d, const std::string& key, int D, float eps, DLn* L) {
+static int dt_ln(Engine& e, const std::string& key, int D, float eps, DLn* L) {
   L->D = D; L->eps = eps;
   CHK(L->g = e.up_f32(key + ".weight", {D}));
   CHK(L->b = e.up_f32(key + ".bias", {D}));
-  CHK(L->gg = (float*)e.dalloc((size_t)D * 4, true));
-  CHK(L->gb = (float*)e.dalloc((size_t)D * 4, true));
-  d.grads[key + ".weight"] = {L->gg, D};
-  d.grads[key + ".bias"] = {L->gb, D};
-  OptParam pg, pb;
-  pg.key = key + ".weight"; pg.w = L->g; pg.g = L->gg; pg.n = D;
-  pb.key = key + ".bias"; pb.w = L->b; pb.g = L->gb; pb.n = D;
-  e.opt_add(pg); e.opt_add(pb);
+  OptParam p;
+  p.n = D; p.decoder = true;
+  p.key = key + ".weight"; p.w = L->g; CHK(L->gg = e.train_add(p));
+  p.key = key + ".bias"; p.w = L->b; CHK(L->gb = e.train_add(p));
   return 0;
 }
-static int dt_attn(Engine& e, DecTrain& d, const std::string& key, int inner, DAttn* A) {
+static int dt_attn(Engine& e, const std::string& key, int inner, DAttn* A) {
   A->inner = inner;
-  RUN(dt_lin(e, d, key + ".q_proj", inner, 256, &A->q));
-  RUN(dt_lin(e, d, key + ".k_proj", inner, 256, &A->k));
-  RUN(dt_lin(e, d, key + ".v_proj", inner, 256, &A->v));
-  return dt_lin(e, d, key + ".out_proj", 256, inner, &A->o);
+  RUN(dt_lin(e, key + ".q_proj", inner, 256, &A->q));
+  RUN(dt_lin(e, key + ".k_proj", inner, 256, &A->k));
+  RUN(dt_lin(e, key + ".v_proj", inner, 256, &A->v));
+  return dt_lin(e, key + ".out_proj", 256, inner, &A->o);
 }
-// ConvTranspose2d(k = 2, s = 2) weight [ci, co, 2, 2] as the GEMM operand [(dy*2+dx)*co_n + co][ci]; gradients are exposed in this
-// layout under "<key>.weight@gemm" / "<key>.bias@gemm" (bias tiled over the 4 sub-pixels): micro_sam_b200/sam.py folds them back
-static int dt_convT(Engine& e, DecTrain& d, const std::string& key, int ci, int co, DLin* L) {
+// ConvTranspose2d(k = 2, s = 2) weight [ci, co, 2, 2] as the GEMM operand [(dy*2+dx)*co + o][ci], registered in this layout under
+// "<key>.weight@gemm"; the bias is registered as [co] and refreshed into the 4 tiles the GEMM epilogue reads
+static int dt_convT(Engine& e, const std::string& key, int ci, int co, DLin* L) {
   const auto* w = e.host(key + ".weight", {ci, co, 2, 2});
   const auto* b = e.host(key + ".bias", {co});
   if (!w || !b) return -1;
@@ -843,20 +840,17 @@ static int dt_convT(Engine& e, DecTrain& d, const std::string& key, int ci, int 
       for (int s = 0; s < 4; ++s) wg[((size_t)s * co + o) * ci + i] = (*w)[((size_t)i * co + o) * 4 + s];
   for (int s = 0; s < 4; ++s)
     for (int o = 0; o < co; ++o) bg[s * co + o] = (*b)[o];
-  L->out = 4 * co; L->in = ci;
+  L->out = 4 * co; L->in = ci; L->tiles = 4;
   CHK(L->w = e.upload_bf16(wg.data(), wg.size()));
   CHK(L->wT = (__nv_bfloat16*)e.dalloc(wg.size() * 2));
   RUN(launch_transpose_bf16(L->w, 4 * co, ci, L->wT, 0));
   CHK(L->bias = e.upload_f32(bg.data(), bg.size()));
-  CHK(L->gw = (float*)e.dalloc(wg.size() * 4, true));
-  CHK(L->gb = (float*)e.dalloc(bg.size() * 4, true));
-  d.grads[key + ".weight@gemm"] = {L->gw, (int64_t)wg.size()};
-  d.grads[key + ".bias@gemm"] = {L->gb, (int64_t)bg.size()};
   OptParam pw, pb;
-  pw.key = key + ".weight@gemm"; CHK(pw.w = e.upload_f32(wg.data(), wg.size())); pw.g = L->gw; pw.n = (int64_t)wg.size();
-  pw.refresh = 1; pw.dst = L->w; pw.dstT = L->wT; pw.rows = 4 * co; pw.cols = ci;
-  pb.key = key + ".bias@gemm"; pb.w = L->bias; pb.g = L->gb; pb.n = (int64_t)bg.size(); pb.refresh = 6;
-  e.opt_add(pw); e.opt_add(pb);
+  pw.key = key + ".weight@gemm"; pw.n = (int64_t)wg.size(); pw.decoder = true;
+  pw.refresh = Refresh::Cast; pw.dst = L->w; pw.dstT = L->wT; pw.rows = 4 * co; pw.cols = ci;
+  pb.key = key + ".bias"; pb.n = co; pb.decoder = true; pb.refresh = Refresh::TileBias4; pb.dst4 = L->bias;
+  CHK(L->gw = e.train_add(pw, wg.data()));
+  CHK(L->gb = e.train_add(pb, b->data()));
   return 0;
 }
 
@@ -873,27 +867,27 @@ int Engine::dec_train_setup() {
     for (int l = 0; l < 2; ++l) {
       const std::string p = tr + "layers." + std::to_string(l) + ".";
       DLayer& L = d.layer[l];
-      RUN(dt_attn(*this, d, p + "self_attn", 256, &L.self));
-      RUN(dt_attn(*this, d, p + "cross_attn_token_to_image", 128, &L.t2i));
-      RUN(dt_attn(*this, d, p + "cross_attn_image_to_token", 128, &L.i2t));
-      RUN(dt_ln(*this, d, p + "norm1", 256, 1e-5f, &L.n1));
-      RUN(dt_ln(*this, d, p + "norm2", 256, 1e-5f, &L.n2));
-      RUN(dt_ln(*this, d, p + "norm3", 256, 1e-5f, &L.n3));
-      RUN(dt_ln(*this, d, p + "norm4", 256, 1e-5f, &L.n4));
-      RUN(dt_lin(*this, d, p + "mlp.lin1", 2048, 256, &L.mlp1));
-      RUN(dt_lin(*this, d, p + "mlp.lin2", 256, 2048, &L.mlp2));
+      RUN(dt_attn(*this, p + "self_attn", 256, &L.self));
+      RUN(dt_attn(*this, p + "cross_attn_token_to_image", 128, &L.t2i));
+      RUN(dt_attn(*this, p + "cross_attn_image_to_token", 128, &L.i2t));
+      RUN(dt_ln(*this, p + "norm1", 256, 1e-5f, &L.n1));
+      RUN(dt_ln(*this, p + "norm2", 256, 1e-5f, &L.n2));
+      RUN(dt_ln(*this, p + "norm3", 256, 1e-5f, &L.n3));
+      RUN(dt_ln(*this, p + "norm4", 256, 1e-5f, &L.n4));
+      RUN(dt_lin(*this, p + "mlp.lin1", 2048, 256, &L.mlp1));
+      RUN(dt_lin(*this, p + "mlp.lin2", 256, 2048, &L.mlp2));
     }
-    RUN(dt_attn(*this, d, tr + "final_attn_token_to_image", 128, &d.fin));
-    RUN(dt_ln(*this, d, tr + "norm_final_attn", 256, 1e-5f, &d.nfin));
-    RUN(dt_convT(*this, d, m + "output_upscaling.0", 256, 64, &d.ct1));
-    RUN(dt_ln(*this, d, m + "output_upscaling.1", 64, 1e-6f, &d.upln));
-    RUN(dt_convT(*this, d, m + "output_upscaling.3", 64, 32, &d.ct2));
+    RUN(dt_attn(*this, tr + "final_attn_token_to_image", 128, &d.fin));
+    RUN(dt_ln(*this, tr + "norm_final_attn", 256, 1e-5f, &d.nfin));
+    RUN(dt_convT(*this, m + "output_upscaling.0", 256, 64, &d.ct1));
+    RUN(dt_ln(*this, m + "output_upscaling.1", 64, 1e-6f, &d.upln));
+    RUN(dt_convT(*this, m + "output_upscaling.3", 64, 32, &d.ct2));
     for (int i = 0; i < 4; ++i)
       for (int j = 0; j < 3; ++j)
-        RUN(dt_lin(*this, d, m + "output_hypernetworks_mlps." + std::to_string(i) + ".layers." + std::to_string(j), j == 2 ? 32 : 256, 256, &d.hyper[i][j]));
+        RUN(dt_lin(*this, m + "output_hypernetworks_mlps." + std::to_string(i) + ".layers." + std::to_string(j), j == 2 ? 32 : 256, 256, &d.hyper[i][j]));
     for (int j = 0; j < 3; ++j)
-      RUN(dt_lin(*this, d, m + "iou_prediction_head.layers." + std::to_string(j), j == 2 ? 4 : 256, 256, &d.iou[j], 32));
-    // embedding tables
+      RUN(dt_lin(*this, m + "iou_prediction_head.layers." + std::to_string(j), j == 2 ? 4 : 256, 256, &d.iou[j], 32));
+    // embedding tables: the 4 point embeddings and the output tokens (iou token, then the 4 mask tokens) are each one buffer
     std::vector<float> pe(4 * 256), ot(5 * 256);
     for (int i = 0; i < 4; ++i) {
       const auto* w = host("prompt_encoder.point_embeddings." + std::to_string(i) + ".weight", {1, 256});
@@ -911,17 +905,17 @@ int Engine::dec_train_setup() {
     CHK(d.no_mask = up_f32("prompt_encoder.no_mask_embed.weight", {1, 256}));
     CHK(d.g_point_emb = (float*)dalloc(4 * 256 * 4, true));
     CHK(d.g_out_tokens = (float*)dalloc(5 * 256 * 4, true));
-    CHK(d.g_nap = (float*)dalloc(256 * 4, true));
-    CHK(d.g_no_mask = (float*)dalloc(256 * 4, true));
-    d.grads["prompt_encoder.point_embeddings@stack"] = {d.g_point_emb, 4 * 256};
-    d.grads["mask_decoder.output_tokens@stack"] = {d.g_out_tokens, 5 * 256};
-    d.grads["prompt_encoder.not_a_point_embed.weight"] = {d.g_nap, 256};
-    d.grads["prompt_encoder.no_mask_embed.weight"] = {d.g_no_mask, 256};
     OptParam p;
-    p.key = "prompt_encoder.point_embeddings@stack"; p.w = d.point_emb; p.g = d.g_point_emb; p.n = 4 * 256; p.refresh = 5; opt_add(p);
-    p.key = "prompt_encoder.not_a_point_embed.weight"; p.w = d.not_a_point; p.g = d.g_nap; p.n = 256; p.refresh = 5; opt_add(p);
-    p.key = "mask_decoder.output_tokens@stack"; p.w = d.out_tokens; p.g = d.g_out_tokens; p.n = 5 * 256; p.refresh = 0; opt_add(p);
-    p.key = "prompt_encoder.no_mask_embed.weight"; p.w = d.no_mask; p.g = d.g_no_mask; p.n = 256; p.refresh = 0; opt_add(p);
+    p.decoder = true;
+    for (int i = 0; i < 4; ++i) {
+      p.key = "prompt_encoder.point_embeddings." + std::to_string(i) + ".weight"; p.w = d.point_emb + i * 256; p.g = d.g_point_emb + i * 256;
+      p.n = 256;
+      CHK(train_add(p));
+    }
+    p.key = "prompt_encoder.not_a_point_embed.weight"; p.w = d.not_a_point; p.g = nullptr; p.n = 256; CHK(d.g_nap = train_add(p));
+    p.key = m + "iou_token.weight"; p.w = d.out_tokens; p.g = d.g_out_tokens; p.n = 256; CHK(train_add(p));
+    p.key = m + "mask_tokens.weight"; p.w = d.out_tokens + 256; p.g = d.g_out_tokens + 256; p.n = 4 * 256; CHK(train_add(p));
+    p.key = "prompt_encoder.no_mask_embed.weight"; p.w = d.no_mask; p.g = nullptr; p.n = 256; CHK(d.g_no_mask = train_add(p));
     return 0;
   };
   rc = go();
@@ -961,7 +955,7 @@ int Engine::md_setup() {
   return 0;
 }
 
-// the ten tensors join the gradient table and the optimizer (after every tensor registered before); AdamW updates them only after a
+// the ten tensors join the registry (after every tensor registered before); AdamW updates them only after a
 // masked backward has written their gradient since the last msam_decoder_zero_grads (torch.optim.AdamW skips a parameter whose grad
 // is None), with their own step count
 int Engine::md_register() {
@@ -969,11 +963,9 @@ int Engine::md_register() {
   DecTrain& d = *dtrain;
   if (d.md_registered) return 0;
   for (const MdTensor& t : kMdTensors) {
-    const std::string key = kMdPrefix + t.key;
-    d.grads[key] = {d.md_g + t.off, md_numel(t)};
     OptParam p;
-    p.key = key; p.w = d.md_w + t.off; p.g = d.md_g + t.off; p.n = md_numel(t); p.written = &d.md_written;
-    opt_add(p);
+    p.key = kMdPrefix + t.key; p.w = d.md_w + t.off; p.g = d.md_g + t.off; p.n = md_numel(t); p.written = &d.md_written; p.decoder = true;
+    CHK(train_add(p));
   }
   d.md_registered = true;
   return 0;
@@ -1177,15 +1169,6 @@ int Engine::decoder_train_backward(int slot, const float* d_low_res, const float
   return 0;
 }
 
-int Engine::decoder_grad(const char* name, float* dst, int64_t n, cudaStream_t st) {
-  if (!dtrain) return set_error("msam_decoder_grad: decoder training mode was never entered");
-  auto it = dtrain->grads.find(name);
-  if (it == dtrain->grads.end()) return set_error("msam_decoder_grad: no gradient named '%s'", name);
-  if (it->second.second != n) return set_error("msam_decoder_grad: '%s' has %lld elements, caller expects %lld", name, (long long)it->second.second, (long long)n);
-  if (cudaMemcpyAsync(dst, it->second.first, (size_t)n * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess) return set_error("msam_decoder_grad: copy failed");
-  return 0;
-}
-
 void Engine::dec_train_free() {
   if (!dtrain) return;
   for (DecSlot& s : dtrain->slot)
@@ -1196,10 +1179,14 @@ void Engine::dec_train_free() {
 
 int Engine::decoder_zero_grads(cudaStream_t st) {
   if (!dtrain) return 0;
-  for (auto& kv : dtrain->grads)
-    if (cudaMemsetAsync(kv.second.first, 0, (size_t)kv.second.second * 4, st) != cudaSuccess) return set_error("decoder training: memset failed");
+  for (const OptParam& p : opt)
+    if (p.decoder && cudaMemsetAsync(p.g, 0, (size_t)p.n * 4, st) != cudaSuccess) return set_error("decoder training: memset failed");
   dtrain->md_written = false;
   return 0;
+}
+
+int Engine::dec_train_refresh_prompt_tables(cudaStream_t st) {
+  return dtrain ? dec_set_prompt_tables(dtrain->point_emb, dtrain->not_a_point, st) : 0;
 }
 
 }  // namespace msam

@@ -22,18 +22,6 @@ namespace msam {
 #define CHK(p) do { if (!(p)) return -1; } while (0)
 #define RUN(x) do { if (x) return -1; } while (0)
 
-namespace {
-
-// [o][k][c] (GEMM operand of the 3x3 neck conv) gradient -> upstream [o][c][k]
-__global__ void neck2_grad_relayout_kernel(const float* __restrict__ g, int C, float* __restrict__ out) {
-  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (long)C * C * 9) return;
-  const int c = i % C, k = (i / C) % 9, o = i / (9 * C);
-  out[((long)o * C + c) * 9 + k] = g[i];
-}
-
-}  // namespace
-
 struct TrainSave {
   __nv_bfloat16 *qkv_wT = nullptr, *proj_wT = nullptr, *fc1_wT = nullptr, *fc2_wT = nullptr;
   float *g_ln1_g = nullptr, *g_ln1_b = nullptr, *g_ln2_g = nullptr, *g_ln2_b = nullptr, *g_qkv_w = nullptr, *g_qkv_b = nullptr,
@@ -47,21 +35,14 @@ struct TrainState {
   std::vector<TrainSave> blk;
   __nv_bfloat16 *neck1_wT = nullptr, *neck2_wT = nullptr;
   float *g_patch_w = nullptr, *g_patch_b = nullptr, *g_pos = nullptr, *g_neck1_w = nullptr, *g_neck_ln1_g = nullptr, *g_neck_ln1_b = nullptr,
-        *g_neck2_w = nullptr, *g_neck2_w_up = nullptr, *g_neck_ln2_g = nullptr, *g_neck_ln2_b = nullptr;
+        *g_neck2_w = nullptr, *g_neck_ln2_g = nullptr, *g_neck_ln2_b = nullptr;
   // scratch
   float *dx = nullptr, *dxn = nullptr, *dtok = nullptr;
   __nv_bfloat16 *gb = nullptr, *hid = nullptr, *dhid = nullptr, *xn = nullptr, *xn_win = nullptr, *dqkv = nullptr, *do_win = nullptr,
                 *dcol = nullptr;
   float *S = nullptr, *T = nullptr, *dq = nullptr, *dk = nullptr, *dv = nullptr, *drt = nullptr;
   __nv_bfloat16 *P = nullptr, *dS = nullptr, *dT = nullptr;
-  std::unordered_map<std::string, std::pair<float*, int64_t>> grads;   // upstream key -> (device fp32 buffer, elements)
 };
-
-static float* galloc(Engine& e, TrainState& t, const std::string& name, int64_t n) {
-  float* p = (float*)e.dalloc((size_t)n * 4, true);
-  if (p && !name.empty()) t.grads[name] = {p, n};
-  return p;
-}
 
 int Engine::train_setup(cudaStream_t st) {
   if (train) return 0;
@@ -74,78 +55,63 @@ int Engine::train_setup(cudaStream_t st) {
   const std::string e = "image_encoder.";
   t.acts.resize(cfg.depth);
   t.blk.resize(cfg.depth);
-  // optimizer registry (train_opt.cu): fp32 parameters are updated in place, bf16 operands (and their W^T) from fp32 masters
-  auto inplace = [&](const std::string& k, float* w, float* g, int64_t n) { OptParam q; q.key = k; q.w = w; q.g = g; q.n = n; opt_add(q); };
-  auto casted = [&](const std::string& k, float* g, __nv_bfloat16* dst, int rows, int cols, __nv_bfloat16* dstT, int refresh = 1) -> int {
-    OptParam q; q.key = k; q.g = g; q.n = (int64_t)rows * cols; q.refresh = refresh; q.dst = dst; q.dstT = dstT; q.rows = rows; q.cols = cols;
-    CHK(q.w = opt_master_from_host(k, q.n));
-    opt_add(q);
-    return dstT ? launch_transpose_bf16(dst, rows, cols, dstT, st) : 0;
+  // the registry (train_opt.cu): fp32 parameters are their own masters; bf16 operands (and their W^T) are refreshed from fp32 masters
+  auto param = [&](const std::string& k, float* w, int64_t n) { OptParam q; q.key = k; q.w = w; q.n = n; return train_add(q); };
+  auto operand = [&](const std::string& k, __nv_bfloat16* dst, int rows, int cols, __nv_bfloat16* dstT, const float* init = nullptr) -> float* {
+    OptParam q; q.key = k; q.n = (int64_t)rows * cols; q.refresh = Refresh::Cast; q.dst = dst; q.dstT = dstT; q.rows = rows; q.cols = cols;
+    if (dstT && launch_transpose_bf16(dst, rows, cols, dstT, st)) return nullptr;
+    return train_add(q, init);
   };
   for (int i = 0; i < cfg.depth; ++i) {
     VitBlockActs& a = t.acts[i];
     TrainSave& s = t.blk[i];
-    const bool glob = enc.blocks[i].global;
-    const AttnBwdGeom geo = rel_table_geom(glob, cfg.window_size, g);
-    const int S = geo.side;
+    EncBlock& b = enc.blocks[i];
+    const AttnBwdGeom geo = rel_table_geom(b.global, cfg.window_size, g);
     const std::string p = e + "blocks." + std::to_string(i) + ".";
     CHK(a.x_in = (float*)dalloc(M * D * 4));
     CHK(a.x_mid = (float*)dalloc(M * D * 4));
-    CHK(a.qkv = (__nv_bfloat16*)dalloc((glob ? M : Mq) * 3 * D * 2));
+    CHK(a.qkv = (__nv_bfloat16*)dalloc((b.global ? M : Mq) * 3 * D * 2));
     CHK(a.attn = (__nv_bfloat16*)dalloc(M * D * 2));
     CHK(a.pre = (__nv_bfloat16*)dalloc(M * 4 * D * 2));
     CHK(s.qkv_wT = (__nv_bfloat16*)dalloc((size_t)3 * D * D * 2));
     CHK(s.proj_wT = (__nv_bfloat16*)dalloc((size_t)D * D * 2));
     CHK(s.fc1_wT = (__nv_bfloat16*)dalloc((size_t)4 * D * D * 2));
     CHK(s.fc2_wT = (__nv_bfloat16*)dalloc((size_t)4 * D * D * 2));
-    CHK(s.g_ln1_g = galloc(*this, t, p + "norm1.weight", D));
-    CHK(s.g_ln1_b = galloc(*this, t, p + "norm1.bias", D));
-    CHK(s.g_ln2_g = galloc(*this, t, p + "norm2.weight", D));
-    CHK(s.g_ln2_b = galloc(*this, t, p + "norm2.bias", D));
-    CHK(s.g_qkv_w = galloc(*this, t, p + "attn.qkv.weight", (int64_t)3 * D * D));
-    CHK(s.g_qkv_b = galloc(*this, t, p + "attn.qkv.bias", 3 * D));
-    CHK(s.g_proj_w = galloc(*this, t, p + "attn.proj.weight", (int64_t)D * D));
-    CHK(s.g_proj_b = galloc(*this, t, p + "attn.proj.bias", D));
-    CHK(s.g_fc1_w = galloc(*this, t, p + "mlp.lin1.weight", (int64_t)4 * D * D));
-    CHK(s.g_fc1_b = galloc(*this, t, p + "mlp.lin1.bias", 4 * D));
-    CHK(s.g_fc2_w = galloc(*this, t, p + "mlp.lin2.weight", (int64_t)4 * D * D));
-    CHK(s.g_fc2_b = galloc(*this, t, p + "mlp.lin2.bias", D));
-    CHK(s.g_rel_h = galloc(*this, t, p + "attn.rel_pos_h", (int64_t)(2 * S - 1) * hd));
-    CHK(s.g_rel_w = galloc(*this, t, p + "attn.rel_pos_w", (int64_t)(2 * S - 1) * hd));
-    EncBlock& b = enc.blocks[i];
-    inplace(p + "norm1.weight", b.ln1_g, s.g_ln1_g, D); inplace(p + "norm1.bias", b.ln1_b, s.g_ln1_b, D);
-    inplace(p + "norm2.weight", b.ln2_g, s.g_ln2_g, D); inplace(p + "norm2.bias", b.ln2_b, s.g_ln2_b, D);
-    RUN(casted(p + "attn.qkv.weight", s.g_qkv_w, b.qkv_w, 3 * D, D, s.qkv_wT)); inplace(p + "attn.qkv.bias", b.qkv_b, s.g_qkv_b, 3 * D);
-    RUN(casted(p + "attn.proj.weight", s.g_proj_w, b.proj_w, D, D, s.proj_wT)); inplace(p + "attn.proj.bias", b.proj_b, s.g_proj_b, D);
-    RUN(casted(p + "mlp.lin1.weight", s.g_fc1_w, b.fc1_w, 4 * D, D, s.fc1_wT)); inplace(p + "mlp.lin1.bias", b.fc1_b, s.g_fc1_b, 4 * D);
-    RUN(casted(p + "mlp.lin2.weight", s.g_fc2_w, b.fc2_w, D, 4 * D, s.fc2_wT)); inplace(p + "mlp.lin2.bias", b.fc2_b, s.g_fc2_b, D);
+    CHK(s.g_ln1_g = param(p + "norm1.weight", b.ln1_g, D));
+    CHK(s.g_ln1_b = param(p + "norm1.bias", b.ln1_b, D));
+    CHK(s.g_ln2_g = param(p + "norm2.weight", b.ln2_g, D));
+    CHK(s.g_ln2_b = param(p + "norm2.bias", b.ln2_b, D));
+    CHK(s.g_qkv_w = operand(p + "attn.qkv.weight", b.qkv_w, 3 * D, D, s.qkv_wT));
+    CHK(s.g_qkv_b = param(p + "attn.qkv.bias", b.qkv_b, 3 * D));
+    CHK(s.g_proj_w = operand(p + "attn.proj.weight", b.proj_w, D, D, s.proj_wT));
+    CHK(s.g_proj_b = param(p + "attn.proj.bias", b.proj_b, D));
+    CHK(s.g_fc1_w = operand(p + "mlp.lin1.weight", b.fc1_w, 4 * D, D, s.fc1_wT));
+    CHK(s.g_fc1_b = param(p + "mlp.lin1.bias", b.fc1_b, 4 * D));
+    CHK(s.g_fc2_w = operand(p + "mlp.lin2.weight", b.fc2_w, D, 4 * D, s.fc2_wT));
+    CHK(s.g_fc2_b = param(p + "mlp.lin2.bias", b.fc2_b, D));
     for (int hw = 0; hw < 2; ++hw) {
       OptParam q;
-      q.key = p + (hw ? "attn.rel_pos_w" : "attn.rel_pos_h"); q.g = hw ? s.g_rel_w : s.g_rel_h; q.n = (int64_t)(2 * S - 1) * hd;
-      q.refresh = 3; q.dst = b.rel_table; q.rows = 2 * S - 1; q.cols = hd; q.cols_pad = rel_table_cols(hd); q.row_off = hw ? geo.woff : 0;
-      CHK(q.w = opt_master_from_host(q.key, q.n));
-      opt_add(q);
+      q.key = p + (hw ? "attn.rel_pos_w" : "attn.rel_pos_h"); q.n = (int64_t)(2 * geo.side - 1) * hd; q.refresh = Refresh::RelPosRows;
+      q.dst = b.rel_table; q.rows = 2 * geo.side - 1; q.cols = hd; q.cols_pad = rel_table_cols(hd); q.row_off = hw ? geo.woff : 0;
+      CHK((hw ? s.g_rel_w : s.g_rel_h) = train_add(q));
     }
   }
   CHK(t.neck1_wT = (__nv_bfloat16*)dalloc((size_t)C * D * 2));
   CHK(t.neck2_wT = (__nv_bfloat16*)dalloc((size_t)9 * C * C * 2));
-  CHK(t.g_patch_w = galloc(*this, t, e + "patch_embed.proj.weight", (int64_t)D * 768));
-  CHK(t.g_patch_b = galloc(*this, t, e + "patch_embed.proj.bias", D));
-  CHK(t.g_pos = galloc(*this, t, e + "pos_embed", (int64_t)T * D));
-  CHK(t.g_neck1_w = galloc(*this, t, e + "neck.0.weight", (int64_t)C * D));
-  CHK(t.g_neck_ln1_g = galloc(*this, t, e + "neck.1.weight", C));
-  CHK(t.g_neck_ln1_b = galloc(*this, t, e + "neck.1.bias", C));
-  CHK(t.g_neck2_w = galloc(*this, t, "", (int64_t)9 * C * C));
-  CHK(t.g_neck2_w_up = galloc(*this, t, e + "neck.2.weight", (int64_t)9 * C * C));
-  CHK(t.g_neck_ln2_g = galloc(*this, t, e + "neck.3.weight", C));
-  CHK(t.g_neck_ln2_b = galloc(*this, t, e + "neck.3.bias", C));
-  RUN(casted(e + "patch_embed.proj.weight", t.g_patch_w, enc.patch_w, D, 768, nullptr));
-  inplace(e + "patch_embed.proj.bias", enc.patch_b, t.g_patch_b, D);
-  inplace(e + "pos_embed", enc.pos_embed, t.g_pos, (int64_t)T * D);
-  RUN(casted(e + "neck.0.weight", t.g_neck1_w, enc.neck_conv1, C, D, t.neck1_wT));
-  inplace(e + "neck.1.weight", enc.neck_ln1_g, t.g_neck_ln1_g, C); inplace(e + "neck.1.bias", enc.neck_ln1_b, t.g_neck_ln1_b, C);
-  RUN(casted(e + "neck.2.weight", t.g_neck2_w_up, enc.neck_conv2, C, 9 * C, t.neck2_wT, 4));   // refresh 4 reads rows = C
-  inplace(e + "neck.3.weight", enc.neck_ln2_g, t.g_neck_ln2_g, C); inplace(e + "neck.3.bias", enc.neck_ln2_b, t.g_neck_ln2_b, C);
+  CHK(t.g_patch_w = operand(e + "patch_embed.proj.weight", enc.patch_w, D, 768, nullptr));
+  CHK(t.g_patch_b = param(e + "patch_embed.proj.bias", enc.patch_b, D));
+  CHK(t.g_pos = param(e + "pos_embed", enc.pos_embed, (int64_t)T * D));
+  CHK(t.g_neck1_w = operand(e + "neck.0.weight", enc.neck_conv1, C, D, t.neck1_wT));
+  CHK(t.g_neck_ln1_g = param(e + "neck.1.weight", enc.neck_ln1_g, C));
+  CHK(t.g_neck_ln1_b = param(e + "neck.1.bias", enc.neck_ln1_b, C));
+  {   // master and gradient in the implicit GEMM's layout: the gradient is the wgrad GEMM's output itself
+    auto it = dec_host.find(e + "neck.2.weight");
+    if (it == dec_host.end()) return set_error("training: no host copy of '%sneck.2.weight'", e.c_str());
+    const std::vector<float> w = conv3x3_gemm_layout(it->second.data, C);
+    CHK(t.g_neck2_w = operand(e + "neck.2.weight@gemm", enc.neck_conv2, C, 9 * C, t.neck2_wT, w.data()));
+  }
+  CHK(t.g_neck_ln2_g = param(e + "neck.3.weight", enc.neck_ln2_g, C));
+  CHK(t.g_neck_ln2_b = param(e + "neck.3.bias", enc.neck_ln2_b, C));
   // scratch
   const size_t Dm = D > C ? D : C;
   CHK(t.dx = (float*)dalloc(M * Dm * 4));
@@ -282,11 +248,6 @@ int Engine::encode_backward(const float* d_out, cudaStream_t st) {
   RUN(launch_layernorm_bwd(ws.neck2, M, C, enc.neck_ln2_g, 1e-6f, t.dtok, 0, g, cfg.window_size, 0, t.dx, t.g_neck_ln2_g, t.g_neck_ln2_b, st));
   RUN(launch_cast_bf16(t.dx, (long)M * C, t.gb, st));
   RUN(linear_wgrad(t.gb, ws.neck_col, M, C, 9 * C, t.g_neck2_w, nullptr, st));
-  {
-    const long n = (long)C * C * 9;
-    neck2_grad_relayout_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t.g_neck2_w, C, t.g_neck2_w_up);
-    count_launch();
-  }
   RUN(linear_dgrad(*this, t.gb, t.neck2_wT, M, C, 9 * C, t.dcol, 0, st));
   RUN(launch_col2im3x3(t.dcol, B, g, C, t.dtok, st));
   RUN(zero(t.g_neck_ln1_g, C)); RUN(zero(t.g_neck_ln1_b, C));
@@ -340,16 +301,6 @@ int Engine::encode_backward(const float* d_out, cudaStream_t st) {
   RUN(launch_sum_batch(t.dx, B, (long)T * D, t.g_pos, 0, st));
   RUN(launch_cast_bf16(t.dx, (long)M * D, t.gb, st));
   RUN(linear_wgrad(t.gb, ws.patches, M, D, 768, t.g_patch_w, t.g_patch_b, st));
-  return 0;
-}
-
-int Engine::encoder_grad(const char* name, float* dst, int64_t n, cudaStream_t st) {
-  if (!train) return set_error("msam_encoder_grad: training mode was never entered");
-  auto it = train->grads.find(name);
-  if (it == train->grads.end()) return set_error("msam_encoder_grad: no gradient named '%s'", name);
-  if (it->second.second != n) return set_error("msam_encoder_grad: '%s' has %lld elements, caller expects %lld", name, (long long)it->second.second, (long long)n);
-  if (cudaMemcpyAsync(dst, it->second.first, (size_t)n * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
-    return set_error("msam_encoder_grad: copy failed");
   return 0;
 }
 

@@ -164,6 +164,14 @@ float* Engine::up_f32(const std::string& name, std::initializer_list<int64_t> sh
   return h ? upload_f32(h->data(), h->size()) : nullptr;
 }
 
+std::vector<float> conv3x3_gemm_layout(const std::vector<float>& w, int C) {
+  std::vector<float> r((size_t)C * 9 * C);
+  for (int o = 0; o < C; ++o)
+    for (int c = 0; c < C; ++c)
+      for (int k = 0; k < 9; ++k) r[((size_t)o * 9 + k) * C + c] = w[((size_t)o * C + c) * 9 + k];
+  return r;
+}
+
 // ------------------------------------------------------------------------------------------------ weights
 #define CHK(p) do { if (!(p)) return -1; } while (0)
 
@@ -214,10 +222,7 @@ int Engine::finalize_encoder() {
   {
     const auto* w = host(e + "neck.2.weight", {C, C, 3, 3});
     CHK(w);
-    std::vector<float> r((size_t)C * 9 * C);
-    for (int o = 0; o < C; ++o)
-      for (int c = 0; c < C; ++c)
-        for (int k = 0; k < 9; ++k) r[((size_t)o * 9 + k) * C + c] = (*w)[((size_t)o * C + c) * 9 + k];
+    const std::vector<float> r = conv3x3_gemm_layout(*w, C);
     CHK(enc.neck_conv2 = upload_bf16(r.data(), r.size()));
   }
   CHK(enc.neck_ln2_g = up_f32(e + "neck.3.weight", {C}));
@@ -705,10 +710,6 @@ int msam_encode_backward(msam_handle* h, const float* d_out, void* stream) {
   if (!h || !d_out) return set_error("msam_encode_backward: null argument");
   return h->eng.encode_backward(d_out, (cudaStream_t)stream);
 }
-int msam_encoder_grad(msam_handle* h, const char* name, float* dst, int64_t n, void* stream) {
-  if (!h || !name || !dst) return set_error("msam_encoder_grad: null argument");
-  return h->eng.encoder_grad(name, dst, n, (cudaStream_t)stream);
-}
 int msam_decoder_train_forward(msam_handle* h, int slot, const float* emb_nchw, const float* sparse, const int32_t* emb_index, int n_sparse,
                                int P, int multimask, float* low_res, float* iou, void* stream) {
   return msam_decoder_train_forward_ex(h, slot, emb_nchw, sparse, emb_index, n_sparse, P, nullptr, multimask, low_res, iou, stream);
@@ -728,10 +729,6 @@ int msam_decoder_train_backward(msam_handle* h, int slot, const float* d_low_res
   if (!h || !d_emb_nchw) return set_error("msam_decoder_train_backward: null argument");
   return h->eng.decoder_train_backward(slot, d_low_res, d_iou, d_emb_nchw, (cudaStream_t)stream);
 }
-int msam_decoder_grad(msam_handle* h, const char* name, float* dst, int64_t n, void* stream) {
-  if (!h || !name || !dst) return set_error("msam_decoder_grad: null argument");
-  return h->eng.decoder_grad(name, dst, n, (cudaStream_t)stream);
-}
 int msam_decoder_zero_grads(msam_handle* h, void* stream) {
   if (!h) return set_error("msam_decoder_zero_grads: null handle");
   return h->eng.decoder_zero_grads((cudaStream_t)stream);
@@ -743,10 +740,6 @@ int msam_mask_loss_backward(const float* low_res, const uint8_t* targets, const 
 int msam_optimizer_step(msam_handle* h, float lr, float beta1, float beta2, float eps, float weight_decay, void* stream) {
   if (!h) return set_error("msam_optimizer_step: null handle");
   return h->eng.optimizer_step(lr, beta1, beta2, eps, weight_decay, (cudaStream_t)stream);
-}
-int msam_train_param(msam_handle* h, const char* key, float* dst, int64_t n, void* stream) {
-  if (!h || !key || !dst) return set_error("msam_train_param: null argument");
-  return h->eng.train_param(key, dst, n, (cudaStream_t)stream);
 }
 int msam_train_tensor_count(msam_handle* h) { return h ? (int)h->eng.opt.size() : -1; }
 int msam_train_tensor_info(msam_handle* h, int i, char* key_buf, int cap, void** grad, void** master, int64_t* n) {

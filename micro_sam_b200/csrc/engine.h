@@ -72,20 +72,34 @@ struct TinyVit {
   float *x = nullptr, *x2 = nullptr;
 };
 
-// One trainable tensor of the optimizer (train_opt.cu): fp32 master weights (the live parameter buffer itself when the kernels read
-// fp32: biases, LayerNorm, embedding tables), its gradient, AdamW moments, and how the packed operands are refreshed after an update.
+// How the operand a kernel reads is rebuilt from an updated fp32 master (train_opt.cu)
+enum class Refresh {
+  None,        // the kernels read the master itself
+  Cast,        // dst [n] = bf16(master)
+  RelPosRows,  // rows [row_off, row_off + rows) of the bf16 rel-pos table dst [*, cols_pad] = master [rows, cols]
+  TileBias4,   // dst4 [4, n] = master [n] repeated: a conv-transpose bias as the GEMM epilogue reads it, one tile per sub-pixel
+};
+
+// One trainable tensor (the registry Engine::opt, train_opt.cu): fp32 master weights (the live parameter buffer itself when the
+// kernels read fp32: biases, LayerNorm, embedding tables), its gradient, AdamW moments, and how the operands are refreshed after
+// an update.  Every entry is an upstream tensor with its upstream element count; a key "<name>@gemm" holds it in the GEMM layout
+// of its convolution, a permutation of the upstream layout (micro_sam_b200/sam.py:B200Sam._upstream).
 struct OptParam {
-  std::string key;              // gradient key: upstream name, or "<name>@gemm" / "@stack" for packed layouts
+  std::string key;
   float *w = nullptr, *g = nullptr, *m = nullptr, *v = nullptr;
   int64_t n = 0;
+  bool decoder = false;           // the gradient accumulates until msam_decoder_zero_grads; else msam_encode_backward overwrites it
   const bool* written = nullptr;  // non-null: AdamW skips the tensor while *written is false (no gradient since the last zeroing)
   int64_t steps = 0;              // ... and counts its own steps for the bias correction (with written only)
-  int refresh = 0;              // 0 none | 1 cast -> dst | 3 rows of a rel-pos table | 4 neck 3x3 conv relayout | 5 prompt-encoder
-                                // tables of the inference decoder | 6 conv-transpose bias (fold the 4 tiles first)
+  Refresh refresh = Refresh::None;
   __nv_bfloat16 *dst = nullptr;
   __nv_bfloat16* dstT = nullptr;  // non-null: after the refresh, dstT [cols, rows] = dst [rows, cols]^T (W^T of the dgrad GEMMs)
+  float* dst4 = nullptr;
   int rows = 0, cols = 0, cols_pad = 0, row_off = 0;
 };
+
+// 3x3 conv weight [o][c][ky][kx] -> the layout of its implicit GEMM, [o][ky * 3 + kx][c] (engine.cu)
+std::vector<float> conv3x3_gemm_layout(const std::vector<float>& w, int C);
 
 struct DecoderState;  // decoder.cu
 struct TrainState;    // encoder_train.cu
@@ -129,11 +143,10 @@ struct Engine {
   // blocks, no neck (the fp32 residual stream is left in ws.x).  keep: null for inference, else one VitBlockActs per block.
   int vit_forward(const uint8_t* u8, const float* f32, int nb, int hh, int ww, const VitBlockActs* keep, float* out, cudaStream_t st,
                   int stop_after = -1);
-  // encoder_train.cu (cfg 5): forward keeping activations, backward, gradient read-out by upstream key name
+  // encoder_train.cu (cfg 5): forward keeping activations, backward
   int train_setup(cudaStream_t st);
   int encode_train(const float* f32, int B, float* out, cudaStream_t st);
   int encode_backward(const float* d_out, cudaStream_t st);
-  int encoder_grad(const char* name, float* dst, int64_t n, cudaStream_t st);
   void train_invalidate();
   void train_free();       // encoder_train.cu: host-side training state (device buffers are in `allocs`)
   void dec_train_free();   // decoder_train.cu: per-slot arenas + host-side state
@@ -142,18 +155,18 @@ struct Engine {
   int decoder_train_forward(int slot, const float* emb_nchw, const float* sparse, const int* emb_index, int Ts, int P,
                             const float* mask_in, int multimask, float* low_res, float* iou, cudaStream_t st);
   int decoder_train_backward(int slot, const float* d_low_res, const float* d_iou, float* d_emb_nchw, cudaStream_t st);
-  int decoder_grad(const char* name, float* dst, int64_t n, cudaStream_t st);
   int decoder_zero_grads(cudaStream_t st);
+  int dec_train_refresh_prompt_tables(cudaStream_t st);   // the inference prompt encoder's tables <- the training masters
   int md_setup();      // mask_downscaling masters + gradient buffer
-  int md_register();   // ... joining the gradient table and the optimizer (first masked training forward)
+  int md_register();   // ... joining the registry (first masked training forward)
   int op_mask_downscaling_train(const float* mask, int P, const float* d_dense, float* dense_out, float* grads_out, cudaStream_t st);
   const float* dec_pos();   // decoder.cu: dense positional encoding, token-major [4096, 256] fp32
   int dec_set_prompt_tables(const float* point_emb_4x256, const float* not_a_point, cudaStream_t st);   // decoder.cu
-  // train_opt.cu: AdamW over every registered tensor + refresh of the packed operands; read-out of the master weights
-  float* opt_master_from_host(const std::string& key, int64_t n);
-  void opt_add(const OptParam& p) { opt.push_back(p); }
+  // train_opt.cu: registration of a trainable tensor, AdamW over every registered tensor + refresh of the operands.
+  // train_add returns the gradient buffer of p, or null on error.  p.g null: a zeroed buffer of p.n floats is allocated.
+  // p.w null: the master is an fp32 upload of p.n floats from `init`, or from the host copy dec_host[p.key] when init is null.
+  float* train_add(OptParam p, const float* init = nullptr);
   int optimizer_step(float lr, float beta1, float beta2, float eps, float weight_decay, cudaStream_t st);
-  int train_param(const char* key, float* dst, int64_t n, cudaStream_t st);
   int set_image_embedding(const float* feat, cudaStream_t st);  // decoder.cu
   int decode(const float* points, const float* labels, int np, const float* boxes, const float* mask_in, int P, int multimask,
              float* low_res, float* iou, cudaStream_t st);  // decoder.cu

@@ -141,6 +141,9 @@ def _device_view(ptr: int, n: int, device) -> torch.Tensor:
     return torch.as_tensor(_DevBuf(ptr, n), device=device)
 
 
+_DECODER_PREFIXES = ("mask_decoder.", "prompt_encoder.")
+
+
 class _DecoderFn(torch.autograd.Function):
     """prompt encoder + mask decoder of ONE image with a backward pass (csrc/decoder_train.cu): (embedding [256,64,64], sparse prompt
     embeddings [P,Ts,256], mask prompts [P,1,256,256] or None) -> (low-res logits [P,M,256,256], IoU predictions [P,M]).  backward
@@ -425,52 +428,43 @@ class B200Sam:
         with mask prompts has run."""
         if not getattr(self, "_decoder_grads_valid", False):
             raise RuntimeError("no decoder gradients: run decoder_train(...) and backward() first")
-        return self._decoder_tensors(_lib.lib().msam_decoder_grad)
+        return self._upstream(lambda k: k.startswith(_DECODER_PREFIXES), master=False)
 
-    def _decoder_tensors(self, getter, params: bool = False) -> Dict[str, torch.Tensor]:
-        """Decoder / prompt-encoder tensors (gradients or master weights) from the engine's packed layouts to upstream keys / shapes."""
-        def fetch(name, n):
-            g = torch.empty(n, device=self.device, dtype=torch.float32)
-            _lib.check(getter(self._h, name.encode(), _lib.ptr(g), n, _lib.cur_stream()))
-            return g
+    def _registry(self):
+        """[(key, gradient, master)]: zero-copy fp32 views of every trainable tensor of the engine (msam_train_tensor_info)."""
+        L = _lib.lib()
+        out = []
+        buf = ctypes.create_string_buffer(256)
+        for i in range(max(L.msam_train_tensor_count(self._h), 0)):
+            g, w, cnt = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_int64()
+            _lib.check(L.msam_train_tensor_info(self._h, i, buf, 256, ctypes.byref(g), ctypes.byref(w), ctypes.byref(cnt)))
+            out.append((buf.value.decode(), _device_view(g.value, cnt.value, self.device), _device_view(w.value, cnt.value, self.device)))
+        return out
+
+    def _upstream(self, keep, master: bool) -> Dict[str, torch.Tensor]:
+        """Copies of the registered gradients (or, master=True, fp32 master weights) whose upstream key passes `keep`, keyed and
+        shaped like the upstream state dict.  A "<name>@gemm" tensor is its convolution's weight in the layout of its GEMM, a
+        permutation of the upstream one: ConvTranspose2d [ci, co, 2, 2] as [(dy, dx, co), ci], Conv2d [o, c, 3, 3] as [o, (ky, kx), c]."""
         out = {}
-        for k, v in self._state.items():
-            if not (k.startswith("mask_decoder.") or k.startswith("prompt_encoder.")):
+        for key, g, w in self._registry():
+            k = key.removesuffix("@gemm")
+            if not keep(k) or ("mask_downscaling" in k and not self._mask_grads_valid):
                 continue
-            if k.endswith("positional_encoding_gaussian_matrix") or ("mask_downscaling" in k and not self._mask_grads_valid):
-                continue
-            if "output_upscaling.0" in k or "output_upscaling.3" in k:       # ConvTranspose2d [ci, co, 2, 2] <- GEMM layout [(dy,dx,co), ci]
-                ci, co = self._state[k.rsplit(".", 1)[0] + ".weight"].shape[:2]
-                if k.endswith(".weight"):
-                    out[k] = fetch(k + "@gemm", 4 * co * ci).view(2, 2, co, ci).permute(3, 2, 0, 1).contiguous()
-                else:
-                    t4 = fetch(k + "@gemm", 4 * co).view(4, co)      # the bias is kept as 4 identical tiles, its gradient as 4 partial sums
-                    out[k] = t4[0].clone() if params else t4.sum(0)
-            elif "point_embeddings" in k:
-                i = int(k.split(".")[2])
-                out[k] = fetch("prompt_encoder.point_embeddings@stack", 4 * 256).view(4, 1, 256)[i]
-            elif k == "mask_decoder.iou_token.weight":
-                out[k] = fetch("mask_decoder.output_tokens@stack", 5 * 256).view(5, 256)[:1]
-            elif k == "mask_decoder.mask_tokens.weight":
-                out[k] = fetch("mask_decoder.output_tokens@stack", 5 * 256).view(5, 256)[1:]
-            elif k.startswith("mask_decoder.iou_prediction_head.layers.2."):   # 4 outputs padded to 32 GEMM columns
-                out[k] = (fetch(k, 32 * 256).view(32, 256)[:4] if k.endswith(".weight") else fetch(k, 32)[:4]).contiguous()
+            t, shape = (w if master else g), self._state[k].shape
+            if k == key:
+                t = t.view(shape)
+            elif shape[2] == 2:
+                t = t.view(2, 2, shape[1], shape[0]).permute(3, 2, 0, 1)
             else:
-                out[k] = fetch(k, v.numel()).view(v.shape)
+                t = t.view(shape[0], 3, 3, shape[1]).permute(0, 3, 1, 2)
+            out[k] = t.clone(memory_format=torch.contiguous_format)
         return out
 
     def grad_views(self):
-        """Zero-copy torch views of the engine's fp32 gradient buffers [(key, tensor)] (keys as in the C API: a few carry packed
-        layouts, `@gemm` / `@stack`).  In-place operations on them (all-reduce, clipping, scaling) are seen by `optimizer_step()`."""
-        L = _lib.lib()
-        n = L.msam_train_tensor_count(self._h)
-        out = []
-        buf = ctypes.create_string_buffer(256)
-        for i in range(max(n, 0)):
-            g, w, cnt = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_int64()
-            _lib.check(L.msam_train_tensor_info(self._h, i, buf, 256, ctypes.byref(g), ctypes.byref(w), ctypes.byref(cnt)))
-            out.append((buf.value.decode(), _device_view(g.value, cnt.value, self.device)))
-        return out
+        """Zero-copy torch views of the engine's fp32 gradient buffers [(key, tensor)], one per trainable tensor with its upstream
+        element count; three convolution weights are held in their GEMM layout under "<name>@gemm" (see `_upstream`).  In-place
+        operations on them (all-reduce, clipping, scaling) are seen by `optimizer_step()`, which itself writes none of them."""
+        return [(k, g) for k, g, _ in self._registry()]
 
     def allreduce_grads(self, world_size: int) -> int:
         """DDP semantics (micro_sam/training/training.py:train_sam): average every gradient over the ranks with ONE all-reduce of a
@@ -486,31 +480,17 @@ class B200Sam:
 
     def trained_state_dict(self) -> Dict[str, torch.Tensor]:
         """Upstream-keyed state dict with the fp32 master weights of the optimizer (CPU tensors); untouched tensors as loaded."""
-        L = _lib.lib()
+        dec, enc = getattr(self, "_decoder_grads_valid", False), getattr(self, "_encoder_grads_valid", False)
         out = dict(self._state)
-        if getattr(self, "_decoder_grads_valid", False):
-            out.update({k: v.cpu() for k, v in self._decoder_tensors(L.msam_train_param, params=True).items()})
-        if getattr(self, "_encoder_grads_valid", False):
-            for k, v in self._state.items():
-                if k.startswith("image_encoder."):
-                    g = torch.empty(v.shape, device=self.device, dtype=torch.float32)
-                    _lib.check(L.msam_train_param(self._h, k.encode(), _lib.ptr(g), g.numel(), _lib.cur_stream()))
-                    out[k] = g.cpu()
+        out.update({k: v.cpu() for k, v in self._upstream(
+            lambda k: (dec and k.startswith(_DECODER_PREFIXES)) or (enc and k.startswith("image_encoder.")), master=True).items()})
         return out
 
     def encoder_grads(self, names=None) -> Dict[str, torch.Tensor]:
         """fp32 gradients of the image-encoder parameters after a backward pass, keyed and shaped like the upstream state dict."""
         if not getattr(self, "_encoder_grads_valid", False):
             raise RuntimeError("no encoder gradients: run image_encoder(x) in train() mode and call backward() first")
-        out = {}
-        L = _lib.lib()
-        for k, v in self._state.items():
-            if not k.startswith("image_encoder.") or (names is not None and k not in names):
-                continue
-            g = torch.empty(v.shape, device=self.device, dtype=torch.float32)
-            _lib.check(L.msam_encoder_grad(self._h, k.encode(), _lib.ptr(g), g.numel(), _lib.cur_stream()))
-            out[k] = g
-        return out
+        return self._upstream(lambda k: k.startswith("image_encoder.") and (names is None or k in names), master=False)
 
     def bind_embedding(self, f: torch.Tensor) -> None:
         """Bind a (1,256,64,64) image embedding as the decoder's current image (SamPredictor.features assignment).  The

@@ -11,7 +11,7 @@ nearly orthogonal to the gradient and averages out of it, while a scaled or part
 tensor, so the bounds are per family of tensors (decoder_train_mirror.GRAD_BOUNDS).
 
 Each case goes through `B200Sam.decoder_train` (prompt encoder on the GPU; T = 5 + n_sparse) and compares low_res, iou,
-dL/d embedding and every tensor of `decoder_grads()` (which also checks the folding of the packed `@gemm` / `@stack` layouts) with
+dL/d embedding and every tensor of `decoder_grads()` (which also checks the unpacking of the `@gemm` layouts) with
 the mirror fed the GPU's own sparse prompt embeddings and dense positional encoding.  Metrics: rel-L2 and the worst per-row error
 for the outputs (rows: prompts x masks x logit rows, prompts, embedding channels); rel-L2 and |slope - 1| for a gradient.
 Gradients that are analytically zero (k_proj biases; tensors the prompts do not reach) are compared absolutely, against the
