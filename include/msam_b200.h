@@ -185,6 +185,13 @@ int msam_mask_nms(const uint8_t* masks, int n, int h, int w, const float* boxes_
  * out bf16 (out_fp32=0) or fp32; act: 0 none, 1 GELU(erf), 2 ReLU. */
 int msam_op_gemm(const void* A, const void* W, int M, int N, int K, const float* bias, const float* residual,
                  int res_rows, void* out, int out_fp32, int act, void* stream);
+/* The same kernel with every field of its argument block (csrc/kernels.h:GemmArgs): row pitches lda / ldw (>= K, multiples of 8),
+ * ldc / ldr (0 = N; ldc even), residual fp32 or bf16 (res_bf16) indexed by row % res_rows (0 = M), act_after_res = apply `act` after
+ * the residual add, epi = 1: LayerNorm over the N = 256 columns of each row (ln_gamma / ln_beta / ln_eps; bf16 out, bf16 residual or
+ * none, no act).  num_sms caps the grid of the persistent kernel (<= 0 = the device's SM count): results must not depend on it. */
+int msam_op_gemm_ex(const void* A, const void* W, int M, int N, int K, int lda, int ldw, const float* bias, const void* residual,
+                    int res_rows, int ldr, int res_bf16, void* out, int ldc, int out_fp32, int act, int act_after_res, int epi,
+                    const float* ln_gamma, const float* ln_beta, float ln_eps, int num_sms, void* stream);
 /* Weight gradient of a linear layer (first piece of msam_*_backward, cfg 5): out[M,N] fp32 = A[K,M]^T B[K,N], A = dY
  * (tokens x out-features), B = X (tokens x in-features), both bf16 row-major -- torch autograd's dW = dY^T X. */
 int msam_op_gemm_tn(const void* A, const void* B, int M, int N, int K, float* out, void* stream);
@@ -271,6 +278,31 @@ int msam_op_bgemm(const void* A, const void* B, int a_mn, int b_mn, int M, int N
 /* LayerNorm backward over fp32 rows (csrc/backward.cu); dgamma / dbeta are ACCUMULATED into (zero them first). */
 int msam_op_layernorm_bwd(const float* x, int rows, int D, const float* gamma, float eps, const float* dy, int window_mode,
                           int accumulate, float* dx, float* dgamma, float* dbeta, void* stream);
+/* Row-wise / element-wise stages of the encoder backward pass (csrc/backward.cu), exposed for the op-level tests.  `global` selects
+ * the geometry of csrc/kernels.h:rel_table_geom: 0 = 14 x 14 window (196 keys, T rows of nt = 64 columns, rel_pos_w at woff = 32),
+ * 1 = 64 x 64 global (4096 keys, nt = 256, woff = 128).  n_batch = (windows | images) * heads; a batch entry has n_tok query rows.
+ * attn_probs: P[row, :pitch_p] bf16 = softmax_k(scale * S[row, k] + T[row, qh - kh + side - 1] + T[row, woff + qw - kw + side - 1]),
+ * zero in columns [n_tok, pitch_p); S fp32 rows of pitch_s, T fp32 rows of nt.
+ * attn_ds: dS = P o (dP - sum_k P dP) (bf16, pitch_p, zero pad columns) and dT bf16 rows of nt = the bias gradient summed into the
+ * table-row index of each key (every other entry zero). */
+int msam_op_attn_probs(const float* S, const float* T, int64_t n_batch, int global, int pitch_s, int pitch_p, float scale, void* P_bf16,
+                       void* stream);
+int msam_op_attn_ds(const void* P_bf16, const float* dP, int64_t n_batch, int global, int pitch_s, int pitch_p, void* dS_bf16,
+                    void* dT_bf16, void* stream);
+/* dq / dk / dv fp32 [outer, heads, T, d] -> dqkv bf16 [outer * T, 3 * heads * d]; d % 4 == 0. */
+int msam_op_pack_dqkv(const float* dq, const float* dk, const float* dv, int outer, int heads, int T, int d, void* dqkv_bf16, void* stream);
+/* dpre = dh * GELU'(pre) (exact erf form), bf16, n % 8 == 0; dpre may alias dh. */
+int msam_op_gelu_bwd(const void* dh_bf16, const void* pre_bf16, int64_t n, void* dpre_bf16, void* stream);
+/* out[N] fp32 += column sums of bf16 x[rows, N] (bias gradients). */
+int msam_op_colsum(const void* x_bf16, int64_t rows, int N, float* out, void* stream);
+/* image-order bf16 [B * 4096, D] -> 14 x 14 window-partitioned [B * 25 * 196, D], zero pad rows; D % 8 == 0. */
+int msam_op_window_gather(const void* x_bf16, int B, int D, void* out_win_bf16, void* stream);
+/* Adjoint of the 3 x 3 / pad 1 im2col of the neck: dcol bf16 [B * g * g, 9 * C] -> out fp32 [B * g * g, C]; C % 8 == 0. */
+int msam_op_col2im3x3(const void* dcol_bf16, int B, int g, int C, float* out, void* stream);
+/* out[n] (+)= sum_b x[b, n], fp32. */
+int msam_op_sum_batch(const float* x, int64_t n_batch, int64_t n, float* out, int accumulate, void* stream);
+/* out bf16 [cols, rows] = in [rows, cols]^T. */
+int msam_op_transpose_bf16(const void* in_bf16, int rows, int cols, void* out_bf16, void* stream);
 /* Training prompts (csrc/prompts.cu).  Random draws come from Philox4x32-10 keyed by `seed`, counter (image, object, draw): the
  * result depends on the seed and the inputs only.
  *

@@ -94,6 +94,17 @@ def lib() -> ctypes.CDLL:
         L.msam_op_layernorm_bwd.argtypes = [c_void_p, c_int, c_int, c_void_p, c_float, c_void_p, c_int, c_int, c_void_p, c_void_p,
                                             c_void_p, c_void_p]
         L.msam_debug_attn_trace.argtypes = [c_void_p]
+        L.msam_op_gemm_ex.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
+                                      c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_void_p]
+        L.msam_op_attn_probs.argtypes = [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_float, c_void_p, c_void_p]
+        L.msam_op_attn_ds.argtypes = [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]
+        L.msam_op_pack_dqkv.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
+        L.msam_op_gelu_bwd.argtypes = [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]
+        L.msam_op_colsum.argtypes = [c_void_p, c_int64, c_int, c_void_p, c_void_p]
+        L.msam_op_window_gather.argtypes = [c_void_p, c_int, c_int, c_void_p, c_void_p]
+        L.msam_op_col2im3x3.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]
+        L.msam_op_sum_batch.argtypes = [c_void_p, c_int64, c_int64, c_void_p, c_int, c_void_p]
+        L.msam_op_transpose_bf16.argtypes = [c_void_p, c_int, c_int, c_void_p, c_void_p]
         L.msam_decoder_train_forward.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
                                                  c_void_p]
         L.msam_decoder_train_forward_ex.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p,

@@ -658,6 +658,20 @@ int msam_op_gemm(const void* A, const void* W, int M, int N, int K, const float*
   return launch_gemm(a, sm_count(), (cudaStream_t)stream);
 }
 
+int msam_op_gemm_ex(const void* A, const void* W, int M, int N, int K, int lda, int ldw, const float* bias, const void* residual,
+                    int res_rows, int ldr, int res_bf16, void* out, int ldc, int out_fp32, int act, int act_after_res, int epi,
+                    const float* ln_gamma, const float* ln_beta, float ln_eps, int num_sms, void* stream) {
+  if (!A || !W || !out) return set_error("msam_op_gemm_ex: null argument");
+  if (lda < K || ldw < K) return set_error("msam_op_gemm_ex: lda=%d / ldw=%d below K=%d", lda, ldw, K);
+  if ((ldc > 0 && ldc < N) || (ldr > 0 && ldr < N)) return set_error("msam_op_gemm_ex: ldc=%d / ldr=%d below N=%d", ldc, ldr, N);
+  GemmArgs a;
+  a.A = (const __nv_bfloat16*)A; a.W = (const __nv_bfloat16*)W; a.M = M; a.N = N; a.K = K; a.lda = lda; a.ldw = ldw;
+  a.bias = bias; a.residual = residual; a.res_rows = res_rows; a.ldr = ldr; a.res_bf16 = res_bf16;
+  a.out = out; a.ldc = ldc; a.out_fp32 = out_fp32; a.act = act; a.act_after_res = act_after_res;
+  a.epi = epi; a.ln_gamma = ln_gamma; a.ln_beta = ln_beta; a.ln_eps = ln_eps;
+  return launch_gemm(a, num_sms > 0 ? num_sms : sm_count(), (cudaStream_t)stream);
+}
+
 int msam_op_gemm_tn(const void* A, const void* B, int M, int N, int K, float* out, void* stream) {
   if (!A || !B || !out) return set_error("msam_op_gemm_tn: null argument");
   return launch_gemm_tn((const __nv_bfloat16*)A, (const __nv_bfloat16*)B, M, N, K, M, N, out, N, (cudaStream_t)stream);
@@ -764,6 +778,63 @@ int msam_op_bgemm(const void* A, const void* B, int a_mn, int b_mn, int M, int N
 int msam_op_layernorm_bwd(const float* x, int rows, int D, const float* gamma, float eps, const float* dy, int window_mode,
                           int accumulate, float* dx, float* dgamma, float* dbeta, void* stream) {
   return launch_layernorm_bwd(x, rows, D, gamma, eps, dy, window_mode, 64, 14, accumulate, dx, dgamma, dbeta, (cudaStream_t)stream);
+}
+
+// ---- element-wise / row-wise stages of the encoder backward pass (backward.cu), one entry point per launcher
+static int attn_bwd_pitches_ok(const char* who, const AttnBwdGeom& g, long n_batch, int pitch_s, int pitch_p) {
+  if (n_batch <= 0) return set_error("%s: n_batch=%ld", who, n_batch);
+  if (pitch_s < g.n_tok || pitch_p < g.n_tok) return set_error("%s: pitch_s=%d / pitch_p=%d below %d keys", who, pitch_s, pitch_p, g.n_tok);
+  return 0;
+}
+int msam_op_attn_probs(const float* S, const float* T, int64_t n_batch, int global, int pitch_s, int pitch_p, float scale, void* P,
+                       void* stream) {
+  if (!S || !T || !P) return set_error("msam_op_attn_probs: null argument");
+  const AttnBwdGeom g = rel_table_geom(global != 0, 14, 64);
+  if (attn_bwd_pitches_ok("msam_op_attn_probs", g, (long)n_batch, pitch_s, pitch_p)) return -1;
+  return launch_attn_probs(S, T, (long)n_batch, g, pitch_s, pitch_p, scale, (__nv_bfloat16*)P, (cudaStream_t)stream);
+}
+int msam_op_attn_ds(const void* P, const float* dP, int64_t n_batch, int global, int pitch_s, int pitch_p, void* dS, void* dT,
+                    void* stream) {
+  if (!P || !dP || !dS || !dT) return set_error("msam_op_attn_ds: null argument");
+  const AttnBwdGeom g = rel_table_geom(global != 0, 14, 64);
+  if (attn_bwd_pitches_ok("msam_op_attn_ds", g, (long)n_batch, pitch_s, pitch_p)) return -1;
+  return launch_attn_ds((const __nv_bfloat16*)P, dP, (long)n_batch, g, pitch_s, pitch_p, (__nv_bfloat16*)dS, (__nv_bfloat16*)dT,
+                        (cudaStream_t)stream);
+}
+int msam_op_pack_dqkv(const float* dq, const float* dk, const float* dv, int outer, int heads, int T, int d, void* dqkv, void* stream) {
+  if (!dq || !dk || !dv || !dqkv) return set_error("msam_op_pack_dqkv: null argument");
+  if (outer <= 0 || heads <= 0 || T <= 0 || d <= 0 || d % 4) return set_error("msam_op_pack_dqkv: d=%d must be a positive multiple of 4", d);
+  return launch_pack_dqkv(dq, dk, dv, outer, heads, T, d, (__nv_bfloat16*)dqkv, (cudaStream_t)stream);
+}
+int msam_op_gelu_bwd(const void* dh, const void* pre, int64_t n, void* dpre, void* stream) {
+  if (!dh || !pre || !dpre) return set_error("msam_op_gelu_bwd: null argument");
+  if (n <= 0) return set_error("msam_op_gelu_bwd: n=%lld", (long long)n);
+  return launch_gelu_bwd((const __nv_bfloat16*)dh, (const __nv_bfloat16*)pre, (long)n, (__nv_bfloat16*)dpre, (cudaStream_t)stream);
+}
+int msam_op_colsum(const void* x, int64_t rows, int N, float* out, void* stream) {
+  if (!x || !out) return set_error("msam_op_colsum: null argument");
+  if (rows <= 0 || N <= 0) return set_error("msam_op_colsum: rows=%lld N=%d", (long long)rows, N);
+  return launch_colsum((const __nv_bfloat16*)x, (long)rows, N, out, (cudaStream_t)stream);
+}
+int msam_op_window_gather(const void* x, int B, int D, void* out_win, void* stream) {
+  if (!x || !out_win) return set_error("msam_op_window_gather: null argument");
+  if (B <= 0 || D <= 0 || D % 8) return set_error("msam_op_window_gather: D=%d must be a positive multiple of 8", D);
+  return launch_window_gather((const __nv_bfloat16*)x, B, 64, 14, D, (__nv_bfloat16*)out_win, (cudaStream_t)stream);
+}
+int msam_op_col2im3x3(const void* dcol, int B, int g, int C, float* out, void* stream) {
+  if (!dcol || !out) return set_error("msam_op_col2im3x3: null argument");
+  if (B <= 0 || g <= 0 || C <= 0 || C % 8) return set_error("msam_op_col2im3x3: C=%d must be a positive multiple of 8", C);
+  return launch_col2im3x3((const __nv_bfloat16*)dcol, B, g, C, out, (cudaStream_t)stream);
+}
+int msam_op_sum_batch(const float* x, int64_t n_batch, int64_t n, float* out, int accumulate, void* stream) {
+  if (!x || !out) return set_error("msam_op_sum_batch: null argument");
+  if (n_batch <= 0 || n <= 0) return set_error("msam_op_sum_batch: n_batch=%lld n=%lld", (long long)n_batch, (long long)n);
+  return launch_sum_batch(x, (long)n_batch, (long)n, out, accumulate, (cudaStream_t)stream);
+}
+int msam_op_transpose_bf16(const void* in, int rows, int cols, void* out, void* stream) {
+  if (!in || !out) return set_error("msam_op_transpose_bf16: null argument");
+  if (rows <= 0 || cols <= 0) return set_error("msam_op_transpose_bf16: rows=%d cols=%d", rows, cols);
+  return launch_transpose_bf16((const __nv_bfloat16*)in, rows, cols, (__nv_bfloat16*)out, (cudaStream_t)stream);
 }
 
 // debug hook: device buffer of 64 x 16 uint64 phase timestamps, or NULL to switch off
