@@ -327,6 +327,26 @@ int msam_prompt_sample_points(const uint8_t* targets, const int32_t* counts, con
 int msam_prompt_iterative(const uint8_t* targets, const float* low_res, const float* iou, int M, const uint8_t* pred, int n,
                           int n_per_img, int in_h, int in_w, int orig_h, int orig_w, uint64_t seed, int32_t* coords, int32_t* labels,
                           void* stream);
+/* segment_from_mask's mask -> prompt derivation on the device (csrc/volume.cu; prompt_based_segmentation.py:24-101 here,
+ * micro_sam/prompt_based_segmentation.py:28-140 upstream), for multi_dimensional_segmentation.segment_mask_in_volume.
+ * mask: uint8 [H, W] with row pitch ld >= W (a tile's outer block may be a view into a larger frame); pixels == 1 are the
+ * object.  H, W <= 8192; with want_logits, shapes whose resize to the longest side 256 needs more than 72 taps per output
+ * pixel (2 * ceil(in / out) + 1, e.g. 8192 x 111) are refused.  workspace: msam_mask_prompts_workspace(H, W) bytes of device memory.
+ * stats int64 [12]: count, sum_y, sum_x, (y0, x0, y1, x1) python box of the object (exclusive ends), (x0, y0, x1, y1) the
+ * _process_box(box_extension) box (rounded half to even, clipped to the mask), n_points (-1: more than 8192 peak candidates).
+ * box1024 fp32 [4] (or NULL): that box through ResizeLongestSide(1024).apply_boxes for original size (H, W).
+ * want_logits: logits fp32 [256, 256] = _compute_logits_from_mask, bit-identical to torch's CPU antialiased resize.
+ * point_mode 0: none; 1: use_single_point; 2: _compute_points_from_mask's inner (d = 3) + outer (d = 5) peaks.  points fp32
+ * [max_points, 2] (x, y) in the 1024 frame, labels fp32 [max_points] (1 / 0); only the first max_points are written, stats[11]
+ * holds the full count.  field fp32 [H * W] (or NULL): the smoothed distance field of the box crop, row-major with the crop's
+ * width as pitch.  An empty mask gives count 0, zero boxes, no points and all -hi logits. */
+int64_t msam_mask_prompts_workspace(int H, int W);
+int msam_mask_prompts(const uint8_t* mask, int H, int W, int ld, double box_extension, int want_logits, int point_mode, int max_points,
+                      void* workspace, int64_t ws_bytes, int64_t* stats, float* box1024, float* logits, float* points, float* labels,
+                      float* field, void* stream);
+/* util.compute_iou's counts (micro_sam/util.py:1266-1280): counts int64 [2] = (|a == 1 & b == 1|, |a == 1 | b == 1|) of two
+ * uint8 [H, W] masks with row pitches lda, ldb.  The ratio is formed by the caller in fp64. */
+int msam_mask_iou_counts(const uint8_t* a, int lda, const uint8_t* b, int ldb, int H, int W, int64_t* counts, void* stream);
 /* debug: device buffer of 64 x 16 uint64 %globaltimer stamps written by the window-attention kernels, NULL = off */
 int msam_debug_attn_trace(void* dev_buf);
 

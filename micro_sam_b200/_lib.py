@@ -122,6 +122,11 @@ def lib() -> ctypes.CDLL:
                                                 c_uint64, c_void_p, c_void_p, c_void_p, c_void_p]
         L.msam_prompt_iterative.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_uint64,
                                             c_void_p, c_void_p, c_void_p]
+        L.msam_mask_prompts_workspace.restype = c_int64
+        L.msam_mask_prompts_workspace.argtypes = [c_int, c_int]
+        L.msam_mask_prompts.argtypes = [c_void_p, c_int, c_int, c_int, c_double, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p,
+                                        c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
+        L.msam_mask_iou_counts.argtypes = [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]
         _lib = L
     return _lib
 

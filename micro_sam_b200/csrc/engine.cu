@@ -609,6 +609,19 @@ int msam_prompt_iterative(const uint8_t* targets, const float* low_res, const fl
   return prompt_iterative(targets, low_res, iou, M, pred, n, n_per_img, in_h, in_w, orig_h, orig_w, seed, coords, labels,
                           (cudaStream_t)stream);
 }
+int64_t msam_mask_prompts_workspace(int H, int W) { return H > 0 && W > 0 ? mask_prompts_workspace(H, W) : -1; }
+int msam_mask_prompts(const uint8_t* mask, int H, int W, int ld, double box_extension, int want_logits, int point_mode, int max_points,
+                      void* workspace, int64_t ws_bytes, int64_t* stats, float* box1024, float* logits, float* points, float* labels,
+                      float* field, void* stream) {
+  if (!mask || !workspace || !stats || (want_logits && !logits) || (point_mode && (!points || !labels)))
+    return set_error("msam_mask_prompts: null argument");
+  return mask_prompts(mask, H, W, ld, box_extension, want_logits, point_mode, max_points, workspace, ws_bytes, stats, box1024, logits,
+                      points, labels, field, (cudaStream_t)stream);
+}
+int msam_mask_iou_counts(const uint8_t* a, int lda, const uint8_t* b, int ldb, int H, int W, int64_t* counts, void* stream) {
+  if (!a || !b || !counts) return set_error("msam_mask_iou_counts: null argument");
+  return mask_iou_counts(a, lda, b, ldb, H, W, counts, (cudaStream_t)stream);
+}
 int msam_to_image(const void* src, int dtype, int h, int w, int c, uint8_t* out_hwc3, uint32_t* scratch6, void* stream) {
   return post_to_image(src, dtype, h, w, c, out_hwc3, scratch6, (cudaStream_t)stream);
 }

@@ -228,4 +228,11 @@ int prompt_sample_points(const uint8_t* targets, const int32_t* counts, const in
 int prompt_iterative(const uint8_t* targets, const float* low_res, const float* iou, int M, const uint8_t* pred, int n, int n_per_img,
                      int in_h, int in_w, int H, int W, uint64_t seed, int32_t* coords, int32_t* labels, cudaStream_t st);
 
+// ---- volume.cu: segment_from_mask's prompt derivation and compute_iou's counts (segment_mask_in_volume)
+int64_t mask_prompts_workspace(int H, int W);
+int mask_prompts(const uint8_t* mask, int H, int W, int ld, double box_extension, int want_logits, int point_mode, int max_points,
+                 void* workspace, int64_t ws_bytes, int64_t* stats, float* box1024, float* logits, float* points, float* labels,
+                 float* field, cudaStream_t st);
+int mask_iou_counts(const uint8_t* a, int lda, const uint8_t* b, int ldb, int H, int W, int64_t* counts, cudaStream_t st);
+
 }  // namespace msam

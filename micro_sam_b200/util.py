@@ -620,6 +620,13 @@ def set_precomputed(predictor, image_embeddings: ImageEmbeddings, i: Optional[in
     return predictor
 
 
+def compute_iou(mask1: np.ndarray, mask2: np.ndarray) -> float:
+    """util.compute_iou (util.py:1266-1280): overlap / (union + 1e-7) of the pixels == 1, in fp64."""
+    overlap = np.logical_and(mask1 == 1, mask2 == 1).sum()
+    union = np.logical_or(mask1 == 1, mask2 == 1).sum()
+    return float(overlap) / (float(union) + 1e-7)
+
+
 # ------------------------------------------------------------------------------------------------ label image assembly
 def finish_ws_size(h: int, w: int) -> int:
     """int32 workspace elements of msam_finish_segmentation (include/msam_b200.h)."""
