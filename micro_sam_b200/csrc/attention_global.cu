@@ -45,12 +45,6 @@ struct GParams {
   float scale_log2;
 };
 
-__device__ __forceinline__ float gex2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
 template <int D>
 __global__ void __launch_bounds__(288, 1)
 attn_global_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmRTh,
@@ -214,12 +208,12 @@ attn_global_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_const
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
       const float m_new = fmaxf(m_run[rs], mx);
-      const float f = gex2(m_run[rs] - m_new);
+      const float f = ex2_approx(m_run[rs] - m_new);
       m_run[rs] = m_new;
       float ls = 0.f;
 #pragma unroll
       for (int jj = 0; jj < 16; ++jj) {
-        const float p0 = gex2(sacc[4 * jj + 2 * rs] - m_new), p1 = gex2(sacc[4 * jj + 2 * rs + 1] - m_new);
+        const float p0 = ex2_approx(sacc[4 * jj + 2 * rs] - m_new), p1 = ex2_approx(sacc[4 * jj + 2 * rs + 1] - m_new);
         ls += p0 + p1;
         pk[2 * jj + rs] = pack_bf16(p0, p1);
       }
@@ -278,9 +272,7 @@ int launch_global_t(const AttnArgs& a, cudaStream_t stream) {
              (double)a.batch * 4096 * a.heads * D * 2 * 4);
   launch_pdl(attn_global_kernel<D>, dim3(32, a.heads, a.batch), dim3(288), C::SMEM_BYTES, stream, tmQKV, tmRTh, tmRTw, p);
   prof_end(stream);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("global attention launch failed: %s", cudaGetErrorString(e));
-  count_launch();
+  LAUNCH_CHECK("global attention");
   return 0;
 }
 

@@ -48,11 +48,6 @@ struct W8Params {
   unsigned long long* trace;
 };
 
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
 __device__ __forceinline__ float fmax3(float a, float b, float c) { return fmaxf(a, fmaxf(b, c)); }
 __device__ __forceinline__ unsigned long long gtimer() {
   unsigned long long t;
@@ -326,9 +321,7 @@ static int launch_attn_window2_t(const AttnArgs& a, cudaStream_t stream) {
              (double)groups * a.heads * (4.0 * 196 * 196 * D + 4.0 * 196 * S * D), (double)groups * 196 * a.heads * D * 2 * 4);
   launch_pdl(attn_window2_kernel<D>, dim3(2, a.heads, groups), dim3(W8_THREADS), W8_SMEM, stream, tmQ, tmKV, tmRT, p);
   prof_end(stream);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("window attention launch failed: %s", cudaGetErrorString(e));
-  count_launch();
+  LAUNCH_CHECK("window attention");
   return 0;
 }
 

@@ -10,30 +10,6 @@ namespace msam {
 
 namespace {
 
-__device__ __forceinline__ uint32_t bpk2(float a, float b) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&v);
-}
-__device__ __forceinline__ float blo(uint32_t w) { return __uint_as_float(w << 16); }
-__device__ __forceinline__ float bhi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-
-#define BWD_CHECK(what)                                                                              \
-  do {                                                                                               \
-    cudaError_t e_ = cudaGetLastError();                                                             \
-    if (e_ != cudaSuccess) return set_error(what " launch failed: %s", cudaGetErrorString(e_));      \
-    count_launch();                                                                                  \
-  } while (0)
-
 // ---------------------------------------------------------------------------------------------------------------
 // LayerNorm backward, one warp per row (rows strided over the grid), row held in registers as in the forward kernel:
 //   xhat = (x - mean) rstd,  g = dy gamma,  dx = rstd (g - mean(g) - xhat mean(g xhat)),  dgamma += dy xhat,  dbeta += dy.
@@ -135,14 +111,10 @@ __global__ void gelu_fwd_kernel(const uint4* __restrict__ pre, long n8, uint4* _
   uint32_t o[4];
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
-    const float a = blo(w[j]), b = bhi(w[j]);
-    o[j] = bpk2(0.5f * a * (1.0f + erff(a * 0.70710678118654752440f)), 0.5f * b * (1.0f + erff(b * 0.70710678118654752440f)));
+    const float a = bf16_lo(w[j]), b = bf16_hi(w[j]);
+    o[j] = pack_bf16(gelu_erf(a), gelu_erf(b));
   }
   out[i] = make_uint4(o[0], o[1], o[2], o[3]);
-}
-// d/dx [x Phi(x)] = Phi(x) + x phi(x)
-__device__ __forceinline__ float gelu_grad(float x) {
-  return 0.5f * (1.0f + erff(x * 0.70710678118654752440f)) + x * 0.3989422804014327f * __expf(-0.5f * x * x);
 }
 __global__ void gelu_bwd_kernel(const uint4* __restrict__ dh, const uint4* __restrict__ pre, long n8, uint4* __restrict__ out) {
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -151,7 +123,8 @@ __global__ void gelu_bwd_kernel(const uint4* __restrict__ dh, const uint4* __res
   const uint32_t w[4] = {u.x, u.y, u.z, u.w}, gw[4] = {g.x, g.y, g.z, g.w};
   uint32_t o[4];
 #pragma unroll
-  for (int j = 0; j < 4; ++j) o[j] = bpk2(blo(gw[j]) * gelu_grad(blo(w[j])), bhi(gw[j]) * gelu_grad(bhi(w[j])));
+  for (int j = 0; j < 4; ++j)
+    o[j] = pack_bf16(bf16_lo(gw[j]) * gelu_erf_grad_fast(bf16_lo(w[j])), bf16_hi(gw[j]) * gelu_erf_grad_fast(bf16_hi(w[j])));
   out[i] = make_uint4(o[0], o[1], o[2], o[3]);
 }
 
@@ -276,7 +249,7 @@ __global__ void pack_dqkv_kernel(const float* __restrict__ dq, const float* __re
   const float4 v = *reinterpret_cast<const float4*>(src);
   const int D = heads * d;
   __nv_bfloat16* dst = dqkv + ((long)w * T + t) * (3 * D) + which * D + h * d + c4 * 4;
-  *reinterpret_cast<uint2*>(dst) = make_uint2(bpk2(v.x, v.y), bpk2(v.z, v.w));
+  *reinterpret_cast<uint2*>(dst) = make_uint2(pack_bf16(v.x, v.y), pack_bf16(v.z, v.w));
 }
 
 __global__ void sum_batch_kernel(const float* __restrict__ x, long n_batch, long n, float* __restrict__ out, int accumulate) {
@@ -315,7 +288,7 @@ __global__ void col2im3x3_kernel(const __nv_bfloat16* __restrict__ dcol, int B, 
     const uint4 u = *reinterpret_cast<const uint4*>(dcol + (((b * g + oy) * g + ox) * 9 + k) * (long)C + cc * 8);
     const uint32_t w[4] = {u.x, u.y, u.z, u.w};
 #pragma unroll
-    for (int j = 0; j < 4; ++j) { acc[2 * j] += blo(w[j]); acc[2 * j + 1] += bhi(w[j]); }
+    for (int j = 0; j < 4; ++j) { acc[2 * j] += bf16_lo(w[j]); acc[2 * j + 1] += bf16_hi(w[j]); }
   }
   float4* o = reinterpret_cast<float4*>(out + tok * C + cc * 8);
   o[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
@@ -326,7 +299,7 @@ __global__ void cast_f32_kernel(const uint2* __restrict__ x, long n4, float4* __
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n4) return;
   const uint2 u = x[i];
-  out[i] = make_float4(blo(u.x), bhi(u.x), blo(u.y), bhi(u.y));
+  out[i] = make_float4(bf16_lo(u.x), bf16_hi(u.x), bf16_lo(u.y), bf16_hi(u.y));
 }
 
 // out [cols, rows] = in [rows, cols]^T in 32 x 32 tiles through shared memory; block = (32, 8)
@@ -352,33 +325,33 @@ int launch_layernorm_bwd(const float* x, int rows, int D, const float* gamma, fl
   layernorm_bwd_kernel<<<blocks, LNB_WARPS * 32, 2 * D * sizeof(float), stream>>>(x, rows, D, gamma, eps, dy, window_mode, grid, ws,
                                                                                  accumulate, dx, dgamma, dbeta);
   prof_end(stream);
-  BWD_CHECK("layernorm_bwd");
+  LAUNCH_CHECK("layernorm_bwd");
   return 0;
 }
 int launch_gelu_fwd(const __nv_bfloat16* pre, long n, __nv_bfloat16* out, cudaStream_t stream) {
   if (n % 8) return set_error("gelu: n must be a multiple of 8");
   gelu_fwd_kernel<<<(unsigned)((n / 8 + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const uint4*>(pre), n / 8, reinterpret_cast<uint4*>(out));
-  BWD_CHECK("gelu_fwd");
+  LAUNCH_CHECK("gelu_fwd");
   return 0;
 }
 int launch_gelu_bwd(const __nv_bfloat16* dh, const __nv_bfloat16* pre, long n, __nv_bfloat16* dpre, cudaStream_t stream) {
   if (n % 8) return set_error("gelu: n must be a multiple of 8");
   gelu_bwd_kernel<<<(unsigned)((n / 8 + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const uint4*>(dh), reinterpret_cast<const uint4*>(pre),
                                                                       n / 8, reinterpret_cast<uint4*>(dpre));
-  BWD_CHECK("gelu_bwd");
+  LAUNCH_CHECK("gelu_bwd");
   return 0;
 }
 int launch_colsum(const __nv_bfloat16* x, long rows, int N, float* out, cudaStream_t stream) {
   if (rows <= 0) return 0;
   colsum_kernel<<<dim3((N + 63) / 64, (unsigned)((rows + 255) / 256)), 256, 0, stream>>>(x, rows, N, out);
-  BWD_CHECK("colsum");
+  LAUNCH_CHECK("colsum");
   return 0;
 }
 int launch_window_gather(const __nv_bfloat16* x, int B, int grid, int ws, int D, __nv_bfloat16* out_win, cudaStream_t stream) {
   const int wpr = (grid + ws - 1) / ws;
   const long total = (long)B * wpr * wpr * ws * ws * (D / 8);
   window_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(x, B, grid, ws, D, out_win);
-  BWD_CHECK("window_gather");
+  LAUNCH_CHECK("window_gather");
   return 0;
 }
 int launch_attn_probs(const float* S, const float* T, long n_batch, AttnBwdGeom g, int pitch_s, int pitch_p, float scale,
@@ -387,7 +360,7 @@ int launch_attn_probs(const float* S, const float* T, long n_batch, AttnBwdGeom 
   prof_begin(stream, "attn_bwd softmax", 0.0, (double)rows * (pitch_s * 4.0 + pitch_p * 2.0));
   attn_probs_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(S, T, rows, g, pitch_s, pitch_p, scale, P);
   prof_end(stream);
-  BWD_CHECK("attn_probs");
+  LAUNCH_CHECK("attn_probs");
   return 0;
 }
 int launch_attn_ds(const __nv_bfloat16* P, const float* dP, long n_batch, AttnBwdGeom g, int pitch_s, int pitch_p,
@@ -397,42 +370,42 @@ int launch_attn_ds(const __nv_bfloat16* P, const float* dP, long n_batch, AttnBw
   prof_begin(stream, "attn_bwd dS", 0.0, (double)rows * (pitch_s * 4.0 + pitch_p * 4.0));
   attn_ds_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, stream>>>(P, dP, rows, g, pitch_s, pitch_p, dS, dT);
   prof_end(stream);
-  BWD_CHECK("attn_ds");
+  LAUNCH_CHECK("attn_ds");
   return 0;
 }
 int launch_pack_dqkv(const float* dq, const float* dk, const float* dv, int outer, int heads, int T, int d, __nv_bfloat16* dqkv,
                      cudaStream_t stream) {
   const long total = (long)outer * heads * T * (d / 4) * 3;
   pack_dqkv_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(dq, dk, dv, outer, heads, T, d, dqkv);
-  BWD_CHECK("pack_dqkv");
+  LAUNCH_CHECK("pack_dqkv");
   return 0;
 }
 int launch_sum_batch(const float* x, long n_batch, long n, float* out, int accumulate, cudaStream_t stream) {
   sum_batch_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(x, n_batch, n, out, accumulate);
-  BWD_CHECK("sum_batch");
+  LAUNCH_CHECK("sum_batch");
   return 0;
 }
 int launch_nchw_to_tok(const float* nchw, int B, int C, int T, float* tok, cudaStream_t stream) {
   if (C % 32 || T % 32) return set_error("nchw_to_tok: C and T must be multiples of 32");
   nchw_to_tok_kernel<<<dim3(T / 32, C / 32, B), dim3(32, 8), 0, stream>>>(nchw, C, T, tok);
-  BWD_CHECK("nchw_to_tok");
+  LAUNCH_CHECK("nchw_to_tok");
   return 0;
 }
 int launch_col2im3x3(const __nv_bfloat16* dcol, int B, int g, int C, float* out, cudaStream_t stream) {
   const long total = (long)B * g * g * (C / 8);
   col2im3x3_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(dcol, B, g, C, out);
-  BWD_CHECK("col2im");
+  LAUNCH_CHECK("col2im");
   return 0;
 }
 int launch_cast_f32(const __nv_bfloat16* x, long n, float* out, cudaStream_t stream) {
   if (n % 4) return set_error("cast: n must be a multiple of 4");
   cast_f32_kernel<<<(unsigned)((n / 4 + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const uint2*>(x), n / 4, reinterpret_cast<float4*>(out));
-  BWD_CHECK("cast_f32");
+  LAUNCH_CHECK("cast_f32");
   return 0;
 }
 int launch_transpose_bf16(const __nv_bfloat16* in, int rows, int cols, __nv_bfloat16* out, cudaStream_t stream) {
   transpose_bf16_kernel<<<dim3((cols + 31) / 32, (rows + 31) / 32), dim3(32, 8), 0, stream>>>(in, rows, cols, out);
-  BWD_CHECK("transpose");
+  LAUNCH_CHECK("transpose");
   return 0;
 }
 

@@ -198,9 +198,7 @@ static int launch_bgemm_t(const BGemmArgs& a, cudaStream_t stream) {
              ((double)a.M * a.K + (double)a.N * a.K) * 2 * a.heads * a.outer + (double)a.M * a.N * 4 * a.heads * a.outer);
   bgemm_kernel<A_MN, B_MN><<<grid, THREADS, SMEM_BYTES, stream>>>(tmA, tmB, p);
   prof_end(stream);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("bgemm launch failed: %s", cudaGetErrorString(e));
-  count_launch();
+  LAUNCH_CHECK("bgemm");
   return 0;
 }
 

@@ -7,6 +7,7 @@
 // Exact algebraic hoist: in layer 0 the image-side projections (k/v of token->image, q of image->token) act on
 // `image_embedding + dense (+ pe)`, identical for every prompt when no mask prompt is given -> computed once per
 // image in set_image_embedding (SURVEY.md 8d).
+#include "device_util.cuh"
 #include "engine.h"
 
 #include <algorithm>
@@ -78,13 +79,6 @@ struct DecoderState {
 };
 
 // ================================================================================================ kernels
-__device__ __forceinline__ float bf_lo(uint32_t w) { return __uint_as_float(w << 16); }
-__device__ __forceinline__ float bf_hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
-__device__ __forceinline__ uint32_t pk2(float a, float b) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&v);
-}
-
 // Dense PE of the 64x64 pixel-centre grid (PositionEmbeddingRandom.forward) -> token-major [g*g, 256].
 __global__ void dense_pe_kernel(const float* __restrict__ G, int g, float* __restrict__ pos) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -118,7 +112,6 @@ __global__ void set_image_kernel(const float* __restrict__ feat, const float* __
 
 // Mask prompts (PromptEncoder._embed_masks): keys0[p, token, :] = image_embedding[token, :] + mask_downscaling(mask[p])[:, token]
 // grid = (4096 / 16, P), block = 256 (thread = output channel; 16 tokens per block).  LayerNorm2d: eps 1e-6, biased variance.
-__device__ __forceinline__ float gelu_exact(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 __global__ void __launch_bounds__(256)
 mask_dense_kernel(const float* __restrict__ mask, const float* __restrict__ w1, const float* __restrict__ b1,
                   const float* __restrict__ g1, const float* __restrict__ be1, const float* __restrict__ w2,
@@ -145,7 +138,7 @@ mask_dense_kernel(const float* __restrict__ mask, const float* __restrict__ w1, 
     for (int c = 0; c < 4; ++c) var += (y[c] - mean) * (y[c] - mean);
     const float rstd = rsqrtf(var * 0.25f + 1e-6f);
 #pragma unroll
-    for (int c = 0; c < 4; ++c) sa[tk][c * 4 + sy * 2 + sx] = gelu_exact((y[c] - mean) * rstd * g1[c] + be1[c]);
+    for (int c = 0; c < 4; ++c) sa[tk][c * 4 + sy * 2 + sx] = gelu_erf((y[c] - mean) * rstd * g1[c] + be1[c]);
   }
   __syncthreads();
   if (tid < 16) {  // stage 2: thread = token: 16 channels (w2[o][c][sy][sx] contiguous = [o][16])
@@ -164,7 +157,7 @@ mask_dense_kernel(const float* __restrict__ mask, const float* __restrict__ w1, 
     for (int o = 0; o < 16; ++o) var += (z[o] - mean) * (z[o] - mean);
     const float rstd = rsqrtf(var * (1.0f / 16) + 1e-6f);
 #pragma unroll
-    for (int o = 0; o < 16; ++o) sg[tid][o] = gelu_exact((z[o] - mean) * rstd * g2[o] + be2[o]);
+    for (int o = 0; o < 16; ++o) sg[tid][o] = gelu_erf((z[o] - mean) * rstd * g2[o] + be2[o]);
   }
   __syncthreads();
   float w[16];
@@ -307,7 +300,7 @@ __global__ void token_self_attn_kernel(const __nv_bfloat16* __restrict__ q, int 
     const float inv = 1.f / l;
     __nv_bfloat16* dst = out + ((long)p * T + lane) * 256 + h * 32;
 #pragma unroll
-    for (int d = 0; d < 32; d += 2) *reinterpret_cast<uint32_t*>(dst + d) = pk2(o[d] * inv, o[d + 1] * inv);
+    for (int d = 0; d < 32; d += 2) *reinterpret_cast<uint32_t*>(dst + d) = pack_bf16(o[d] * inv, o[d + 1] * inv);
   }
 }
 
@@ -334,7 +327,7 @@ i2t_attn_kernel(const __nv_bfloat16* __restrict__ qimg, int ldq, long q_stride_r
     const uint4 qa = *reinterpret_cast<const uint4*>(qp), qb = *reinterpret_cast<const uint4*>(qp + 8);
     const uint32_t qw[8] = {qa.x, qa.y, qa.z, qa.w, qb.x, qb.y, qb.z, qb.w};
 #pragma unroll
-    for (int i = 0; i < 8; ++i) { qf[r][2 * i] = bf_lo(qw[i]); qf[r][2 * i + 1] = bf_hi(qw[i]); }
+    for (int i = 0; i < 8; ++i) { qf[r][2 * i] = bf16_lo(qw[i]); qf[r][2 * i + 1] = bf16_hi(qw[i]); }
   }
   float s[2][TMAX], m[2] = {-1e30f, -1e30f};
 #pragma unroll
@@ -373,10 +366,10 @@ i2t_attn_kernel(const __nv_bfloat16* __restrict__ qimg, int ldq, long q_stride_r
     const float inv = 1.f / l[r];
     const int n = blockIdx.x * 64 + (threadIdx.x >> 3) + 32 * r;
     uint4 o0, o1;
-    o0.x = pk2(o[r][0] * inv, o[r][1] * inv); o0.y = pk2(o[r][2] * inv, o[r][3] * inv);
-    o0.z = pk2(o[r][4] * inv, o[r][5] * inv); o0.w = pk2(o[r][6] * inv, o[r][7] * inv);
-    o1.x = pk2(o[r][8] * inv, o[r][9] * inv); o1.y = pk2(o[r][10] * inv, o[r][11] * inv);
-    o1.z = pk2(o[r][12] * inv, o[r][13] * inv); o1.w = pk2(o[r][14] * inv, o[r][15] * inv);
+    o0.x = pack_bf16(o[r][0] * inv, o[r][1] * inv); o0.y = pack_bf16(o[r][2] * inv, o[r][3] * inv);
+    o0.z = pack_bf16(o[r][4] * inv, o[r][5] * inv); o0.w = pack_bf16(o[r][6] * inv, o[r][7] * inv);
+    o1.x = pack_bf16(o[r][8] * inv, o[r][9] * inv); o1.y = pack_bf16(o[r][10] * inv, o[r][11] * inv);
+    o1.z = pack_bf16(o[r][12] * inv, o[r][13] * inv); o1.w = pack_bf16(o[r][14] * inv, o[r][15] * inv);
     __nv_bfloat16* dst = out + ((long)p * NI + n) * DI + h * 16;
     *reinterpret_cast<uint4*>(dst) = o0;
     *reinterpret_cast<uint4*>(dst + 8) = o1;
@@ -387,14 +380,6 @@ __global__ void gather_iou_kernel(const float* __restrict__ iou32, int P, int m0
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < P * nm) out[i] = iou32[(long)(i / nm) * 32 + m0 + i % nm];
 }
-
-#define LAUNCH_CHECK(name)                                                                        \
-  do {                                                                                            \
-    cudaError_t e_ = cudaGetLastError();                                                          \
-    if (e_ != cudaSuccess) return set_error(name " launch failed: %s", cudaGetErrorString(e_)); \
-    count_launch();                                                                               \
-  } while (0)
-#define CHK(p) do { if (!(p)) return -1; } while (0)
 
 // ================================================================================================ weights
 static int load_attn(Engine& E, const std::string& p, int inner, AttnW& w, bool fuse_qkv) {

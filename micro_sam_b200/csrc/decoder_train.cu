@@ -11,6 +11,7 @@
 // (accumulated: every consumer ADDS) and a bf16 copy (the GEMM operand).  Parameter gradients accumulate across calls (images,
 // sub-iterations) until msam_decoder_zero_grads.  Prompts: points and / or boxes, with the dense prompt no_mask_embed or, for mask
 // prompts, mask_downscaling(mask) (md_* kernels: fp32, taped by keeping the mask; no gradient w.r.t. the mask itself).
+#include "device_util.cuh"
 #include "engine.h"
 
 #include <algorithm>
@@ -19,31 +20,7 @@
 
 namespace msam {
 
-#define CHK(p) do { if (!(p)) return -1; } while (0)
-#define RUN(x) do { if (x) return -1; } while (0)
-#define KCHECK(what)                                                                                 \
-  do {                                                                                               \
-    cudaError_t e_ = cudaGetLastError();                                                             \
-    if (e_ != cudaSuccess) return set_error(what " launch failed: %s", cudaGetErrorString(e_));      \
-    count_launch();                                                                                  \
-  } while (0)
-
 namespace {
-
-__device__ __forceinline__ uint32_t dpk2(float a, float b) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&v);
-}
-__device__ __forceinline__ float dwarp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float dwarp_max(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
 
 // out_bf16[r, c] = bf16(a[r, c] + b[r % b_rows, c]); b may be null.  n4 = rows * cols / 4
 __global__ void add_cast_kernel(const float4* __restrict__ a, const float4* __restrict__ b, long n4, long b_n4, uint2* __restrict__ out) {
@@ -51,7 +28,7 @@ __global__ void add_cast_kernel(const float4* __restrict__ a, const float4* __re
   if (i >= n4) return;
   float4 v = a[i];
   if (b) { const float4 w = b[i % b_n4]; v.x += w.x; v.y += w.y; v.z += w.z; v.w += w.w; }
-  out[i] = make_uint2(dpk2(v.x, v.y), dpk2(v.z, v.w));
+  out[i] = make_uint2(pack_bf16(v.x, v.y), pack_bf16(v.z, v.w));
 }
 // dst += src (fp32)
 __global__ void add_inplace_kernel(float4* __restrict__ dst, const float4* __restrict__ src, long n4) {
@@ -74,7 +51,7 @@ __global__ void grad_cast_kernel(const float4* __restrict__ g, const uint2* __re
     if (!(__uint_as_float(y.y << 16) > 0.f)) v.z = 0.f;
     if (!(__uint_as_float(y.y & 0xffff0000u) > 0.f)) v.w = 0.f;
   }
-  out[i] = make_uint2(dpk2(v.x, v.y), dpk2(v.z, v.w));
+  out[i] = make_uint2(pack_bf16(v.x, v.y), pack_bf16(v.z, v.w));
 }
 // strided row copy / accumulate: dst[r * dp + c] (+)= src[r * sp + c], c < cols
 __global__ void copy_rows_kernel(const float* __restrict__ src, long sp, float* __restrict__ dst, long dp, long rows, int cols, int accumulate) {
@@ -94,10 +71,10 @@ __global__ void softmax_rows_kernel(const float* __restrict__ S, long rows, int 
   __nv_bfloat16* p = P + row * pitch;
   float m = -INFINITY;
   for (int k = lane; k < n_valid; k += 32) m = fmaxf(m, s[k]);
-  m = dwarp_max(m);
+  m = warp_max(m);
   float l = 0.f;
   for (int k = lane; k < n_valid; k += 32) l += __expf(s[k] - m);
-  const float inv = 1.0f / dwarp_sum(l);
+  const float inv = 1.0f / warp_sum(l);
   for (int k = lane; k < pitch; k += 32) p[k] = __float2bfloat16(k < n_valid ? __expf(s[k] - m) * inv : 0.f);
 }
 // dS = P o (dP - sum_k P dP)
@@ -111,7 +88,7 @@ __global__ void ds_rows_kernel(const __nv_bfloat16* __restrict__ P, const float*
   __nv_bfloat16* ds = dS + row * pitch;
   float del = 0.f;
   for (int k = lane; k < n_valid; k += 32) del += __bfloat162float(p[k]) * dp[k];
-  del = dwarp_sum(del);
+  del = warp_sum(del);
   for (int k = lane; k < pitch; k += 32) ds[k] = __float2bfloat16(k < n_valid ? __bfloat162float(p[k]) * (dp[k] - del) : 0.f);
 }
 // tokens [P, T, 256]: rows 0..4 = output tokens (iou token, 4 mask tokens), rows 5.. = sparse prompt embeddings [P, Ts, 256]
@@ -188,7 +165,7 @@ __global__ void masks_grad_kernel(const float* __restrict__ d_low, int P, int nm
   const long p = i / 65536;
   float v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   for (int m = 0; m < nm; ++m) v[m0 + m] = d_low[((p * nm + m) * 256 + Y) * 256 + X];
-  *reinterpret_cast<uint4*>(out8 + (p * 65536 + up_row(Y, X)) * 8) = make_uint4(dpk2(v[0], v[1]), dpk2(v[2], v[3]), dpk2(v[4], v[5]), dpk2(v[6], v[7]));
+  *reinterpret_cast<uint4*>(out8 + (p * 65536 + up_row(Y, X)) * 8) = make_uint4(pack_bf16(v[0], v[1]), pack_bf16(v[2], v[3]), pack_bf16(v[4], v[5]), pack_bf16(v[6], v[7]));
 }
 
 inline unsigned nblk(long n, int per = 256) { return (unsigned)((n + per - 1) / per); }
@@ -203,11 +180,6 @@ constexpr int MD_SMALL = MD_W3;      // parameters of the two strided stages (re
 constexpr int MD_BIG = MD_N - MD_W3; // W3 + b3 (reduced from md_keys_grad_kernel's partials)
 constexpr int MD_PIX_TILE = 128;     // pixels per tile of md_param_grad_kernel (= its block size)
 constexpr int MD_GRID2 = 256;        // most blocks of md_param_grad_kernel: partial rows to reduce, independent of the device
-
-__device__ __forceinline__ float md_gelu(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
-__device__ __forceinline__ float md_gelu_grad(float x) {   // d/dx [x Phi(x)] = Phi(x) + x phi(x), exact erf form
-  return 0.5f * (1.0f + erff(x * 0.70710678118654752440f)) + x * 0.39894228040143267794f * expf(-0.5f * x * x);
-}
 
 // Stages of one output pixel.  Index s = sy * 2 + sx is the stage-1 sub-pixel, k = dy * 2 + dx the position in a 2x2 conv window;
 // stage-1 channel c of sub-pixel s sits at c * 4 + s, the order of W2's input index (W2 [o][c][sy][sx]).  LayerNorm2d statistics are
@@ -264,12 +236,12 @@ __device__ __forceinline__ void md_pixel(const float* __restrict__ mask_p, int p
     float m[4], n[4], a[4];
     md_stage1(mask_p, pix, s, W, m, n, a);
 #pragma unroll
-    for (int c = 0; c < 4; ++c) h1[c * 4 + s] = md_gelu(a[c]);
+    for (int c = 0; c < 4; ++c) h1[c * 4 + s] = gelu_erf(a[c]);
   }
   float n2[16], a2[16];
   md_stage2(h1, W, n2, a2);
 #pragma unroll
-  for (int o = 0; o < 16; ++o) h2[o] = md_gelu(a2[o]);
+  for (int o = 0; o < 16; ++o) h2[o] = gelu_erf(a2[o]);
 }
 
 // Forward: out[p, pix, c] = dense_p[c, pix] (+ emb_nchw[c, pix]); h2_out[p, pix, 0..15] = stage-2 output (the 1x1 conv's input,
@@ -389,7 +361,7 @@ md_param_grad_kernel(const float* __restrict__ mask, const float* __restrict__ d
         for (int c = 0; c < 4; ++c) {
           const int j = c * 4 + s;
           n1[j] = n[c];
-          h1[j] = md_gelu(a[c]);
+          h1[j] = gelu_erf(a[c]);
           s_h1[j * MD_LD + tid] = h1[j];
           s_da1[j * MD_LD + tid] = a[c];
         }
@@ -402,7 +374,7 @@ md_param_grad_kernel(const float* __restrict__ mask, const float* __restrict__ d
         float mdn = 0.f, mdnn = 0.f;
 #pragma unroll
         for (int o = 0; o < 16; ++o) {
-          const float da = dh[o] * md_gelu_grad(a2[o]);
+          const float da = dh[o] * gelu_erf_grad(a2[o]);
           s_da2[o * MD_LD + tid] = da;
           s_e2[o * MD_LD + tid] = da * n2[o];
           dz[o] = da * W[MD_G2 + o];          // dL/d n2, turned into dL/d z below
@@ -421,7 +393,7 @@ md_param_grad_kernel(const float* __restrict__ mask, const float* __restrict__ d
         float dh1 = 0.f;
 #pragma unroll
         for (int o = 0; o < 16; ++o) dh1 += dz[o] * W[MD_W2 + o * 16 + k];
-        const float da = dh1 * md_gelu_grad(s_da1[k * MD_LD + tid]);
+        const float da = dh1 * gelu_erf_grad(s_da1[k * MD_LD + tid]);
         s_da1[k * MD_LD + tid] = da;
         s_e1[k * MD_LD + tid] = da * n1[k];
         s_dy1[k * MD_LD + tid] = da * W[MD_G1 + (k >> 2)];    // dL/d n1, turned into dL/d y1 below
@@ -494,7 +466,7 @@ __global__ void md_reduce_kernel(const float* __restrict__ part_small, int rows_
   const long pitch = small ? MD_SMALL : MD_BIG;
   float s = 0.f;
   for (int r = lane; r < rows; r += 32) s += src[(long)r * pitch];
-  s = dwarp_sum(s);
+  s = warp_sum(s);
   if (lane == 0) grads[j] = accumulate ? grads[j] + s : s;
 }
 
@@ -515,21 +487,21 @@ inline MdScratch md_carve(float* base, int P) {
 int md_forward(const float* mask, int P, const float* W, const float* emb_nchw, float* out, __nv_bfloat16* out_bf, const MdScratch& s,
                cudaStream_t st) {
   md_forward_kernel<<<dim3(4096 / 16, P), 256, 0, st>>>(mask, W, emb_nchw, out, out_bf, s.h2);
-  KCHECK("md_forward");
+  LAUNCH_CHECK("md_forward");
   return 0;
 }
 // g = dL/d keys0 [P * 4096, 256] -> d_emb_nchw (if non-null) and the ten parameter gradients, added to (accumulate) or written over grads
 int md_backward(const float* g, const float* mask, int P, const float* W, float* d_emb_nchw, const MdScratch& s, float* grads,
                 int accumulate, cudaStream_t st) {
   md_keys_grad_kernel<<<4096 / 16, 256, 0, st>>>(g, s.h2, W, P, d_emb_nchw, s.d_h2, s.part_big);
-  KCHECK("md_keys_grad");
+  LAUNCH_CHECK("md_keys_grad");
   const size_t smem = (size_t)MD_TERMS * MD_LD * 4;
   if (cudaFuncSetAttribute(md_param_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
     return set_error("md_param_grad: shared-memory attribute failed");
   md_param_grad_kernel<<<md_grid2(P), MD_PIX_TILE, smem, st>>>(mask, s.d_h2, W, P, s.part_small);
-  KCHECK("md_param_grad");
+  LAUNCH_CHECK("md_param_grad");
   md_reduce_kernel<<<nblk((long)MD_N * 32), 256, 0, st>>>(s.part_small, md_grid2(P), s.part_big, 4096 / 16, grads, accumulate);
-  KCHECK("md_reduce");
+  LAUNCH_CHECK("md_reduce");
   return 0;
 }
 
@@ -605,12 +577,12 @@ struct Ctx {
 
 int cast_grad(const float* g, const __nv_bfloat16* relu_y, long n, __nv_bfloat16* out, cudaStream_t st) {
   grad_cast_kernel<<<nblk(n / 4), 256, 0, st>>>((const float4*)g, (const uint2*)relu_y, n / 4, (uint2*)out);
-  KCHECK("grad_cast");
+  LAUNCH_CHECK("grad_cast");
   return 0;
 }
 int add_inplace(float* dst, const float* src, long n, cudaStream_t st) {
   add_inplace_kernel<<<nblk(n / 4), 256, 0, st>>>((float4*)dst, (const float4*)src, n / 4);
-  KCHECK("add_inplace");
+  LAUNCH_CHECK("add_inplace");
   return 0;
 }
 
@@ -669,7 +641,7 @@ int op_add_cast(Ctx& c, const Ten& a, const float* b_v, long b_rows, float* b_g,
   y = c.ten(a.rows, a.cols, false, true, true);
   if (c.err) return -1;
   add_cast_kernel<<<nblk(a.n() / 4), 256, 0, c.st>>>((const float4*)a.v, (const float4*)b_v, a.n() / 4, b_rows * a.cols / 4, (uint2*)y.b);
-  KCHECK("add_cast");
+  LAUNCH_CHECK("add_cast");
   const Ten ain = a, yout = y;
   c.s.tape.push_back([=](cudaStream_t st) -> int {
     RUN(add_inplace(ain.g, yout.g, yout.n(), st));
@@ -698,7 +670,7 @@ int op_attention(Ctx& c, const Ten& q, const Ten& k, const Ten& v, int P, int Tq
   a.heads = heads; a.outer = P; a.out = S; a.ldc = pitch; a.o_hstride = s_h; a.o_wstride = s_w; a.alpha = scale;
   RUN(launch_bgemm(a, c.st));
   softmax_rows_kernel<<<nblk(nb * Tq, 8), 256, 0, c.st>>>(S, nb * Tq, Tk, pitch, Pm);
-  KCHECK("softmax_rows");
+  LAUNCH_CHECK("softmax_rows");
   // O = P V, written head-interleaved [P*Tq, inner]
   a = BGemmArgs();
   a.A = Pm; a.B = v.b; a.b_mn = 1; a.M = Tq; a.N = hd; a.K = pitch; a.lda = pitch; a.ldb = inner; a.a_hstride = s_h; a.a_wstride = s_w;
@@ -722,7 +694,7 @@ int op_attention(Ctx& c, const Ten& q, const Ten& k, const Ten& v, int P, int Tq
     a.heads = heads; a.outer = P; a.out = S; a.ldc = pitch; a.o_hstride = s_h; a.o_wstride = s_w;
     RUN(launch_bgemm(a, st));
     ds_rows_kernel<<<nblk(nb * Tq, 8), 256, 0, st>>>(Pm, S, nb * Tq, Tk, pitch, dS);
-    KCHECK("ds_rows");
+    LAUNCH_CHECK("ds_rows");
     // dQ += scale dS K
     a = BGemmArgs();
     a.A = dS; a.B = kk.b; a.b_mn = 1; a.M = Tq; a.N = hd; a.K = pitch; a.lda = pitch; a.ldb = inner; a.a_hstride = s_h; a.a_wstride = s_w;
@@ -764,12 +736,12 @@ int op_slice_rows(Ctx& c, const Ten& x, long offset, long pitch, long rows, int 
   y = c.ten(rows, cols, true, true, true);
   if (c.err) return -1;
   copy_rows_kernel<<<nblk(rows * cols), 256, 0, c.st>>>(x.v + offset, pitch, y.v, cols, rows, cols, 0);
-  KCHECK("slice_rows");
+  LAUNCH_CHECK("slice_rows");
   RUN(launch_cast_bf16(y.v, y.n(), y.b, c.st));
   const Ten xin = x, yout = y;
   c.s.tape.push_back([=](cudaStream_t st) -> int {
     copy_rows_kernel<<<nblk(rows * cols), 256, 0, st>>>(yout.g, cols, xin.g + offset, pitch, rows, cols, 1);
-    KCHECK("slice_rows_bwd");
+    LAUNCH_CHECK("slice_rows_bwd");
     return 0;
   });
   return 0;
@@ -1019,7 +991,7 @@ int Engine::decoder_train_forward(int slot, const float* emb_nchw, const float* 
   Ten keys0 = c.ten(Ri, 256, true, true, true);
   if (c.err) return -1;
   assemble_tokens_kernel<<<nblk(Rt * 256), 256, 0, st>>>(d.out_tokens, sparse, P, T, Ts, tok.v);
-  KCHECK("assemble_tokens");
+  LAUNCH_CHECK("assemble_tokens");
   RUN(launch_cast_bf16(tok.v, tok.n(), tok.b, st));
   if (mask_in) {   // dense prompt = mask_downscaling(mask); the mask is kept: the backward pass recomputes the stages from it
     s.mask = (float*)c.take((size_t)P * 65536 * 4);
@@ -1031,7 +1003,7 @@ int Engine::decoder_train_forward(int slot, const float* emb_nchw, const float* 
     RUN(md_forward(s.mask, P, d.md_w, emb_nchw, keys0.v, keys0.b, s.md, st));
   } else {
     src_broadcast_kernel<<<dim3(128, 8), dim3(32, 8), 0, st>>>(emb_nchw, d.no_mask, P, keys0.v);
-    KCHECK("src_broadcast");
+    LAUNCH_CHECK("src_broadcast");
     RUN(launch_cast_bf16(keys0.v, keys0.n(), keys0.b, st));
   }
   s.tok = tok; s.keys0 = keys0;
@@ -1088,12 +1060,12 @@ int Engine::decoder_train_forward(int slot, const float* emb_nchw, const float* 
     RUN(op_linear(c, h1, d.hyper[i][1], h2, 2, nullptr, true));
     RUN(op_linear(c, h2, d.hyper[i][2], h3, 0, nullptr, false));       // [P, 32]
     copy_rows_kernel<<<nblk((long)P * 32), 256, 0, st>>>(h3.v, 32, hyper.v + i * 32, 8 * 32, P, 32, 0);
-    KCHECK("hyper_gather");
+    LAUNCH_CHECK("hyper_gather");
     const Ten h3c = h3, hyc = hyper;
     const int ii = i, PP = P;
     s.tape.push_back([=](cudaStream_t st2) -> int {
       copy_rows_kernel<<<nblk((long)PP * 32), 256, 0, st2>>>(hyc.g + ii * 32, 8 * 32, h3c.g, 32, PP, 32, 1);
-      KCHECK("hyper_scatter");
+      LAUNCH_CHECK("hyper_scatter");
       return 0;
     });
   }
@@ -1105,7 +1077,7 @@ int Engine::decoder_train_forward(int slot, const float* emb_nchw, const float* 
     RUN(op_linear(c, h1, d.iou[1], h2, 2, nullptr, true));
     RUN(op_linear(c, h2, d.iou[2], s.iou32, 0, nullptr, false));       // [P, 32], columns 0..3 real
     copy_rows_kernel<<<nblk((long)P * s.nm), 256, 0, st>>>(s.iou32.v + s.m0, 32, iou, s.nm, P, s.nm, 0);
-    KCHECK("iou_out");
+    LAUNCH_CHECK("iou_out");
   }
   // masks = hyper @ upscaled: per prompt [65536 x 32] x [32 x 4]
   s.low4 = c.ten((long)P * 65536, 4, true, false, false);
@@ -1117,7 +1089,7 @@ int Engine::decoder_train_forward(int slot, const float* emb_nchw, const float* 
     g.b_rows_valid = 4; g.heads = 1; g.outer = P; g.out = s.low4.v; g.ldc = 4; g.o_wstride = 65536L * 4;
     RUN(launch_bgemm(g, st));
     masks_out_kernel<<<nblk((long)P * s.nm * 65536), 256, 0, st>>>(s.low4.v, P, s.nm, s.m0, low_res);
-    KCHECK("masks_out");
+    LAUNCH_CHECK("masks_out");
     const Ten upc = up, hyc = hyper;
     __nv_bfloat16* dm = s.dmask8;
     const int PP = P;
@@ -1147,23 +1119,23 @@ int Engine::decoder_train_backward(int slot, const float* d_low_res, const float
   const int P = s.P;
   if (d_low_res) {
     masks_grad_kernel<<<nblk((long)P * 65536), 256, 0, st>>>(d_low_res, P, s.nm, s.m0, s.dmask8);
-    KCHECK("masks_grad");
+    LAUNCH_CHECK("masks_grad");
   } else if (cudaMemsetAsync(s.dmask8, 0, (size_t)P * 65536 * 16, st) != cudaSuccess) {
     return set_error("decoder training: memset failed");
   }
   if (d_iou) {
     copy_rows_kernel<<<nblk((long)P * s.nm), 256, 0, st>>>(d_iou, s.nm, s.iou32.g + s.m0, 32, P, s.nm, 1);
-    KCHECK("iou_grad");
+    LAUNCH_CHECK("iou_grad");
   }
   for (auto it = s.tape.rbegin(); it != s.tape.rend(); ++it) RUN((*it)(st));
   token_grads_kernel<<<s.T, 256, 0, st>>>(s.tok.g, s.emb_index, P, s.T, s.Ts, d.g_out_tokens, d.g_point_emb, d.g_nap);
-  KCHECK("token_grads");
+  LAUNCH_CHECK("token_grads");
   if (s.mask) {
     RUN(md_backward(s.keys0.g, s.mask, P, d.md_w, d_emb_nchw, s.md, d.md_g, 1, st));
     d.md_written = true;
   } else {
     src_grad_kernel<<<dim3(128, 8), dim3(32, 8), 0, st>>>(s.keys0.g, P, d_emb_nchw, d.g_no_mask);
-    KCHECK("src_grad");
+    LAUNCH_CHECK("src_grad");
   }
   s.live = false;   // gradients of the activations are consumed: one backward per forward
   return 0;

@@ -6,11 +6,6 @@
 
 namespace msam {
 
-__device__ __forceinline__ uint32_t pack2(float a, float b) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&v);
-}
-
 // ---------------------------------------------------------------------------------------------------------------
 // Sam.preprocess + PatchEmbed im2col.  Output A[b*g*g + ty*g + tx][c*256 + py*16 + px] (bf16), matching the flattened
 // Conv2d weight [D, 3*16*16].  Source is either uint8 HWC (h x w <= img x img; normalise + zero-pad fused:
@@ -48,8 +43,8 @@ __global__ void patchify_kernel(const uint8_t* __restrict__ u8, const float* __r
     }
   }
   uint4 o0, o1;
-  o0.x = pack2(v[0], v[1]); o0.y = pack2(v[2], v[3]); o0.z = pack2(v[4], v[5]); o0.w = pack2(v[6], v[7]);
-  o1.x = pack2(v[8], v[9]); o1.y = pack2(v[10], v[11]); o1.z = pack2(v[12], v[13]); o1.w = pack2(v[14], v[15]);
+  o0.x = pack_bf16(v[0], v[1]); o0.y = pack_bf16(v[2], v[3]); o0.z = pack_bf16(v[4], v[5]); o0.w = pack_bf16(v[6], v[7]);
+  o1.x = pack_bf16(v[8], v[9]); o1.y = pack_bf16(v[10], v[11]); o1.z = pack_bf16(v[12], v[13]); o1.w = pack_bf16(v[14], v[15]);
   uint4* dst = reinterpret_cast<uint4*>(out + tok * 768 + c * 256 + py * 16);
   dst[0] = o0;
   dst[1] = o1;
@@ -61,9 +56,7 @@ int launch_patchify(const uint8_t* u8, const float* f32, int B, int h, int w, in
   const long total = (long)B * g * g * 48;
   patchify_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(u8, f32, B, h, w, img, mean[0], mean[1], mean[2],
                                                                     stdv[0], stdv[1], stdv[2], out);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("patchify launch failed: %s", cudaGetErrorString(e));
-  count_launch();
+  LAUNCH_CHECK("patchify");
   return 0;
 }
 
@@ -95,9 +88,7 @@ __global__ void layernorm_rows_kernel(const float* __restrict__ x, int rows, int
       sum += (v[i].x + v[i].y) + (v[i].z + v[i].w);
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  const float mean = sum / (float)D;
+  const float mean = warp_sum(sum) / (float)D;
   float sq = 0.f;
 #pragma unroll
   for (int i = 0; i < LN_MAX_V4; ++i) {
@@ -107,9 +98,7 @@ __global__ void layernorm_rows_kernel(const float* __restrict__ x, int rows, int
       sq += (a * a + b * b) + (c * c + d * d);
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-  const float rstd = rsqrtf(sq / (float)D + eps);
+  const float rstd = rsqrtf(warp_sum(sq) / (float)D + eps);
 
   long orow = warp;
   if (mode == 1) {
@@ -131,17 +120,12 @@ __global__ void layernorm_rows_kernel(const float* __restrict__ x, int rows, int
       r.y = (v[i].y - mean) * rstd * g.y + bb.y;
       r.z = (v[i].z - mean) * rstd * g.z + bb.z;
       r.w = (v[i].w - mean) * rstd * g.w + bb.w;
-      if (act == 1) {
-        r.x = 0.5f * r.x * (1.0f + erff(r.x * 0.70710678118654752440f));
-        r.y = 0.5f * r.y * (1.0f + erff(r.y * 0.70710678118654752440f));
-        r.z = 0.5f * r.z * (1.0f + erff(r.z * 0.70710678118654752440f));
-        r.w = 0.5f * r.w * (1.0f + erff(r.w * 0.70710678118654752440f));
-      }
-      if (out) *reinterpret_cast<uint2*>(out + orow * D + 4 * k) = make_uint2(pack2(r.x, r.y), pack2(r.z, r.w));
+      if (act == 1) { r.x = gelu_erf(r.x); r.y = gelu_erf(r.y); r.z = gelu_erf(r.z); r.w = gelu_erf(r.w); }
+      if (out) *reinterpret_cast<uint2*>(out + orow * D + 4 * k) = make_uint2(pack_bf16(r.x, r.y), pack_bf16(r.z, r.w));
       if (out_f32) *reinterpret_cast<float4*>(out_f32 + orow * D + 4 * k) = r;
       if (out2) {
         const float4 a = __ldg(a4 + k);
-        *reinterpret_cast<uint2*>(out2 + orow * D + 4 * k) = make_uint2(pack2(r.x + a.x, r.y + a.y), pack2(r.z + a.z, r.w + a.w));
+        *reinterpret_cast<uint2*>(out2 + orow * D + 4 * k) = make_uint2(pack_bf16(r.x + a.x, r.y + a.y), pack_bf16(r.z + a.z, r.w + a.w));
       }
     }
   }
@@ -156,9 +140,7 @@ int launch_layernorm(const LnArgs& a, cudaStream_t stream) {
   launch_pdl(layernorm_rows_kernel, dim3(blocks), dim3(warps_per_block * 32), 0, stream, a.x, a.rows, a.D, a.gamma, a.beta, a.eps,
              a.out, a.window_mode, a.grid, a.ws, a.add, a.add_rows, a.out2, a.out_f32, a.act);
   prof_end(stream);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("layernorm launch failed: %s", cudaGetErrorString(e));
-  count_launch();
+  LAUNCH_CHECK("layernorm");
   return 0;
 }
 
@@ -175,17 +157,12 @@ __global__ void layernorm2d_nchw_kernel(const float* __restrict__ x, int T, cons
   for (int t = warp * 4; t < warp * 4 + 4; ++t) {
     const float4* src = reinterpret_cast<const float4*>(x + (tok0 + t) * C);
     const float4 a = src[lane], b = src[lane + 32];
-    float sum = (a.x + a.y) + (a.z + a.w) + (b.x + b.y) + (b.z + b.w);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    const float mean = sum / C;
+    const float mean = warp_sum((a.x + a.y) + (a.z + a.w) + (b.x + b.y) + (b.z + b.w)) / C;
     float d[8] = {a.x - mean, a.y - mean, a.z - mean, a.w - mean, b.x - mean, b.y - mean, b.z - mean, b.w - mean};
     float sq = 0.f;
 #pragma unroll
     for (int i = 0; i < 8; ++i) sq += d[i] * d[i];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-    const float rstd = rsqrtf(sq / C + eps);
+    const float rstd = rsqrtf(warp_sum(sq) / C + eps);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const int c = (i < 4) ? (4 * lane + i) : (128 + 4 * lane + (i - 4));
@@ -201,9 +178,7 @@ int launch_layernorm2d_nchw(const float* x, int B, int T, const float* gamma, co
                             cudaStream_t stream) {
   if (T % 32 != 0) return set_error("layernorm2d: T=%d must be a multiple of 32", T);
   layernorm2d_nchw_kernel<<<(unsigned)((long)B * T / 32), 256, 0, stream>>>(x, T, gamma, beta, eps, out);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("layernorm2d launch failed: %s", cudaGetErrorString(e));
-  count_launch();
+  LAUNCH_CHECK("layernorm2d");
   return 0;
 }
 
@@ -212,16 +187,14 @@ __global__ void cast_bf16_kernel(const float* __restrict__ x, long n4, __nv_bflo
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n4) return;
   const float4 v = reinterpret_cast<const float4*>(x)[i];
-  reinterpret_cast<uint2*>(out)[i] = make_uint2(pack2(v.x, v.y), pack2(v.z, v.w));
+  reinterpret_cast<uint2*>(out)[i] = make_uint2(pack_bf16(v.x, v.y), pack_bf16(v.z, v.w));
 }
 int launch_cast_bf16(const float* x, long n, __nv_bfloat16* out, cudaStream_t stream) {
   if (n % 4 != 0) return set_error("cast: n must be a multiple of 4");
   const long n4 = n / 4;
   if (n4 == 0) return 0;
   cast_bf16_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, stream>>>(x, n4, out);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("cast launch failed: %s", cudaGetErrorString(e));
-  count_launch();
+  LAUNCH_CHECK("cast");
   return 0;
 }
 
@@ -248,9 +221,7 @@ __global__ void im2col3x3_kernel(const __nv_bfloat16* __restrict__ x, int B, int
 int launch_im2col3x3(const __nv_bfloat16* x, int B, int g, int C, __nv_bfloat16* out, cudaStream_t stream) {
   const long total = (long)B * g * g * 9 * (C / 8);
   im2col3x3_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(x, B, g, C, out);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("im2col launch failed: %s", cudaGetErrorString(e));
-  count_launch();
+  LAUNCH_CHECK("im2col");
   return 0;
 }
 

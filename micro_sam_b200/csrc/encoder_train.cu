@@ -19,9 +19,6 @@
 
 namespace msam {
 
-#define CHK(p) do { if (!(p)) return -1; } while (0)
-#define RUN(x) do { if (x) return -1; } while (0)
-
 struct TrainSave {
   __nv_bfloat16 *qkv_wT = nullptr, *proj_wT = nullptr, *fc1_wT = nullptr, *fc2_wT = nullptr;
   float *g_ln1_g = nullptr, *g_ln1_b = nullptr, *g_ln2_g = nullptr, *g_ln2_b = nullptr, *g_qkv_w = nullptr, *g_qkv_b = nullptr,

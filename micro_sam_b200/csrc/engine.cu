@@ -19,7 +19,13 @@ int set_error(const char* fmt, ...) {
   va_end(ap);
   return -1;
 }
-void count_launch() { ++g_launches; }
+static void count_launch() { ++g_launches; }
+int launch_check(const char* name) {
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error("%s launch failed: %s", name, cudaGetErrorString(e));
+  count_launch();
+  return 0;
+}
 bool pdl_enabled() {
   // every kernel of the chain needs its predecessor's output at once, so only the short prologues could overlap -> off unless
   // MSAM_PDL=1
@@ -173,8 +179,6 @@ std::vector<float> conv3x3_gemm_layout(const std::vector<float>& w, int C) {
 }
 
 // ------------------------------------------------------------------------------------------------ weights
-#define CHK(p) do { if (!(p)) return -1; } while (0)
-
 int Engine::finalize_encoder() {
   const int D = cfg.embed_dim, hd = D / cfg.num_heads, g = cfg.image_size / cfg.patch_size;
   const std::string e = "image_encoder.";

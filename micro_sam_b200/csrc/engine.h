@@ -11,6 +11,10 @@
 #include "kernels.h"
 #include "tensormap.h"
 
+// Early returns (-1) of the int-returning host functions: CHK when a result is null / false, RUN when a return code is nonzero.
+#define CHK(p) do { if (!(p)) return -1; } while (0)
+#define RUN(x) do { if (x) return -1; } while (0)
+
 namespace msam {
 
 struct HostTensor {

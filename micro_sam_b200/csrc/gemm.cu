@@ -51,7 +51,6 @@ struct GemmParams {
   float ln_eps;
 };
 
-__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 // GELU(x) = 0.5 x (1 + erf(x / sqrt 2)) for values that are stored as bf16 or consumed by bf16-operand products:
 // erf from Abramowitz-Stegun 7.1.25 (three terms, |abs err| <= 2.5e-5 -- measured 2.6e-5 on the GELU over [-10, 10],
 // two orders below the bf16 rounding of the operands it feeds), branch-free with the approximate MUFU ops:
@@ -334,9 +333,7 @@ static int launch_gemm_bn(const GemmArgs& a, int num_sms, cudaStream_t stream) {
   }
   launch_pdl(gemm_bf16_kernel<BN, EPI>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, stream, tmA, tmB, p);
   prof_end(stream);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("gemm launch failed: %s", cudaGetErrorString(e));
-  count_launch();
+  LAUNCH_CHECK("gemm");
   return 0;
 }
 

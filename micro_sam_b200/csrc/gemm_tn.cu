@@ -162,9 +162,7 @@ static int launch_gemm_mn(const __nv_bfloat16* A, const __nv_bfloat16* B, int M,
   prof_begin(stream, A_MN ? "gemm_tn (wgrad)" : "gemm_nn (dgrad)", 2.0 * M * N * K, (double)K * (M + N) * 2 + (double)M * N * 4);
   gemm_tn_kernel<A_MN><<<grid, THREADS, SMEM_BYTES, stream>>>(tmA, tmB, out, M, N, K, ldc, accumulate);
   prof_end(stream);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("gemm_tn launch failed: %s", cudaGetErrorString(e));
-  count_launch();
+  LAUNCH_CHECK("gemm_tn");
   return 0;
 }
 

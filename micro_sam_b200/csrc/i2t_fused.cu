@@ -72,12 +72,6 @@ struct I2tParams {
   float eps;
 };
 
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
 __global__ void __launch_bounds__(i2t::THREADS, 1)
 i2t_fused_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                  const __grid_constant__ CUtensorMap tmM, const __grid_constant__ CUtensorMap tmV,
@@ -339,9 +333,7 @@ int launch_i2t_fused(const I2tFusedArgs& a, int num_sms, cudaStream_t stream) {
   prof_begin(stream, a.mode ? "i2t_fused (own keys)" : "i2t_fused (shared image)", (double)a.P * 4096 * (2.0 * 256 * 64 * (a.mode ? 2 : 1) + 2.0 * 64 * 256), bytes);
   i2t_fused_kernel<<<grid, THREADS, SMEM_BYTES, stream>>>(tmA0, tmA1, tmM, tmV, tmO, p);
   prof_end(stream);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("i2t_fused launch failed: %s", cudaGetErrorString(e));
-  count_launch();
+  LAUNCH_CHECK("i2t_fused");
   return 0;
 }
 
@@ -375,9 +367,7 @@ __global__ void i2t_prep_kernel(const __nv_bfloat16* __restrict__ ktok, const __
 int launch_i2t_prep(const __nv_bfloat16* ktok, const __nv_bfloat16* vtok, const float* bq, int P, int T,
                     __nv_bfloat16* kexp, __nv_bfloat16* vexp, float* sbias, cudaStream_t stream) {
   i2t_prep_kernel<<<P, 256, 0, stream>>>(ktok, vtok, bq, T, kexp, vexp, sbias);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("i2t_prep launch failed: %s", cudaGetErrorString(e));
-  count_launch();
+  LAUNCH_CHECK("i2t_prep");
   return 0;
 }
 

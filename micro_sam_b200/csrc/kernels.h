@@ -23,7 +23,9 @@ cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
 }
 
 int set_error(const char* fmt, ...);  // records msam_last_error(); returns -1
-void count_launch();                  // per-thread launch counter (msam_launch_count)
+// After a launch: records "<name> launch failed: ..." and returns -1 if it failed, else counts it (msam_launch_count), returns 0
+int launch_check(const char* name);
+#define LAUNCH_CHECK(name) do { if (launch_check(name)) return -1; } while (0)
 
 // Optional per-kernel timing (bench.py roofline / per-stage table): CUDA events recorded on the launching stream around a
 // launch, aggregated by `name` (a string literal) in msam_profile_report; flops / bytes = ALGORITHMIC work of the launch.

@@ -383,13 +383,6 @@ filter_nms_kernel(const int32_t* __restrict__ boxes, const float* __restrict__ s
   (void)s_cur;
 }
 
-#define LAUNCH_CHECK(name)                                                                        \
-  do {                                                                                            \
-    cudaError_t e_ = cudaGetLastError();                                                          \
-    if (e_ != cudaSuccess) return set_error(name " launch failed: %s", cudaGetErrorString(e_)); \
-    count_launch();                                                                               \
-  } while (0)
-
 int post_mask_stats(const float* low_res, int n, int in_h, int in_w, int out_h, int out_w, float thr, float off,
                     int32_t* boxes, float* stability, int32_t* area, cudaStream_t st, bool force_generic,
                     const float* thr_arr, const float* lazy_iou, float lazy_iou_thresh, uint8_t* lazy_done) {

@@ -441,13 +441,6 @@ iterative_kernel(const uint8_t* __restrict__ targets, const float* __restrict__ 
   }
 }
 
-#define PROMPT_LAUNCH_CHECK(name)                                                                  \
-  do {                                                                                            \
-    cudaError_t e_ = cudaGetLastError();                                                          \
-    if (e_ != cudaSuccess) return set_error(name " launch failed: %s", cudaGetErrorString(e_));   \
-    count_launch();                                                                               \
-  } while (0)
-
 }  // namespace
 
 int prompt_targets(const void* labels, int label_dtype, int B, int H, int W, const int64_t* ids, const int32_t* n_ids, int n_obj,
@@ -458,7 +451,7 @@ int prompt_targets(const void* labels, int label_dtype, int B, int H, int W, con
   const long HW = (long)H * W;
   // boxes doubles as the min / max accumulator until box_finish_kernel overwrites it with the final boxes
   targets_init_kernel<<<(n + 255) / 256, 256, 0, st>>>(n, counts, boxes);
-  PROMPT_LAUNCH_CHECK("prompt_targets_init");
+  LAUNCH_CHECK("prompt_targets_init");
   const size_t smem = (size_t)n_obj * (sizeof(int64_t) + 5 * sizeof(int));
   const int gx = (int)std::min<long>((HW + 255) / 256, 1024);
   prof_begin(st, "prompt_targets", 0.0, (double)B * HW * (label_dtype ? 8 : 4) + (double)n * HW);
@@ -470,9 +463,9 @@ int prompt_targets(const void* labels, int label_dtype, int B, int H, int W, con
     targets_kernel<int64_t><<<dim3(gx, B), 256, smem, st>>>((const int64_t*)labels, H, W, ids, n_ids, n_obj, targets, counts, boxes);
   }
   prof_end(st);
-  PROMPT_LAUNCH_CHECK("prompt_targets");
+  LAUNCH_CHECK("prompt_targets");
   box_finish_kernel<<<(n + 255) / 256, 256, 0, st>>>(n, n_obj, H, W, box_distortion, seed, boxes, boxes);
-  PROMPT_LAUNCH_CHECK("prompt_box_finish");
+  LAUNCH_CHECK("prompt_box_finish");
   return 0;
 }
 
@@ -490,16 +483,16 @@ int prompt_sample_points(const uint8_t* targets, const int32_t* counts, const in
     if (!scratch) return set_error("prompt_sample_points: the dilation needs a scratch buffer of 2 * n * H * W bytes");
     const int blocks = (int)std::min<long>((total + 255) / 256, 4096);
     dilate_rows_kernel<<<blocks, 256, 0, st>>>(targets, total, W, dilation, scratch);
-    PROMPT_LAUNCH_CHECK("prompt_dilate_rows");
+    LAUNCH_CHECK("prompt_dilate_rows");
     dilate_cols_kernel<<<blocks, 256, 0, st>>>(scratch, total, H, W, dilation, scratch + total);
-    PROMPT_LAUNCH_CHECK("prompt_dilate_cols");
+    LAUNCH_CHECK("prompt_dilate_cols");
     dil = scratch + total;
   }
   prof_begin(st, "prompt_sample_points", 0.0, (double)total * (n_neg > 0 ? 3 : 1));
   sample_points_kernel<<<n, kThreads, 0, st>>>(targets, dil, counts, boxes, centers, n_per_img, H, W, n_pos, n_neg, dilation, seed,
                                                coords, labels);
   prof_end(st);
-  PROMPT_LAUNCH_CHECK("prompt_sample_points");
+  LAUNCH_CHECK("prompt_sample_points");
   return 0;
 }
 
@@ -519,7 +512,7 @@ int prompt_iterative(const uint8_t* targets, const float* low_res, const float* 
   prof_begin(st, "prompt_iterative", 0.0, (double)n * H * W * 2 + (low_res ? (double)n * 65536.0 * 4 : (double)n * H * W * 2));
   iterative_kernel<<<n, kThreads, 0, st>>>(targets, low_res, iou, M, pred, g, n_per_img, seed, coords, labels);
   prof_end(st);
-  PROMPT_LAUNCH_CHECK("prompt_iterative");
+  LAUNCH_CHECK("prompt_iterative");
   return 0;
 }
 

@@ -44,12 +44,6 @@ struct T2iParams {
   float* out;  // [n_items * 128, 256] fp32: softmax-weighted mean of the image tokens per row
 };
 
-__device__ __forceinline__ float ex2f(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
 template <int ROWS, int MODE>
 __global__ void __launch_bounds__(t2i::Cfg<ROWS>::THREADS, 1)
 t2i_fused_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmXS,
@@ -189,12 +183,12 @@ t2i_fused_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
         mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 1));
         mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, 2));
         const float m_new = fmaxf(m_run[rs], mt);
-        const float f = ex2f(m_run[rs] - m_new);
+        const float f = ex2_approx(m_run[rs] - m_new);
         m_run[rs] = m_new;
         float ls = 0.f;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-          const float p0 = ex2f(s[4 * j + 2 * rs] - m_new), p1 = ex2f(s[4 * j + 2 * rs + 1] - m_new);
+          const float p0 = ex2_approx(s[4 * j + 2 * rs] - m_new), p1 = ex2_approx(s[4 * j + 2 * rs + 1] - m_new);
           ls += p0 + p1;
           pk[2 * j + rs] = pack_bf16(p0, p1);
         }
@@ -254,9 +248,7 @@ static int launch_t2i_fused_t(const T2iFusedArgs& a, int num_sms, cudaStream_t s
              (double)a.n_items * (ROWS * 256.0 * 2 + ROWS * 256.0 * 4) + (a.mode ? (double)a.n_items * 4096 * 512 : 0.0));
   t2i_fused_kernel<ROWS, MODE><<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(tmX, tmXS, tmQ, p);
   prof_end(stream);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("t2i_fused launch failed: %s", cudaGetErrorString(e));
-  count_launch();
+  LAUNCH_CHECK("t2i_fused");
   return 0;
 }
 
@@ -325,9 +317,7 @@ t2i_head_proj_kernel(const float* __restrict__ U, const __nv_bfloat16* __restric
 
 int launch_t2i_prep(const __nv_bfloat16* q, int P, int T, int paired, int n_items, __nv_bfloat16* qexp, cudaStream_t stream) {
   t2i_prep_kernel<<<n_items, 256, 0, stream>>>(q, P, T, paired, qexp);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("t2i_prep launch failed: %s", cudaGetErrorString(e));
-  count_launch();
+  LAUNCH_CHECK("t2i_prep");
   return 0;
 }
 int launch_t2i_head_proj(const float* U, const __nv_bfloat16* WvT, const float* bv, int P, int T, int paired,
@@ -343,9 +333,8 @@ int launch_t2i_head_proj(const float* U, const __nv_bfloat16* WvT, const float* 
     if (!attr16) { e = cudaFuncSetAttribute(t2i_head_proj_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 16 * 8192); attr16 = true; }
     if (e == cudaSuccess) t2i_head_proj_kernel<16><<<P, 128, smem, stream>>>(U, WvT, bv, T, paired, out);
   }
-  if (e == cudaSuccess) e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("t2i_head_proj launch failed: %s", cudaGetErrorString(e));
-  count_launch();
+  if (e != cudaSuccess) return set_error("t2i_head_proj launch failed: %s", cudaGetErrorString(e));   // attribute: nothing launched
+  LAUNCH_CHECK("t2i_head_proj");
   return 0;
 }
 

@@ -7,6 +7,7 @@
 // Everything 1x1 / dense is the wgmma GEMM of gemm.cu with BatchNorm folded into weight + bias at load time; the
 // depth-wise convolutions, the window LayerNorm (zero pad tokens BEFORE the norm -> pad rows = LN bias) and the small-window
 // attention are HBM-bound CUDA-core kernels.  Activations: bf16 NHWC in the conv stage, fp32 token-major residual stream after.
+#include "device_util.cuh"
 #include "engine.h"
 
 #include <cmath>
@@ -15,18 +16,10 @@ namespace msam {
 
 namespace {
 
-__device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
-__device__ __forceinline__ uint32_t pk2(float a, float b) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&v);
-}
 __device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
   const uint32_t w[4] = {u.x, u.y, u.z, u.w};
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    f[2 * i] = __uint_as_float(w[i] << 16);
-    f[2 * i + 1] = __uint_as_float(w[i] & 0xffff0000u);
-  }
+  for (int i = 0; i < 4; ++i) { f[2 * i] = bf16_lo(w[i]); f[2 * i + 1] = bf16_hi(w[i]); }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -74,7 +67,7 @@ __global__ void tv_stem1_kernel(const uint8_t* __restrict__ u8, const float* __r
 #pragma unroll
   for (int i = 0; i < 8; ++i) acc[i] = gelu_erf(acc[i]);
   *reinterpret_cast<uint4*>(out + pix * 32 + cg * 8) =
-      make_uint4(pk2(acc[0], acc[1]), pk2(acc[2], acc[3]), pk2(acc[4], acc[5]), pk2(acc[6], acc[7]));
+      make_uint4(pack_bf16(acc[0], acc[1]), pack_bf16(acc[2], acc[3]), pack_bf16(acc[4], acc[5]), pack_bf16(acc[6], acc[7]));
 }
 
 // im2col for a 3x3 / pad 1 conv with stride on bf16 NHWC [B, Hin, Hin, C]: out[opix][(ky*3+kx)*C + c].  One thread = 8 channels.
@@ -129,7 +122,7 @@ __global__ void tv_dwconv_bf16_kernel(const __nv_bfloat16* __restrict__ x, int B
     for (int i = 0; i < 8; ++i) acc[i] = gelu_erf(acc[i]);
   }
   *reinterpret_cast<uint4*>(out + pix * C + cc * 8) =
-      make_uint4(pk2(acc[0], acc[1]), pk2(acc[2], acc[3]), pk2(acc[4], acc[5]), pk2(acc[6], acc[7]));
+      make_uint4(pack_bf16(acc[0], acc[1]), pack_bf16(acc[2], acc[3]), pack_bf16(acc[4], acc[5]), pack_bf16(acc[6], acc[7]));
 }
 
 __global__ void tv_dwconv_f32_kernel(const float* __restrict__ x, int B, int Hin, int C, const float* __restrict__ wt,
@@ -175,7 +168,7 @@ __global__ void tv_ln_window_kernel(const float* __restrict__ x, int B, int H, i
   if (y >= H || xx >= H) {
     for (int k = lane; k < nv; k += 32) {
       const float4 bb = __ldg(b4 + k);
-      *reinterpret_cast<uint2*>(orow + 4 * k) = make_uint2(pk2(bb.x, bb.y), pk2(bb.z, bb.w));
+      *reinterpret_cast<uint2*>(orow + 4 * k) = make_uint2(pack_bf16(bb.x, bb.y), pack_bf16(bb.z, bb.w));
     }
     return;
   }
@@ -187,9 +180,7 @@ __global__ void tv_ln_window_kernel(const float* __restrict__ x, int B, int H, i
     const int k = lane + 32 * i;
     if (k < nv) { v[i] = src[k]; sum += (v[i].x + v[i].y) + (v[i].z + v[i].w); }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  const float mean = sum / (float)D;
+  const float mean = warp_sum(sum) / (float)D;
   float sq = 0.f;
 #pragma unroll
   for (int i = 0; i < TV_LN_V4; ++i) {
@@ -199,9 +190,7 @@ __global__ void tv_ln_window_kernel(const float* __restrict__ x, int B, int H, i
       sq += (a * a + bq * bq) + (c * c + d * d);
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-  const float rstd = rsqrtf(sq / (float)D + eps);
+  const float rstd = rsqrtf(warp_sum(sq) / (float)D + eps);
   const float4* g4 = reinterpret_cast<const float4*>(gamma);
 #pragma unroll
   for (int i = 0; i < TV_LN_V4; ++i) {
@@ -209,8 +198,8 @@ __global__ void tv_ln_window_kernel(const float* __restrict__ x, int B, int H, i
     if (k < nv) {
       const float4 g = __ldg(g4 + k), bb = __ldg(b4 + k);
       *reinterpret_cast<uint2*>(orow + 4 * k) =
-          make_uint2(pk2((v[i].x - mean) * rstd * g.x + bb.x, (v[i].y - mean) * rstd * g.y + bb.y),
-                     pk2((v[i].z - mean) * rstd * g.z + bb.z, (v[i].w - mean) * rstd * g.w + bb.w));
+          make_uint2(pack_bf16((v[i].x - mean) * rstd * g.x + bb.x, (v[i].y - mean) * rstd * g.y + bb.y),
+                     pack_bf16((v[i].z - mean) * rstd * g.z + bb.z, (v[i].w - mean) * rstd * g.w + bb.w));
     }
   }
 }
@@ -307,16 +296,9 @@ tv_attn_kernel(const __nv_bfloat16* __restrict__ qkv, const float* __restrict__ 
 #pragma unroll
   for (int ch = 0; ch < 4; ++ch)
     *reinterpret_cast<uint4*>(orow + ch * 8) =
-        make_uint4(pk2(acc[ch * 8] * inv, acc[ch * 8 + 1] * inv), pk2(acc[ch * 8 + 2] * inv, acc[ch * 8 + 3] * inv),
-                   pk2(acc[ch * 8 + 4] * inv, acc[ch * 8 + 5] * inv), pk2(acc[ch * 8 + 6] * inv, acc[ch * 8 + 7] * inv));
+        make_uint4(pack_bf16(acc[ch * 8] * inv, acc[ch * 8 + 1] * inv), pack_bf16(acc[ch * 8 + 2] * inv, acc[ch * 8 + 3] * inv),
+                   pack_bf16(acc[ch * 8 + 4] * inv, acc[ch * 8 + 5] * inv), pack_bf16(acc[ch * 8 + 6] * inv, acc[ch * 8 + 7] * inv));
 }
-
-#define TV_LAUNCH_CHECK(what)                                                                        \
-  do {                                                                                               \
-    cudaError_t e_ = cudaGetLastError();                                                             \
-    if (e_ != cudaSuccess) return set_error(what " launch failed: %s", cudaGetErrorString(e_));      \
-    count_launch();                                                                                  \
-  } while (0)
 
 int tv_dwconv_bf16(const __nv_bfloat16* x, int B, int Hin, int C, int stride, const float* w, const float* b, int act,
                    __nv_bfloat16* out, cudaStream_t st) {
@@ -324,7 +306,7 @@ int tv_dwconv_bf16(const __nv_bfloat16* x, int B, int Hin, int C, int stride, co
   prof_begin(st, "tinyvit dwconv3x3 (bf16)", 0.0, (double)B * Hin * Hin * C * 2 + (double)total * 16);
   tv_dwconv_bf16_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x, B, Hin, C, stride, w, b, act, out);
   prof_end(st);
-  TV_LAUNCH_CHECK("dwconv");
+  LAUNCH_CHECK("dwconv");
   return 0;
 }
 
@@ -357,8 +339,6 @@ static int fold_conv_bn(Engine& e, const std::string& p, int out, int inner, Fol
   }
   return 0;
 }
-
-#define CHK(p) do { if (!(p)) return -1; } while (0)
 
 static int up_pointwise(Engine& e, const std::string& p, int out, int in, TvConv* c) {  // 1x1 Conv2d_BN -> GEMM operand [out, in]
   FoldedConv f;
@@ -508,10 +488,10 @@ int Engine::encode_tinyvit(const uint8_t* u8, const float* f32, int B, int hh, i
       tv_stem1_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(u8p, f32p, nb, hh, ww, img, mean[0], mean[1], mean[2], stdv[0],
                                                                     stdv[1], stdv[2], tv.stem1.wf, tv.stem1.b, tv.s1);
       prof_end(st);
-      TV_LAUNCH_CHECK("stem conv1");
+      LAUNCH_CHECK("stem conv1");
       const long tc = (long)nb * 256 * 256 * 9 * 4;
       tv_im2col_kernel<<<(unsigned)((tc + 255) / 256), 256, 0, st>>>(tv.s1, nb, 512, 32, 2, tv.col);
-      TV_LAUNCH_CHECK("stem im2col");
+      LAUNCH_CHECK("stem im2col");
       if (tv_gemm(*this, tv.col, tv.stem2.w, nb * 65536, 64, 288, tv.stem2.b, 0, nullptr, 0, 0, tv.a0, 0, st)) return -1;
     }
     int stage_idx = 0;   // stop_after counts: 1 = after layers.0 (incl. its downsample), 2 / 3 / 4 = after layers.1 / 2 / 3
@@ -534,7 +514,7 @@ int Engine::encode_tinyvit(const uint8_t* u8, const float* f32, int B, int hh, i
         {
           const long warps = Mw;
           tv_ln_window_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(tv.x, nb, H, D, wsz, b.an_g, b.an_b, 1e-5f, tv.xw);
-          TV_LAUNCH_CHECK("window layernorm");
+          LAUNCH_CHECK("window layernorm");
         }
         if (tv_gemm(*this, tv.xw, b.qkv_w, Mw, 3 * D, D, b.qkv_b, 0, nullptr, 0, 0, tv.qkv, 0, st)) return -1;
         {
@@ -550,13 +530,13 @@ int Engine::encode_tinyvit(const uint8_t* u8, const float* f32, int B, int hh, i
           if (wsz == 7) tv_attn_kernel<7><<<dim3(nb * nw * nw, S.heads), 64, SM7, st>>>(tv.qkv, b.bias_tab, S.heads, H, scale, tv.attn);
           else tv_attn_kernel<14><<<dim3(nb * nw * nw, S.heads), 224, SM14, st>>>(tv.qkv, b.bias_tab, S.heads, H, scale, tv.attn);
           prof_end(st);
-          TV_LAUNCH_CHECK("window attention");
+          LAUNCH_CHECK("window attention");
         }
         if (tv_gemm(*this, tv.attn, b.proj_w, M, D, D, b.proj_b, 0, tv.x, 0, 0, tv.x2, 1, st)) return -1;
         {
           const long total = (long)M * (D / 4);
           tv_dwconv_f32_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(tv.x2, nb, H, D, b.local.wf, b.local.b, tv.x);
-          TV_LAUNCH_CHECK("local conv");
+          LAUNCH_CHECK("local conv");
         }
         LnArgs l;
         l.x = tv.x; l.rows = M; l.D = D; l.gamma = b.mn_g; l.beta = b.mn_b; l.eps = 1e-5f; l.out = tv.xn;

@@ -8,14 +8,6 @@
 
 namespace msam {
 
-#define RUN(x) do { if (x) return -1; } while (0)
-#define KCHECK(what)                                                                                 \
-  do {                                                                                               \
-    cudaError_t e_ = cudaGetLastError();                                                             \
-    if (e_ != cudaSuccess) return set_error(what " launch failed: %s", cudaGetErrorString(e_));      \
-    count_launch();                                                                                  \
-  } while (0)
-
 namespace {
 
 __global__ void adamw_kernel(float* __restrict__ w, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, long n, float lr,
@@ -81,7 +73,7 @@ int Engine::optimizer_step(float lr, float b1, float b2, float eps, float wd, cu
       if (!p.m || !p.v) return -1;
     }
     adamw_kernel<<<(unsigned)((p.n + 255) / 256), 256, 0, st>>>(p.w, p.g, p.m, p.v, p.n, lr, b1, b2, eps, wd, c1p, c2p);
-    KCHECK("adamw");
+    LAUNCH_CHECK("adamw");
     switch (p.refresh) {
       case Refresh::None:
         break;
@@ -90,11 +82,11 @@ int Engine::optimizer_step(float lr, float b1, float b2, float eps, float wd, cu
         break;
       case Refresh::RelPosRows:
         rel_rows_kernel<<<(unsigned)((p.n + 255) / 256), 256, 0, st>>>(p.w, p.rows, p.cols, p.cols_pad, p.row_off, p.dst);
-        KCHECK("rel_rows");
+        LAUNCH_CHECK("rel_rows");
         break;
       case Refresh::TileBias4:
         tile4_kernel<<<(unsigned)((p.n + 127) / 128), 128, 0, st>>>(p.w, (int)p.n, p.dst4);
-        KCHECK("tile4");
+        LAUNCH_CHECK("tile4");
         break;
     }
     if (p.dstT) RUN(launch_transpose_bf16(p.dst, p.rows, p.cols, p.dstT, st));

@@ -384,9 +384,7 @@ int launch_upscale_fused(const UpscaleFusedArgs& a, int num_sms, cudaStream_t st
   }
   prof_end(stream);
   if (rc) return rc;
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error("upscale_fused launch failed: %s", cudaGetErrorString(e));
-  count_launch();
+  LAUNCH_CHECK("upscale_fused");
   return 0;
 }
 

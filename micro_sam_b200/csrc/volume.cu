@@ -432,13 +432,6 @@ __global__ void iou_kernel(const uint8_t* __restrict__ a, int lda, const uint8_t
   }
 }
 
-#define VOL_LAUNCH_CHECK(name)                                                                     \
-  do {                                                                                            \
-    cudaError_t e_ = cudaGetLastError();                                                          \
-    if (e_ != cudaSuccess) return set_error(name " launch failed: %s", cudaGetErrorString(e_));   \
-    count_launch();                                                                               \
-  } while (0)
-
 int grid_for(long n) { return (int)std::max<long>(1, std::min<long>((n + 255) / 256, 2048)); }
 
 }  // namespace
@@ -459,11 +452,11 @@ int mask_prompts(const uint8_t* mask, int H, int W, int ld, double box_extension
   const Ws w = carve(workspace, H, W);
   const long hw = (long)H * W;
   stats_init_kernel<<<1, 32, 0, st>>>(stats, w.ctr);
-  VOL_LAUNCH_CHECK("mask_prompts_init");
+  LAUNCH_CHECK("mask_prompts_init");
   stats_kernel<<<grid_for(hw), 256, 0, st>>>(mask, H, W, ld, stats);
-  VOL_LAUNCH_CHECK("mask_prompts_stats");
+  LAUNCH_CHECK("mask_prompts_stats");
   finish_kernel<<<1, 1, 0, st>>>(H, W, box_extension, stats, box1024);
-  VOL_LAUNCH_CHECK("mask_prompts_box");
+  LAUNCH_CHECK("mask_prompts_box");
   if (want_logits) {
     // get_preprocess_shape(H, W, 256) on the host: x86-64 fp64 without contraction, as numpy computes it
     const double scale = 256 * 1.0 / std::max(H, W);
@@ -481,42 +474,42 @@ int mask_prompts(const uint8_t* mask, int H, int W, int ld, double box_extension
     const float* tmp = nullptr;
     if (tw != W) {
       resize_h_kernel<<<grid_for((long)H * tw), 256, 0, st>>>(mask, H, W, ld, tw, w.tmp);
-      VOL_LAUNCH_CHECK("mask_prompts_resize_h");
+      LAUNCH_CHECK("mask_prompts_resize_h");
       tmp = w.tmp;
     }
     logits_kernel<<<256, 256, 0, st>>>(mask, ld, tmp, H, W, th, tw, hi, logits);
-    VOL_LAUNCH_CHECK("mask_prompts_logits");
+    LAUNCH_CHECK("mask_prompts_logits");
   }
   if (point_mode) {
     edt_cols_kernel<<<(W + 127) / 128, 128, 0, st>>>(mask, ld, stats, w.g, w.ctr);
-    VOL_LAUNCH_CHECK("mask_prompts_edt_cols");
+    LAUNCH_CHECK("mask_prompts_edt_cols");
     // f1 and rmax are free until the Gaussian and the peak search: they hold the envelopes of the row pass
     edt_rows_kernel<<<(H + 63) / 64, 64, 0, st>>>(stats, w.g, w.ctr, (int32_t*)w.f1, (int32_t*)w.rmax, w.f0);
-    VOL_LAUNCH_CHECK("mask_prompts_edt_rows");
+    LAUNCH_CHECK("mask_prompts_edt_rows");
     gauss_kernel<<<grid_for(hw), 256, 0, st>>>(stats, w.f0, w.f1, 0);
-    VOL_LAUNCH_CHECK("mask_prompts_gauss0");
+    LAUNCH_CHECK("mask_prompts_gauss0");
     gauss_kernel<<<grid_for(hw), 256, 0, st>>>(stats, w.f1, w.f2, 1);
-    VOL_LAUNCH_CHECK("mask_prompts_gauss1");
+    LAUNCH_CHECK("mask_prompts_gauss1");
     unsigned long long* best = (unsigned long long*)(w.ctr + 8);
     if (point_mode == 1) {
       cudaMemsetAsync(best, 0, 8, st);
       argmax_kernel<<<grid_for(hw), 256, 0, st>>>(mask, ld, stats, w.f2, best);
-      VOL_LAUNCH_CHECK("mask_prompts_argmax");
+      LAUNCH_CHECK("mask_prompts_argmax");
     } else {
       for (int which = 0; which < 2; ++which) {
         const int d = which == 0 ? 3 : 5;
         peak_rows_kernel<<<grid_for(hw), 256, 0, st>>>(mask, ld, stats, w.f2, which, d, w.rmax, w.ctr);
-        VOL_LAUNCH_CHECK("mask_prompts_peak_rows");
+        LAUNCH_CHECK("mask_prompts_peak_rows");
         peak_cand_kernel<<<grid_for(hw), 256, 0, st>>>(mask, ld, stats, w.f2, which, d, w.rmax, w.ctr, w.cand);
-        VOL_LAUNCH_CHECK("mask_prompts_peak_cand");
+        LAUNCH_CHECK("mask_prompts_peak_cand");
       }
       const int smem = 8 * kMaxCand;
       cudaFuncSetAttribute(peak_thin_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
       peak_thin_kernel<<<2, 512, smem, st>>>(stats, w.ctr, w.cand, w.kept);
-      VOL_LAUNCH_CHECK("mask_prompts_peak_thin");
+      LAUNCH_CHECK("mask_prompts_peak_thin");
     }
     points_out_kernel<<<1, 32, 0, st>>>(H, W, point_mode, stats, stats, w.ctr, best, w.kept, max_points, points, labels);
-    VOL_LAUNCH_CHECK("mask_prompts_points");
+    LAUNCH_CHECK("mask_prompts_points");
     if (field)
       if (cudaMemcpyAsync(field, w.f2, (size_t)4 * hw, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
         return set_error("mask_prompts: field copy failed");
@@ -530,7 +523,7 @@ int mask_iou_counts(const uint8_t* a, int lda, const uint8_t* b, int ldb, int H,
   if (H <= 0 || W <= 0 || lda < W || ldb < W) return set_error("mask_iou_counts: bad arguments H=%d W=%d lda=%d ldb=%d", H, W, lda, ldb);
   if (cudaMemsetAsync(counts, 0, 16, st) != cudaSuccess) return set_error("mask_iou_counts: memset failed");
   iou_kernel<<<grid_for((long)H * W), 256, 0, st>>>(a, lda, b, ldb, H, W, counts);
-  VOL_LAUNCH_CHECK("mask_iou_counts");
+  LAUNCH_CHECK("mask_iou_counts");
   return 0;
 }
 
