@@ -347,6 +347,22 @@ int msam_mask_prompts(const uint8_t* mask, int H, int W, int ld, double box_exte
 /* util.compute_iou's counts (micro_sam/util.py:1266-1280): counts int64 [2] = (|a == 1 & b == 1|, |a == 1 | b == 1|) of two
  * uint8 [H, W] masks with row pitches lda, ldb.  The ratio is formed by the caller in fp64. */
 int msam_mask_iou_counts(const uint8_t* a, int lda, const uint8_t* b, int ldb, int H, int W, int64_t* counts, void* stream);
+/* Object features of micro-sam's object classification (csrc/objfeat.cu; micro_sam/object_classification.py:20-193): one unit
+ * (image, slice or tile) of _compute_object_features_impl with resize_embedding_shape's grid (ry, rx), accumulated.
+ * emb: fp32 [256, 64, 64] contiguous.  seg: int32 [h, w] with row pitch ld >= w, dense label indices: 0 is background, v in
+ * [1, n_ids] is object v - 1 (other values are ignored).  The segmentation is padded to S = max(h, w) and both it (nearest) and
+ * the embedding (bilinear, Gaussian prefilter on axes with r < 64) are resized to ry x rx as skimage's resize does;
+ * 1 <= ry, rx <= min(S, 8192).  Adds each object's sum of the resized embedding over its resized pixels to sums fp64
+ * [n_ids, 256] and its pixel count to areas int64 [n_ids]; the caller zeroes both before the first unit.  Bit-identical from
+ * run to run.  workspace: msam_object_features_workspace(n_ids) bytes of device memory. */
+int64_t msam_object_features_workspace(int n_ids);
+int msam_object_features(const float* emb, const int32_t* seg, int ld, int h, int w, int ry, int rx, int n_ids, void* workspace,
+                         int64_t ws_bytes, double* sums, int64_t* areas, void* stream);
+/* out [n_ids, 257] (fp64 with out_f64, else fp32): column 0 the area, columns 1..256 sums / area; rows of area 0 are zero. */
+int msam_object_features_finish(const double* sums, const int64_t* areas, int n_ids, int out_f64, void* out, void* stream);
+/* project_prediction_to_segmentation (object_classification.py:196-217): out[i] = values[k] where ids[k] == seg[i], else 0.
+ * seg, out int64 [n]; ids int64 [n_ids] sorted ascending without repeats; values [n_ids] of any 8-byte type, copied bitwise. */
+int msam_project_labels(const int64_t* seg, int64_t n, const int64_t* ids, const int64_t* values, int n_ids, int64_t* out, void* stream);
 /* debug: device buffer of 64 x 16 uint64 %globaltimer stamps written by the window-attention kernels, NULL = off */
 int msam_debug_attn_trace(void* dev_buf);
 

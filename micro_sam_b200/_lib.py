@@ -127,6 +127,12 @@ def lib() -> ctypes.CDLL:
         L.msam_mask_prompts.argtypes = [c_void_p, c_int, c_int, c_int, c_double, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p,
                                         c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
         L.msam_mask_iou_counts.argtypes = [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]
+        L.msam_object_features_workspace.restype = c_int64
+        L.msam_object_features_workspace.argtypes = [c_int]
+        L.msam_object_features.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p,
+                                           c_void_p, c_void_p]
+        L.msam_object_features_finish.argtypes = [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]
+        L.msam_project_labels.argtypes = [c_void_p, c_int64, c_void_p, c_void_p, c_int, c_void_p, c_void_p]
         _lib = L
     return _lib
 

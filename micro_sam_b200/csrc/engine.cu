@@ -626,6 +626,20 @@ int msam_mask_iou_counts(const uint8_t* a, int lda, const uint8_t* b, int ldb, i
   if (!a || !b || !counts) return set_error("msam_mask_iou_counts: null argument");
   return mask_iou_counts(a, lda, b, ldb, H, W, counts, (cudaStream_t)stream);
 }
+int64_t msam_object_features_workspace(int n_ids) { return n_ids >= 0 ? object_features_workspace(n_ids) : -1; }
+int msam_object_features(const float* emb, const int32_t* seg, int ld, int h, int w, int ry, int rx, int n_ids, void* workspace,
+                         int64_t ws_bytes, double* sums, int64_t* areas, void* stream) {
+  if (!emb || !seg || !workspace || !sums || !areas) return set_error("msam_object_features: null argument");
+  return object_features(emb, seg, ld, h, w, ry, rx, n_ids, workspace, ws_bytes, sums, areas, (cudaStream_t)stream);
+}
+int msam_object_features_finish(const double* sums, const int64_t* areas, int n_ids, int out_f64, void* out, void* stream) {
+  if (n_ids > 0 && (!sums || !areas || !out)) return set_error("msam_object_features_finish: null argument");
+  return object_features_finish(sums, areas, n_ids, out_f64, out, (cudaStream_t)stream);
+}
+int msam_project_labels(const int64_t* seg, int64_t n, const int64_t* ids, const int64_t* values, int n_ids, int64_t* out, void* stream) {
+  if (n > 0 && (!seg || !out || (n_ids > 0 && (!ids || !values)))) return set_error("msam_project_labels: null argument");
+  return project_labels(seg, n, ids, values, n_ids, out, (cudaStream_t)stream);
+}
 int msam_to_image(const void* src, int dtype, int h, int w, int c, uint8_t* out_hwc3, uint32_t* scratch6, void* stream) {
   return post_to_image(src, dtype, h, w, c, out_hwc3, scratch6, (cudaStream_t)stream);
 }

@@ -239,4 +239,12 @@ int mask_prompts(const uint8_t* mask, int H, int W, int ld, double box_extension
                  float* field, cudaStream_t st);
 int mask_iou_counts(const uint8_t* a, int lda, const uint8_t* b, int ldb, int H, int W, int64_t* counts, cudaStream_t st);
 
+// ---- objfeat.cu: per-object embedding features of object classification and the projection of object predictions
+int64_t object_features_workspace(int n_ids);
+int object_features(const float* emb, const int32_t* seg, int ld, int h, int w, int ry, int rx, int n_ids, void* workspace,
+                    int64_t ws_bytes, double* sums, int64_t* areas, cudaStream_t st);
+int object_features_finish(const double* sums, const int64_t* areas, int n_ids, int out_f64, void* out, cudaStream_t st);
+int project_labels(const int64_t* seg, int64_t n, const int64_t* ids, const int64_t* values, int n_ids, int64_t* out,
+                   cudaStream_t st);
+
 }  // namespace msam
