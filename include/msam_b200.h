@@ -347,6 +347,11 @@ int msam_mask_prompts(const uint8_t* mask, int H, int W, int ld, double box_exte
 /* util.compute_iou's counts (micro_sam/util.py:1266-1280): counts int64 [2] = (|a == 1 & b == 1|, |a == 1 | b == 1|) of two
  * uint8 [H, W] masks with row pitches lda, ldb.  The ratio is formed by the caller in fp64. */
 int msam_mask_iou_counts(const uint8_t* a, int lda, const uint8_t* b, int ldb, int H, int W, int64_t* counts, void* stream);
+/* The tracking annotator's _shift_object (micro_sam/sam_annotator/util.py:576-579): dst = scipy.ndimage.shift(src, (dy, dx),
+ * order=0, prefilter=False) with mode 'constant', cval 0, bit for bit, for multi_dimensional_segmentation.track_from_prompts.
+ * src, dst: uint8 [H, W] with row pitches ld_src, ld_dst >= W; they must not overlap.  Per axis x = o - s in fp64; dst[o] is 0
+ * unless 0 <= x <= n - 1 on both axes, else src[floor(x + 0.5)].  A NaN shift gives an all-zero plane. */
+int msam_shift_mask(const uint8_t* src, int ld_src, uint8_t* dst, int ld_dst, int H, int W, double dy, double dx, void* stream);
 /* Object features of micro-sam's object classification (csrc/objfeat.cu; micro_sam/object_classification.py:20-193): one unit
  * (image, slice or tile) of _compute_object_features_impl with resize_embedding_shape's grid (ry, rx), accumulated.
  * emb: fp32 [256, 64, 64] contiguous.  seg: int32 [h, w] with row pitch ld >= w, dense label indices: 0 is background, v in

@@ -127,6 +127,7 @@ def lib() -> ctypes.CDLL:
         L.msam_mask_prompts.argtypes = [c_void_p, c_int, c_int, c_int, c_double, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p,
                                         c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
         L.msam_mask_iou_counts.argtypes = [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]
+        L.msam_shift_mask.argtypes = [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_double, c_double, c_void_p]
         L.msam_object_features_workspace.restype = c_int64
         L.msam_object_features_workspace.argtypes = [c_int]
         L.msam_object_features.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p,

@@ -626,6 +626,10 @@ int msam_mask_iou_counts(const uint8_t* a, int lda, const uint8_t* b, int ldb, i
   if (!a || !b || !counts) return set_error("msam_mask_iou_counts: null argument");
   return mask_iou_counts(a, lda, b, ldb, H, W, counts, (cudaStream_t)stream);
 }
+int msam_shift_mask(const uint8_t* src, int ld_src, uint8_t* dst, int ld_dst, int H, int W, double dy, double dx, void* stream) {
+  if (!src || !dst) return set_error("msam_shift_mask: null argument");
+  return shift_mask(src, ld_src, dst, ld_dst, H, W, dy, dx, (cudaStream_t)stream);
+}
 int64_t msam_object_features_workspace(int n_ids) { return n_ids >= 0 ? object_features_workspace(n_ids) : -1; }
 int msam_object_features(const float* emb, const int32_t* seg, int ld, int h, int w, int ry, int rx, int n_ids, void* workspace,
                          int64_t ws_bytes, double* sums, int64_t* areas, void* stream) {

@@ -238,6 +238,7 @@ int mask_prompts(const uint8_t* mask, int H, int W, int ld, double box_extension
                  void* workspace, int64_t ws_bytes, int64_t* stats, float* box1024, float* logits, float* points, float* labels,
                  float* field, cudaStream_t st);
 int mask_iou_counts(const uint8_t* a, int lda, const uint8_t* b, int ldb, int H, int W, int64_t* counts, cudaStream_t st);
+int shift_mask(const uint8_t* src, int ld_src, uint8_t* dst, int ld_dst, int H, int W, double dy, double dx, cudaStream_t st);
 
 // ---- objfeat.cu: per-object embedding features of object classification and the projection of object predictions
 int64_t object_features_workspace(int n_ids);

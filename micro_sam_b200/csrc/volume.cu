@@ -10,6 +10,7 @@
 //               sqrt in fp64), scipy's gaussian_filter(sigma=1) (reflect, radius 4, fp64 sums, fp32 after each axis), then
 //               the first argmax of the inner field or _peak_local_max(inner, 3) + _peak_local_max(outer, 5)
 //   iou       : util.compute_iou's intersection and union counts
+//   shift     : scipy.ndimage.shift(order=0) of a mask by the tracking annotator's motion model (track_from_prompts)
 // Every floating-point operation whose rounding matters is written with an explicit-rounding intrinsic, so nvcc's FMA
 // contraction cannot change a result.
 #include <algorithm>
@@ -432,6 +433,25 @@ __global__ void iou_kernel(const uint8_t* __restrict__ a, int lda, const uint8_t
   }
 }
 
+// scipy.ndimage.shift(src, (dy, dx), order=0, prefilter=False, mode='constant', cval=0): per axis x = o - s in fp64; the
+// pixel is 0 unless 0 <= x <= n - 1 on both axes (a NaN shift fails the test everywhere), else src[floor(x + 0.5)]
+__device__ __forceinline__ int shift_src(int o, double s, int n) {
+  const double x = __dsub_rn((double)o, s);
+  return x >= 0.0 && x <= (double)(n - 1) ? (int)floor(__dadd_rn(x, 0.5)) : -1;
+}
+
+// rows over blockIdx.y (the source row is resolved once per row), columns over x
+__global__ void shift_kernel(const uint8_t* __restrict__ src, int ld_src, uint8_t* __restrict__ dst, int ld_dst, int H, int W, double dy,
+                             double dx) {
+  for (int y = blockIdx.y; y < H; y += gridDim.y) {
+    const int sy = shift_src(y, dy, H);
+    for (int x = blockIdx.x * blockDim.x + threadIdx.x; x < W; x += gridDim.x * blockDim.x) {
+      const int sx = shift_src(x, dx, W);
+      dst[(long)y * ld_dst + x] = (sy >= 0 && sx >= 0) ? src[(long)sy * ld_src + sx] : 0;
+    }
+  }
+}
+
 int grid_for(long n) { return (int)std::max<long>(1, std::min<long>((n + 255) / 256, 2048)); }
 
 }  // namespace
@@ -524,6 +544,14 @@ int mask_iou_counts(const uint8_t* a, int lda, const uint8_t* b, int ldb, int H,
   if (cudaMemsetAsync(counts, 0, 16, st) != cudaSuccess) return set_error("mask_iou_counts: memset failed");
   iou_kernel<<<grid_for((long)H * W), 256, 0, st>>>(a, lda, b, ldb, H, W, counts);
   LAUNCH_CHECK("mask_iou_counts");
+  return 0;
+}
+
+int shift_mask(const uint8_t* src, int ld_src, uint8_t* dst, int ld_dst, int H, int W, double dy, double dx, cudaStream_t st) {
+  if (H <= 0 || W <= 0 || ld_src < W || ld_dst < W)
+    return set_error("shift_mask: bad arguments H=%d W=%d ld_src=%d ld_dst=%d", H, W, ld_src, ld_dst);
+  shift_kernel<<<dim3(std::min((W + 255) / 256, 64), std::min(H, 65535)), 256, 0, st>>>(src, ld_src, dst, ld_dst, H, W, dy, dx);
+  LAUNCH_CHECK("shift_mask");
   return 0;
 }
 
