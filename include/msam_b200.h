@@ -204,6 +204,29 @@ int msam_op_layernorm(const float* x, int rows, int D, const float* gamma, const
 /* Encoder attention on a packed qkv buffer (see csrc/attention.cu). rel_table: bf16 [NT, 64*ceil(hd/64)]. */
 int msam_op_attention(const void* qkv_bf16, const void* rel_table_bf16, void* out_bf16, int batch, int heads, int head_dim,
                       int window, float scale, void* stream);
+/* The TinyViT (vit_t) encoder's CUDA-core kernels, launched as msam_encode launches them (csrc/tinyvit.cu).  Each returns -1 with
+ * a message and launches nothing when an argument breaks what its kernel assumes.
+ * stem: Sam.preprocess of uint8 HWC [B, hh, ww, 3] (zero pad to img x img; hh, ww <= img) or of nothing (f32 = preprocessed
+ * NCHW [B, 3, img, img]; exactly one of u8 / f32), conv3x3/2 pad 1 with w27x32 [(ky*3+kx)*3 + c][32] and b32 (BatchNorm
+ * folded), GELU -> bf16 NHWC [B, img/2, img/2, 32].  img even. */
+int msam_op_tv_stem(const uint8_t* u8, const float* f32, int B, int hh, int ww, int img, const float* w27x32, const float* b32,
+                    void* out_bf16, void* stream);
+/* im2col of a 3x3 / pad 1 conv on bf16 NHWC [B, Hin, Hin, C] -> [B * Ho * Ho, 9 * C] (column (ky*3+kx)*C + c), Ho = Hin / stride;
+ * C % 8 == 0, stride 1 or 2, Hin even with stride 2. */
+int msam_op_tv_im2col(const void* x_bf16, int B, int Hin, int C, int stride, void* out_bf16, void* stream);
+/* Depth-wise conv3x3 pad 1 + bias (w9xC [9][C] fp32, BatchNorm folded), GELU when act, on bf16 NHWC; shapes as im2col. */
+int msam_op_tv_dwconv_bf16(const void* x_bf16, int B, int Hin, int C, int stride, const float* w9xC, const float* b, int act,
+                           void* out_bf16, void* stream);
+/* The same with stride 1 on fp32 NHWC (the blocks' local_conv); C % 4 == 0. */
+int msam_op_tv_dwconv_f32(const float* x, int B, int Hin, int C, const float* w9xC, const float* b, float* out, void* stream);
+/* LayerNorm of fp32 [B, H, H, D] into the window-partitioned bf16 rows [B * nw * nw * ws * ws, D], nw = ceil(H / ws); the rows
+ * of the zero pad tokens are LayerNorm(0) = beta.  D % 4 == 0, D <= 384, ws 7 or 14. */
+int msam_op_tv_ln_window(const float* x, int B, int H, int D, int ws, const float* gamma, const float* beta, float eps,
+                         void* out_bf16, void* stream);
+/* Window attention, head_dim 32, scale 32^-0.5: qkv bf16 [B * nw * nw * ws * ws, heads * 96] (per head [q | k | v], pad tokens
+ * included as keys), bias_tab fp32 [heads, ws * ws] indexed by |dy| * ws + |dx| -> bf16 [B * H * H, heads * 32] in image order. */
+int msam_op_tv_attention(const void* qkv_bf16, const float* bias_tab, int B, int H, int ws, int heads, void* out_bf16,
+                         void* stream);
 /* The three fused mask-decoder blocks, running the code msam_decode runs for them, on explicit bf16 inputs with the weights as
  * loaded.  P <= max_prompts prompts of T tokens (5 <= T <= 16).  num_sms caps the grid of the persistent kernels (0 = the
  * device's SM count): results must not depend on it.

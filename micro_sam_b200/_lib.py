@@ -44,6 +44,12 @@ def lib() -> ctypes.CDLL:
         L.msam_op_gemm_nn.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]
         L.msam_op_layernorm.argtypes = [c_void_p, c_int, c_int, c_void_p, c_void_p, c_float, c_void_p, c_int, c_void_p]
         L.msam_op_attention.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]
+        L.msam_op_tv_stem.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
+        L.msam_op_tv_im2col.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
+        L.msam_op_tv_dwconv_bf16.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p]
+        L.msam_op_tv_dwconv_f32.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
+        L.msam_op_tv_ln_window.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_void_p, c_void_p]
+        L.msam_op_tv_attention.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
         L.msam_op_dec_t2i.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p]
         L.msam_op_dec_i2t.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p]
         L.msam_op_dec_upscale.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p]

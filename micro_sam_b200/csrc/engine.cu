@@ -767,6 +767,71 @@ int msam_op_attention(const void* qkv, const void* rel_table, void* out, int bat
   return launch_attention(a, (cudaStream_t)stream);
 }
 
+// TinyViT kernels: every precondition the kernels rely on without checking it is refused here, before anything is launched.
+static bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+int msam_op_tv_stem(const uint8_t* u8, const float* f32, int B, int hh, int ww, int img, const float* w27x32, const float* b32,
+                    void* out_bf16, void* stream) {
+  if ((u8 == nullptr) == (f32 == nullptr)) return set_error("msam_op_tv_stem: exactly one of u8 / f32 must be given");
+  if (!w27x32 || !b32 || !out_bf16) return set_error("msam_op_tv_stem: null argument");
+  if (B <= 0 || img <= 0 || img % 2) return set_error("msam_op_tv_stem: B=%d, img=%d (img must be even and positive)", B, img);
+  if (u8 && (hh <= 0 || ww <= 0 || hh > img || ww > img))
+    return set_error("msam_op_tv_stem: image %dx%d outside 1..%d", hh, ww, img);
+  if (!aligned16(out_bf16)) return set_error("msam_op_tv_stem: out is not 16-byte aligned");
+  return launch_tv_stem1(u8, f32, B, hh, ww, img, w27x32, b32, (__nv_bfloat16*)out_bf16, (cudaStream_t)stream);
+}
+
+static int tv_conv_args(const char* op, const void* x, int B, int Hin, int C, int stride, int cmul, const void* out) {
+  if (!x || !out) return set_error("%s: null argument", op);
+  if (B <= 0 || Hin <= 0 || C <= 0 || C % cmul) return set_error("%s: B=%d, Hin=%d, C=%d (C must be a multiple of %d)", op, B, Hin, C, cmul);
+  if (stride != 1 && stride != 2) return set_error("%s: stride %d (1 or 2)", op, stride);
+  if (stride == 2 && Hin % 2) return set_error("%s: odd Hin=%d with stride 2 (the kernel's output side is Hin / 2)", op, Hin);
+  if (!aligned16(x) || !aligned16(out)) return set_error("%s: x / out not 16-byte aligned", op);
+  return 0;
+}
+
+int msam_op_tv_im2col(const void* x_bf16, int B, int Hin, int C, int stride, void* out_bf16, void* stream) {
+  if (tv_conv_args("msam_op_tv_im2col", x_bf16, B, Hin, C, stride, 8, out_bf16)) return -1;
+  return launch_tv_im2col((const __nv_bfloat16*)x_bf16, B, Hin, C, stride, (__nv_bfloat16*)out_bf16, (cudaStream_t)stream);
+}
+
+int msam_op_tv_dwconv_bf16(const void* x_bf16, int B, int Hin, int C, int stride, const float* w9xC, const float* b, int act,
+                           void* out_bf16, void* stream) {
+  if (tv_conv_args("msam_op_tv_dwconv_bf16", x_bf16, B, Hin, C, stride, 8, out_bf16)) return -1;
+  if (!w9xC || !b) return set_error("msam_op_tv_dwconv_bf16: null argument");
+  if (!aligned16(w9xC) || !aligned16(b)) return set_error("msam_op_tv_dwconv_bf16: w / b not 16-byte aligned");
+  return launch_tv_dwconv_bf16((const __nv_bfloat16*)x_bf16, B, Hin, C, stride, w9xC, b, act, (__nv_bfloat16*)out_bf16,
+                               (cudaStream_t)stream);
+}
+
+int msam_op_tv_dwconv_f32(const float* x, int B, int Hin, int C, const float* w9xC, const float* b, float* out, void* stream) {
+  if (tv_conv_args("msam_op_tv_dwconv_f32", x, B, Hin, C, 1, 4, out)) return -1;
+  if (!w9xC || !b) return set_error("msam_op_tv_dwconv_f32: null argument");
+  if (!aligned16(w9xC) || !aligned16(b)) return set_error("msam_op_tv_dwconv_f32: w / b not 16-byte aligned");
+  return launch_tv_dwconv_f32(x, B, Hin, C, w9xC, b, out, (cudaStream_t)stream);
+}
+
+int msam_op_tv_ln_window(const float* x, int B, int H, int D, int ws, const float* gamma, const float* beta, float eps,
+                         void* out_bf16, void* stream) {
+  if (!x || !gamma || !beta || !out_bf16) return set_error("msam_op_tv_ln_window: null argument");
+  if (B <= 0 || H <= 0 || D <= 0 || D % 4 || D > 384)
+    return set_error("msam_op_tv_ln_window: B=%d, H=%d, D=%d (D a multiple of 4, at most 384)", B, H, D);
+  if (ws != 7 && ws != 14) return set_error("msam_op_tv_ln_window: window %d (7 or 14)", ws);
+  if (!aligned16(x) || !aligned16(gamma) || !aligned16(beta) || ((uintptr_t)out_bf16 & 7))
+    return set_error("msam_op_tv_ln_window: misaligned pointer");
+  return launch_tv_ln_window(x, B, H, D, ws, gamma, beta, eps, (__nv_bfloat16*)out_bf16, (cudaStream_t)stream);
+}
+
+int msam_op_tv_attention(const void* qkv_bf16, const float* bias_tab, int B, int H, int ws, int heads, void* out_bf16,
+                         void* stream) {
+  if (!qkv_bf16 || !bias_tab || !out_bf16) return set_error("msam_op_tv_attention: null argument");
+  if (B <= 0 || H <= 0 || heads <= 0 || heads > 65535) return set_error("msam_op_tv_attention: B=%d, H=%d, heads=%d", B, H, heads);
+  if (ws != 7 && ws != 14) return set_error("msam_op_tv_attention: window %d (7 or 14)", ws);
+  if (!aligned16(qkv_bf16) || !aligned16(out_bf16)) return set_error("msam_op_tv_attention: qkv / out not 16-byte aligned");
+  return launch_tv_attention((const __nv_bfloat16*)qkv_bf16, bias_tab, B, H, ws, heads, (__nv_bfloat16*)out_bf16,
+                             (cudaStream_t)stream);
+}
+
 int msam_op_dec_t2i(msam_handle* h, int which, const void* q_pe, const void* keys, int P, int T, void* out, int num_sms,
                     void* stream) {
   if (!h) return set_error("msam_op_dec_t2i: null handle");

@@ -206,4 +206,24 @@ int launch_layernorm2d_nchw(const float* x, int B, int T, const float* gamma, co
 int launch_cast_bf16(const float* x, long n, __nv_bfloat16* out, cudaStream_t stream);
 int launch_im2col3x3(const __nv_bfloat16* x, int B, int g, int C, __nv_bfloat16* out, cudaStream_t stream);
 
+// ---- tinyvit.cu : the CUDA-core kernels of the TinyViT (vit_t) encoder.  No argument checks here (the msam_op_tv_* entry
+// points of engine.cu make them); each helper is the launch Engine::encode_tinyvit makes.
+// Stem conv 1: Sam.preprocess of uint8 HWC [B, h, w, 3] (or preprocessed fp32 NCHW [B, 3, img, img] when f32 is set) + conv3x3/2
+// (w [27][32], tap-major (ky*3+kx)*3 + c) + folded BN + GELU -> bf16 NHWC [B, img/2, img/2, 32].
+int launch_tv_stem1(const uint8_t* u8, const float* f32, int B, int h, int w, int img, const float* wt, const float* bias,
+                    __nv_bfloat16* out, cudaStream_t stream);
+// im2col of a 3x3 / pad 1 conv with stride on bf16 NHWC [B, Hin, Hin, C] -> [B * Ho * Ho, 9 * C], Ho = Hin / stride.
+int launch_tv_im2col(const __nv_bfloat16* x, int B, int Hin, int C, int stride, __nv_bfloat16* out, cudaStream_t stream);
+// Depth-wise conv3x3 pad 1 + folded BN (w [9][C], b [C]) (+ GELU when act) on NHWC: bf16 with stride 1 / 2, fp32 with stride 1.
+int launch_tv_dwconv_bf16(const __nv_bfloat16* x, int B, int Hin, int C, int stride, const float* w, const float* b, int act,
+                          __nv_bfloat16* out, cudaStream_t stream);
+int launch_tv_dwconv_f32(const float* x, int B, int Hin, int C, const float* w, const float* b, float* out, cudaStream_t stream);
+// LayerNorm of fp32 [B, H, H, D] scattered into the window-partitioned bf16 rows of ws x ws windows; pad rows = bf16(beta).
+int launch_tv_ln_window(const float* x, int B, int H, int D, int ws, const float* gamma, const float* beta, float eps,
+                        __nv_bfloat16* out, cudaStream_t stream);
+// Window attention (head_dim 32, scale 32^-0.5, bias_tab [heads][ws*ws] indexed by |dy|*ws + |dx|) on window-partitioned qkv
+// [windows * ws*ws, heads * 96] -> bf16 [B*H*H, heads * 32] in image token order.  ws = 7 or 14.
+int launch_tv_attention(const __nv_bfloat16* qkv, const float* bias_tab, int B, int H, int ws, int heads, __nv_bfloat16* out,
+                        cudaStream_t stream);
+
 }  // namespace msam

@@ -300,8 +300,31 @@ tv_attn_kernel(const __nv_bfloat16* __restrict__ qkv, const float* __restrict__ 
                    pack_bf16(acc[ch * 8 + 4] * inv, acc[ch * 8 + 5] * inv), pack_bf16(acc[ch * 8 + 6] * inv, acc[ch * 8 + 7] * inv));
 }
 
-int tv_dwconv_bf16(const __nv_bfloat16* x, int B, int Hin, int C, int stride, const float* w, const float* b, int act,
-                   __nv_bfloat16* out, cudaStream_t st) {
+}  // namespace
+
+// ------------------------------------------------------------------------------------------------ launches
+int launch_tv_stem1(const uint8_t* u8, const float* f32, int B, int h, int w, int img, const float* wt, const float* bias,
+                    __nv_bfloat16* out, cudaStream_t st) {
+  static const float mean[3] = {123.675f, 116.28f, 103.53f}, stdv[3] = {58.395f, 57.12f, 57.375f};
+  const int ho = img / 2;
+  const long total = (long)B * ho * ho * 4;
+  prof_begin(st, "tinyvit stem conv1", 2.0 * B * ho * ho * 27 * 32, (double)B * ((double)img * img * 3 + (double)ho * ho * 32 * 2));
+  tv_stem1_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(u8, f32, B, h, w, img, mean[0], mean[1], mean[2], stdv[0],
+                                                                stdv[1], stdv[2], wt, bias, out);
+  prof_end(st);
+  LAUNCH_CHECK("stem conv1");
+  return 0;
+}
+
+int launch_tv_im2col(const __nv_bfloat16* x, int B, int Hin, int C, int stride, __nv_bfloat16* out, cudaStream_t st) {
+  const long tc = (long)B * (Hin / stride) * (Hin / stride) * 9 * (C / 8);
+  tv_im2col_kernel<<<(unsigned)((tc + 255) / 256), 256, 0, st>>>(x, B, Hin, C, stride, out);
+  LAUNCH_CHECK("stem im2col");
+  return 0;
+}
+
+int launch_tv_dwconv_bf16(const __nv_bfloat16* x, int B, int Hin, int C, int stride, const float* w, const float* b, int act,
+                          __nv_bfloat16* out, cudaStream_t st) {
   const long total = (long)B * (Hin / stride) * (Hin / stride) * (C / 8);
   prof_begin(st, "tinyvit dwconv3x3 (bf16)", 0.0, (double)B * Hin * Hin * C * 2 + (double)total * 16);
   tv_dwconv_bf16_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x, B, Hin, C, stride, w, b, act, out);
@@ -310,7 +333,42 @@ int tv_dwconv_bf16(const __nv_bfloat16* x, int B, int Hin, int C, int stride, co
   return 0;
 }
 
-}  // namespace
+int launch_tv_dwconv_f32(const float* x, int B, int Hin, int C, const float* w, const float* b, float* out, cudaStream_t st) {
+  const long total = (long)B * Hin * Hin * (C / 4);
+  tv_dwconv_f32_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x, B, Hin, C, w, b, out);
+  LAUNCH_CHECK("local conv");
+  return 0;
+}
+
+int launch_tv_ln_window(const float* x, int B, int H, int D, int ws, const float* gamma, const float* beta, float eps,
+                        __nv_bfloat16* out, cudaStream_t st) {
+  const int nw = (H + ws - 1) / ws;
+  const long warps = (long)B * nw * nw * ws * ws;   // one warp per window-partitioned row
+  tv_ln_window_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(x, B, H, D, ws, gamma, beta, eps, out);
+  LAUNCH_CHECK("window layernorm");
+  return 0;
+}
+
+int launch_tv_attention(const __nv_bfloat16* qkv, const float* bias_tab, int B, int H, int ws, int heads, __nv_bfloat16* out,
+                        cudaStream_t st) {
+  const int N = ws * ws, nw = (H + ws - 1) / ws;
+  const long Mw = (long)B * nw * nw * N, M = (long)B * H * H;
+  const float scale = 1.0f / sqrtf(32.0f);
+  prof_begin(st, "tinyvit window attention", 4.0 * B * nw * nw * heads * (double)N * N * 32,
+             (double)Mw * heads * 96 * 2 + (double)M * heads * 32 * 2);
+  constexpr int SM7 = (2 * 52 * 32 + 49) * 4, SM14 = (2 * 196 * 32 + 196) * 4;
+  static bool attr_set = false;
+  if (!attr_set) {
+    if (cudaFuncSetAttribute(tv_attn_kernel<14>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM14) != cudaSuccess)
+      return set_error("tinyvit attention: cudaFuncSetAttribute failed");
+    attr_set = true;
+  }
+  if (ws == 7) tv_attn_kernel<7><<<dim3(B * nw * nw, heads), 64, SM7, st>>>(qkv, bias_tab, heads, H, scale, out);
+  else tv_attn_kernel<14><<<dim3(B * nw * nw, heads), 224, SM14, st>>>(qkv, bias_tab, heads, H, scale, out);
+  prof_end(st);
+  LAUNCH_CHECK("window attention");
+  return 0;
+}
 
 // ------------------------------------------------------------------------------------------------ weights
 namespace {
@@ -467,7 +525,7 @@ static int tv_merge(Engine& e, const TvMerge& m, const __nv_bfloat16* in, int nb
                     float* x_out, cudaStream_t st) {
   const int Min = nb * Hin * Hin, Ho = Hin / stride, Mo = nb * Ho * Ho;
   if (tv_gemm(e, in, m.conv1.w, Min, out_dim, dim, m.conv1.b, 1, nullptr, 0, 0, e.tv.h1, 0, st)) return -1;
-  if (tv_dwconv_bf16(e.tv.h1, nb, Hin, out_dim, stride, m.conv2.wf, m.conv2.b, 1, e.tv.h2, st)) return -1;
+  if (launch_tv_dwconv_bf16(e.tv.h1, nb, Hin, out_dim, stride, m.conv2.wf, m.conv2.b, 1, e.tv.h2, st)) return -1;
   return tv_gemm(e, e.tv.h2, m.conv3.w, Mo, out_dim, out_dim, m.conv3.b, 0, nullptr, 0, 0, x_out, 1, st);
 }
 
@@ -477,29 +535,19 @@ int Engine::encode_tinyvit(const uint8_t* u8, const float* f32, int B, int hh, i
   if (B <= 0) return set_error("msam_encode: empty batch");
   const int img = cfg.image_size, C = cfg.out_chans;
   if (u8 && (hh > img || ww > img || hh <= 0 || ww <= 0)) return set_error("msam_encode_u8: image %dx%d exceeds %d", hh, ww, img);
-  static const float mean[3] = {123.675f, 116.28f, 103.53f}, stdv[3] = {58.395f, 57.12f, 57.375f};
   for (int b0 = 0; b0 < B; b0 += cfg.max_batch) {
     const int nb = (B - b0 < cfg.max_batch) ? (B - b0) : cfg.max_batch;
     const uint8_t* u8p = u8 ? u8 + (size_t)b0 * hh * ww * 3 : nullptr;
     const float* f32p = f32 ? f32 + (size_t)b0 * 3 * img * img : nullptr;
-    {
-      const long total = (long)nb * 512 * 512 * 4;
-      prof_begin(st, "tinyvit stem conv1", 2.0 * nb * 512 * 512 * 27 * 32, (double)nb * (1024.0 * 1024 * 3 + 512.0 * 512 * 32 * 2));
-      tv_stem1_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(u8p, f32p, nb, hh, ww, img, mean[0], mean[1], mean[2], stdv[0],
-                                                                    stdv[1], stdv[2], tv.stem1.wf, tv.stem1.b, tv.s1);
-      prof_end(st);
-      LAUNCH_CHECK("stem conv1");
-      const long tc = (long)nb * 256 * 256 * 9 * 4;
-      tv_im2col_kernel<<<(unsigned)((tc + 255) / 256), 256, 0, st>>>(tv.s1, nb, 512, 32, 2, tv.col);
-      LAUNCH_CHECK("stem im2col");
-      if (tv_gemm(*this, tv.col, tv.stem2.w, nb * 65536, 64, 288, tv.stem2.b, 0, nullptr, 0, 0, tv.a0, 0, st)) return -1;
-    }
+    if (launch_tv_stem1(u8p, f32p, nb, hh, ww, img, tv.stem1.wf, tv.stem1.b, tv.s1, st)) return -1;
+    if (launch_tv_im2col(tv.s1, nb, 512, 32, 2, tv.col, st)) return -1;
+    if (tv_gemm(*this, tv.col, tv.stem2.w, nb * 65536, 64, 288, tv.stem2.b, 0, nullptr, 0, 0, tv.a0, 0, st)) return -1;
     int stage_idx = 0;   // stop_after counts: 1 = after layers.0 (incl. its downsample), 2 / 3 / 4 = after layers.1 / 2 / 3
     __nv_bfloat16 *cur = tv.a0, *nxt = tv.a1;
     for (int i = 0; i < 2; ++i) {   // MBConv @ 256 x 256, 64 channels
       const int M = nb * 65536;
       if (tv_gemm(*this, cur, tv.mb[i].conv1.w, M, 256, 64, tv.mb[i].conv1.b, 1, nullptr, 0, 0, tv.h1, 0, st)) return -1;
-      if (tv_dwconv_bf16(tv.h1, nb, 256, 256, 1, tv.mb[i].conv2.wf, tv.mb[i].conv2.b, 1, tv.h2, st)) return -1;
+      if (launch_tv_dwconv_bf16(tv.h1, nb, 256, 256, 1, tv.mb[i].conv2.wf, tv.mb[i].conv2.b, 1, tv.h2, st)) return -1;
       if (tv_gemm(*this, tv.h2, tv.mb[i].conv3.w, M, 64, 256, tv.mb[i].conv3.b, 1, cur, 1, 1, nxt, 0, st)) return -1;
       __nv_bfloat16* t = cur; cur = nxt; nxt = t;
     }
@@ -511,33 +559,11 @@ int Engine::encode_tinyvit(const uint8_t* u8, const float* f32, int B, int hh, i
       const int D = S.dim, wsz = S.ws, N = wsz * wsz, nw = (H + wsz - 1) / wsz;
       const int M = nb * H * H, Mw = nb * nw * nw * N;
       for (const TvBlock& b : S.blocks) {
-        {
-          const long warps = Mw;
-          tv_ln_window_kernel<<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(tv.x, nb, H, D, wsz, b.an_g, b.an_b, 1e-5f, tv.xw);
-          LAUNCH_CHECK("window layernorm");
-        }
+        if (launch_tv_ln_window(tv.x, nb, H, D, wsz, b.an_g, b.an_b, 1e-5f, tv.xw, st)) return -1;
         if (tv_gemm(*this, tv.xw, b.qkv_w, Mw, 3 * D, D, b.qkv_b, 0, nullptr, 0, 0, tv.qkv, 0, st)) return -1;
-        {
-          const float scale = 1.0f / sqrtf(32.0f);
-          prof_begin(st, "tinyvit window attention", 4.0 * nb * nw * nw * S.heads * (double)N * N * 32, (double)Mw * 3 * D * 2 + (double)M * D * 2);
-          constexpr int SM7 = (2 * 52 * 32 + 49) * 4, SM14 = (2 * 196 * 32 + 196) * 4;
-          static bool attr_set = false;
-          if (!attr_set) {
-            if (cudaFuncSetAttribute(tv_attn_kernel<14>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM14) != cudaSuccess)
-              return set_error("tinyvit attention: cudaFuncSetAttribute failed");
-            attr_set = true;
-          }
-          if (wsz == 7) tv_attn_kernel<7><<<dim3(nb * nw * nw, S.heads), 64, SM7, st>>>(tv.qkv, b.bias_tab, S.heads, H, scale, tv.attn);
-          else tv_attn_kernel<14><<<dim3(nb * nw * nw, S.heads), 224, SM14, st>>>(tv.qkv, b.bias_tab, S.heads, H, scale, tv.attn);
-          prof_end(st);
-          LAUNCH_CHECK("window attention");
-        }
+        if (launch_tv_attention(tv.qkv, b.bias_tab, nb, H, wsz, S.heads, tv.attn, st)) return -1;
         if (tv_gemm(*this, tv.attn, b.proj_w, M, D, D, b.proj_b, 0, tv.x, 0, 0, tv.x2, 1, st)) return -1;
-        {
-          const long total = (long)M * (D / 4);
-          tv_dwconv_f32_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(tv.x2, nb, H, D, b.local.wf, b.local.b, tv.x);
-          LAUNCH_CHECK("local conv");
-        }
+        if (launch_tv_dwconv_f32(tv.x2, nb, H, D, b.local.wf, b.local.b, tv.x, st)) return -1;
         LnArgs l;
         l.x = tv.x; l.rows = M; l.D = D; l.gamma = b.mn_g; l.beta = b.mn_b; l.eps = 1e-5f; l.out = tv.xn;
         if (launch_layernorm(l, st)) return -1;

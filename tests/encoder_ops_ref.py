@@ -217,6 +217,22 @@ def within(got, ref, rows, tol):
     return finite and rel <= tol[0] and row <= tol[1], (rel, row, finite)
 
 
+# ------------------------------------------------------------------------------------------------ output sentinels
+SENT_BF16, SENT_F32 = 1024.0, -7777.0
+
+
+def guarded(n, dtype, margin=4096, device="cuda"):
+    """A flat buffer of n elements with `margin` sentinel elements on each side; returns (whole, inner view)."""
+    s = SENT_BF16 if dtype == torch.bfloat16 else SENT_F32
+    buf = torch.full((n + 2 * margin,), s, device=device, dtype=dtype)
+    return buf, buf[margin:margin + n]
+
+
+def margins_intact(buf, n, margin=4096):
+    s = SENT_BF16 if buf.dtype == torch.bfloat16 else SENT_F32
+    return bool((buf[:margin] == s).all()) and bool((buf[margin + n:] == s).all())
+
+
 def gelu_mismatch(got, ref, pre):
     """largest fraction, over windows of 256 neighbouring points with |pre| <= 3, of outputs that are not the bf16 rounding of
     the reference.  A derivative that is right to fp32 accuracy flips a rounding only at near-ties; one that is off by 1e-3

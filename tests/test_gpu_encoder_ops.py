@@ -27,10 +27,10 @@ import pytest
 import torch
 
 from tests import encoder_ops_ref as R
+from tests.encoder_ops_ref import SENT_BF16, SENT_F32, guarded, margins_intact
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-SENT_BF16, SENT_F32 = 1024.0, -7777.0
 
 
 # ------------------------------------------------------------------------------------------------ helpers
@@ -39,18 +39,6 @@ def L():
     from micro_sam_b200 import _lib
     _lib.lib()
     return _lib
-
-
-def guarded(n, dtype, margin=4096):
-    """A flat buffer of n elements with `margin` sentinel elements on each side; returns (whole, inner view)."""
-    s = SENT_BF16 if dtype == torch.bfloat16 else SENT_F32
-    buf = torch.full((n + 2 * margin,), s, device=DEV, dtype=dtype)
-    return buf, buf[margin:margin + n]
-
-
-def margins_intact(buf, n, margin=4096):
-    s = SENT_BF16 if buf.dtype == torch.bfloat16 else SENT_F32
-    return bool((buf[:margin] == s).all()) and bool((buf[margin + n:] == s).all())
 
 
 def check(name, got, ref, rows, tol):
@@ -315,15 +303,18 @@ _MS = [1, 63, 64, 65, 127, 129, 9800]
 _NS = [32, 96, 160, 128, 384, 256, 768]
 _KS = [8, 24, 72, 200, 768]
 GEMM_TAILS = sorted({(M, _NS[i % 7], _KS[i % 5]) for i, M in enumerate(_MS)} | {(129, N, _KS[(i + 2) % 5]) for i, N in enumerate(_NS)} |
-                    {(65, _NS[(i + 3) % 7], K) for i, K in enumerate(_KS)} | {(9800, 160, 200), (9800, 768, 72), (1, 256, 8)})
+                    {(65, _NS[(i + 3) % 7], K) for i, K in enumerate(_KS)} | {(9800, 160, 200), (9800, 768, 72), (1, 256, 8)} |
+                    {(65536, 64, 288), (65537, 64, 256)})     # TinyViT: stem conv 2 (im2col, K = 288); MBConv conv3 (below)
 
 
 @pytest.mark.parametrize("f32", [True, False], ids=["f32", "bf16"])
 @pytest.mark.parametrize("M,N,K", GEMM_TAILS)
 def test_gemm_tails(L, M, N, K, f32):
     """Partial last row tile, all three BN instantiations incl. a partial last column tile, K down to 8 and not a multiple
-    of 32 or 64 (the TMA box zero-fills the K tail)."""
-    gemm_case(L, f"gemm M={M} N={N} K={K}", M, N, K, seed=M + N + K, f32=f32)
+    of 32 or 64 (the TMA box zero-fills the K tail).  N = 64, K = 256 runs TinyViT's MBConv conv3 epilogue, GELU(conv3(x) +
+    shortcut) with the shortcut a bf16 residual."""
+    kw = dict(res="bf16", act=1, after=1) if (N, K) == (64, 256) else {}
+    gemm_case(L, f"gemm M={M} N={N} K={K}{' bf16 res, GELU after' if kw else ''}", M, N, K, seed=M + N + K, f32=f32, **kw)
 
 
 @pytest.mark.parametrize("f32", [True, False], ids=["f32", "bf16"])
