@@ -621,16 +621,15 @@ static int t2i_block(Engine& E, cudaStream_t st, const AttnW& A, int P, int T, c
   DecoderState& d = *E.dec;
   const int mode = keys ? 1 : 0;
   if (gemm(E, st, qpe, DC, A.q, P * T, DI, DC, A.qb, d.t_q128, DI, 0)) return -1;
-  // T <= 8: 64 rows per prompt (row pp*64 + h*8 + t).  Shared image tokens (mode 0): two prompts per 128-row item;
-  // own keys (mode 1): one 64-row item per prompt (one warpgroup).  T > 8: 128 rows per prompt (h*16 + t).
+  // T <= 8: 64 rows per prompt, two prompts per 128-row item (row pp*64 + h*8 + t).  T > 8: 128 rows per prompt (h*16 + t).
   const int small = T <= 8 ? 1 : 0;
   const int prep_items = small ? (P + 1) / 2 : P;   // 128-row blocks of the Q' operand
   if (launch_t2i_prep(d.t_q128, P, T, small, prep_items, d.qexp, st)) return -1;
   if (gemm(E, st, d.qexp, DI, A.kT, prep_items * 128, DC, DI, nullptr, d.qp, DC, 0)) return -1;
   T2iFusedArgs ta;
   ta.mode = mode;
-  ta.rows = (small && mode) ? 64 : 128;
-  ta.n_items = (small && mode) ? P : prep_items;
+  ta.P = P;
+  ta.paired = small;
   ta.x = mode ? keys : d.src_bf;
   ta.xs = mode ? d.pos_bf : d.src_pe_bf;
   ta.qp = d.qp; ta.out = d.un;

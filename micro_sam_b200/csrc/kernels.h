@@ -151,13 +151,13 @@ int launch_i2t_prep(const __nv_bfloat16* ktok, const __nv_bfloat16* vtok, const 
 // ---- t2i_fused.cu : fused token -> image cross-attention (k / v projections folded into the query / output side; the image
 // tokens are read once and used as both K and V)
 struct T2iFusedArgs {
-  int n_items = 0;                    // work items of `rows` Q' rows
-  int rows = 128;                     // 128: one prompt (h*16 + t) or two prompts (pl*64 + h*8 + t); 64: one prompt, T <= 8
-  int mode = 0;                       // 1: x = keys [n_items*4096, 256], xs = pe;  0: x = src (shared), xs = src + pe
+  int P = 0;                          // prompts
+  int paired = 0;                     // 128-row items of Q' / out: 1 = two prompts (pl*64 + h*8 + t, T <= 8), 0 = one (h*16 + t)
+  int mode = 0;                       // 1: x = keys [P*4096, 256], xs = pe;  0: x = src (shared), xs = src + pe
   const __nv_bfloat16* x = nullptr;
   const __nv_bfloat16* xs = nullptr;
-  const __nv_bfloat16* qp = nullptr;  // Q' [n_items*128, 256]
-  float* out = nullptr;               // [n_items*128, 256]
+  const __nv_bfloat16* qp = nullptr;  // Q' [items*128, 256]
+  float* out = nullptr;               // [items*128, 256]
 };
 int launch_t2i_fused(const T2iFusedArgs& a, int num_sms, cudaStream_t stream);
 int launch_t2i_prep(const __nv_bfloat16* q, int P, int T, int paired, int n_items, __nv_bfloat16* qexp, cudaStream_t stream);
