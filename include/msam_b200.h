@@ -192,6 +192,12 @@ int msam_op_gemm(const void* A, const void* W, int M, int N, int K, const float*
 int msam_op_gemm_ex(const void* A, const void* W, int M, int N, int K, int lda, int ldw, const float* bias, const void* residual,
                     int res_rows, int ldr, int res_bf16, void* out, int ldc, int out_fp32, int act, int act_after_res, int epi,
                     const float* ln_gamma, const float* ln_beta, float ln_eps, int num_sms, void* stream);
+/* msam_op_gemm_ex with the kernel chosen by `path`: 0 = the choice every other caller gets (the 128 x 256 wide-tile kernel for
+ * plain-epilogue products with N % 256 == 0 and at least one such tile per SM of the device, else the tiled kernel), 1 = the
+ * tiled kernel (column groups of 64, BN = 256 / 128 / 64), 2 = the wide-tile kernel (N % 256 == 0, epi = 0; -1 otherwise). */
+int msam_op_gemm_ex2(const void* A, const void* W, int M, int N, int K, int lda, int ldw, const float* bias, const void* residual,
+                     int res_rows, int ldr, int res_bf16, void* out, int ldc, int out_fp32, int act, int act_after_res, int epi,
+                     const float* ln_gamma, const float* ln_beta, float ln_eps, int num_sms, int path, void* stream);
 /* Weight gradient of a linear layer (first piece of msam_*_backward, cfg 5): out[M,N] fp32 = A[K,M]^T B[K,N], A = dY
  * (tokens x out-features), B = X (tokens x in-features), both bf16 row-major -- torch autograd's dW = dY^T X. */
 int msam_op_gemm_tn(const void* A, const void* B, int M, int N, int K, float* out, void* stream);

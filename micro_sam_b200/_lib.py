@@ -102,6 +102,9 @@ def lib() -> ctypes.CDLL:
         L.msam_debug_attn_trace.argtypes = [c_void_p]
         L.msam_op_gemm_ex.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                       c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_void_p]
+        L.msam_op_gemm_ex2.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int,
+                                       c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_int,
+                                       c_int, c_void_p]
         L.msam_op_attn_probs.argtypes = [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_float, c_void_p, c_void_p]
         L.msam_op_attn_ds.argtypes = [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]
         L.msam_op_pack_dqkv.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]

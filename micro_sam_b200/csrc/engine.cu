@@ -730,6 +730,13 @@ int msam_op_gemm(const void* A, const void* W, int M, int N, int K, const float*
 int msam_op_gemm_ex(const void* A, const void* W, int M, int N, int K, int lda, int ldw, const float* bias, const void* residual,
                     int res_rows, int ldr, int res_bf16, void* out, int ldc, int out_fp32, int act, int act_after_res, int epi,
                     const float* ln_gamma, const float* ln_beta, float ln_eps, int num_sms, void* stream) {
+  return msam_op_gemm_ex2(A, W, M, N, K, lda, ldw, bias, residual, res_rows, ldr, res_bf16, out, ldc, out_fp32, act,
+                          act_after_res, epi, ln_gamma, ln_beta, ln_eps, num_sms, GEMM_PATH_AUTO, stream);
+}
+
+int msam_op_gemm_ex2(const void* A, const void* W, int M, int N, int K, int lda, int ldw, const float* bias, const void* residual,
+                     int res_rows, int ldr, int res_bf16, void* out, int ldc, int out_fp32, int act, int act_after_res, int epi,
+                     const float* ln_gamma, const float* ln_beta, float ln_eps, int num_sms, int path, void* stream) {
   if (!A || !W || !out) return set_error("msam_op_gemm_ex: null argument");
   if (lda < K || ldw < K) return set_error("msam_op_gemm_ex: lda=%d / ldw=%d below K=%d", lda, ldw, K);
   if ((ldc > 0 && ldc < N) || (ldr > 0 && ldr < N)) return set_error("msam_op_gemm_ex: ldc=%d / ldr=%d below N=%d", ldc, ldr, N);
@@ -737,7 +744,7 @@ int msam_op_gemm_ex(const void* A, const void* W, int M, int N, int K, int lda, 
   a.A = (const __nv_bfloat16*)A; a.W = (const __nv_bfloat16*)W; a.M = M; a.N = N; a.K = K; a.lda = lda; a.ldw = ldw;
   a.bias = bias; a.residual = residual; a.res_rows = res_rows; a.ldr = ldr; a.res_bf16 = res_bf16;
   a.out = out; a.ldc = ldc; a.out_fp32 = out_fp32; a.act = act; a.act_after_res = act_after_res;
-  a.epi = epi; a.ln_gamma = ln_gamma; a.ln_beta = ln_beta; a.ln_eps = ln_eps;
+  a.epi = epi; a.ln_gamma = ln_gamma; a.ln_beta = ln_beta; a.ln_eps = ln_eps; a.path = path;
   return launch_gemm(a, num_sms > 0 ? num_sms : sm_count(), (cudaStream_t)stream);
 }
 

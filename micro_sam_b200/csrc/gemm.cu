@@ -8,6 +8,7 @@
 //               through shared memory) -> fp32 / bf16 stores (a quad writes 16 or 32 contiguous bytes of a row).
 // One CTA per SM; tiles are distributed round-robin, N-block fastest so that the CTAs that run concurrently share the
 // same A row-block through L2.
+// gemm_wide_kernel (below) runs the large plain-epilogue products on 128 x 256 tiles with wgmma m64n256 per 64-row half.
 //
 // Replaces the nn.Linear / 1x1-conv / conv-transpose / patch-embed conv calls inside segment_anything's ImageEncoderViT /
 // MaskDecoder that micro_sam reaches through util.py:674 (image_encoder) and SamPredictor.predict_torch (inference.py:248,
@@ -71,6 +72,80 @@ __device__ __forceinline__ float apply_act(float x, int act) {
   if (act == 1) return gelu_erf(x);
   if (act == 2) return fmaxf(x, 0.0f);
   return x;
+}
+
+// Plain epilogue of the wide-tile kernel for one accumulator-fragment row of a thread: column pairs col0 + 8 j (+1),
+// j < 32, of `row` from fragment elements 4 j + 2 rs (+1).  Per element the arithmetic of gemm_bf16_kernel's plain epilogue in
+// the same order: bias, the activation (before the residual unless act_after_res), the fp32 or bf16 residual of
+// row % res_rows, the activation after it, the fp32 / bf16 store.  The pairs go in chunks of CH, and within a chunk each
+// step runs over all pairs, so the uniform branches on the epilogue flags are taken once per chunk, the pairs' chains are
+// independent instructions the scheduler can interleave, and the chunk's residual loads are in flight together.  A pair's
+// residual is read by the thread that writes it, before the write, so `out` may alias `residual` (the residual stream
+// updated in place).  N % 256 == 0 here, so every column of the tile is inside the output.
+template <int CH, int R>
+__device__ __forceinline__ void epi_wide_row(const float (&acc)[R], int rs, int row, int col0, const GemmParams& p) {
+  if (row >= p.M) return;
+  const float* res_f = nullptr;
+  const __nv_bfloat16* res_b = nullptr;
+  if (p.residual) {
+    const size_t off = (size_t)(row % p.res_rows) * p.ldr;
+    if (p.res_bf16) res_b = reinterpret_cast<const __nv_bfloat16*>(p.residual) + off;
+    else res_f = reinterpret_cast<const float*>(p.residual) + off;
+  }
+  const bool fast_gelu = !p.act_after_res && p.act == 1 && !p.out_fp32;  // bf16 output: the fast erf is exact to well below the output rounding
+  const int act_before = p.act_after_res ? 0 : p.act, act_after = p.act_after_res ? p.act : 0;
+#pragma unroll
+  for (int j0 = 0; j0 < R / 4; j0 += CH) {
+    float x[2 * CH];
+#pragma unroll
+    for (int c = 0; c < CH; ++c) { x[2 * c] = acc[4 * (j0 + c) + 2 * rs]; x[2 * c + 1] = acc[4 * (j0 + c) + 2 * rs + 1]; }
+    if (p.bias) {
+      float2 b[CH];
+#pragma unroll
+      for (int c = 0; c < CH; ++c) b[c] = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 8 * (j0 + c)));
+#pragma unroll
+      for (int c = 0; c < CH; ++c) { x[2 * c] += b[c].x; x[2 * c + 1] += b[c].y; }
+    }
+    if (fast_gelu) {
+#pragma unroll
+      for (int e = 0; e < 2 * CH; ++e) x[e] = gelu_fast(x[e]);
+    } else if (act_before == 1) {
+#pragma unroll
+      for (int e = 0; e < 2 * CH; ++e) x[e] = gelu_erf(x[e]);
+    } else if (act_before == 2) {
+#pragma unroll
+      for (int e = 0; e < 2 * CH; ++e) x[e] = fmaxf(x[e], 0.0f);
+    }
+    if (res_f) {
+      float2 r[CH];
+#pragma unroll
+      for (int c = 0; c < CH; ++c) r[c] = *reinterpret_cast<const float2*>(res_f + col0 + 8 * (j0 + c));
+#pragma unroll
+      for (int c = 0; c < CH; ++c) { x[2 * c] += r[c].x; x[2 * c + 1] += r[c].y; }
+    } else if (res_b) {
+      uint32_t r[CH];
+#pragma unroll
+      for (int c = 0; c < CH; ++c) r[c] = *reinterpret_cast<const uint32_t*>(res_b + col0 + 8 * (j0 + c));
+#pragma unroll
+      for (int c = 0; c < CH; ++c) { x[2 * c] += __uint_as_float(r[c] << 16); x[2 * c + 1] += __uint_as_float(r[c] & 0xffff0000u); }
+    }
+    if (act_after == 1) {
+#pragma unroll
+      for (int e = 0; e < 2 * CH; ++e) x[e] = gelu_erf(x[e]);
+    } else if (act_after == 2) {
+#pragma unroll
+      for (int e = 0; e < 2 * CH; ++e) x[e] = fmaxf(x[e], 0.0f);
+    }
+    if (p.out_fp32) {
+      float* o = reinterpret_cast<float*>(p.out) + (size_t)row * p.ldc + col0 + 8 * j0;
+#pragma unroll
+      for (int c = 0; c < CH; ++c) *reinterpret_cast<float2*>(o + 8 * c) = make_float2(x[2 * c], x[2 * c + 1]);
+    } else {
+      __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + (size_t)row * p.ldc + col0 + 8 * j0;
+#pragma unroll
+      for (int c = 0; c < CH; ++c) *reinterpret_cast<uint32_t*>(o + 8 * c) = pack_bf16(x[2 * c], x[2 * c + 1]);
+    }
+  }
 }
 
 template <int BN, int EPI>
@@ -296,19 +371,114 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
 }
 
-template <int BN, int EPI>
-static int launch_gemm_bn(const GemmArgs& a, int num_sms, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e =
-        cudaFuncSetAttribute(gemm_bf16_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
-    if (e != cudaSuccess) return set_error("gemm: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
-    attr_set = true;
+// ------------------------------------------------------------------------------------------------ wide tiles
+// gemm_wide_kernel: the large plain-epilogue products (N % 256 == 0, enough 128 x 256 tiles to fill the machine: every
+// linear layer of the ViT encoders).  Same operands, ring protocol and epilogue as gemm_bf16_kernel<256, EPI_PLAIN>, but
+// each of the two consumer warpgroups owns one 64-row half of the 128 x 256 tile and issues wgmma m64n256k16: it reads
+// only its own 8 KB of the A slot (the four n64 column groups above each read all 16 KB), and one instruction covers
+// the whole tile width.  Each accumulator element still sums the same k16 chunks in the same order.  The loading
+// warpgroup gives its registers to the consumers (setmaxnreg: 2 x 128 x 232 + 128 x 40), which hold 128 fp32
+// accumulators per thread.  What bounds both kernels at the encoder's shapes is the epilogue, not the MMAs (DESIGN.md §5):
+// with the epilogue compiled out both run at ~700 TFLOP/s.  So the wide kernel's epilogue (epi_wide_row) steps over 16
+// column pairs at a time instead of branching on the epilogue flags for every pair.
+constexpr int WIDE_BN = 256;
+constexpr int WIDE_STAGES = 4;
+constexpr int WIDE_EPI_CHUNK = 16;                             // epilogue column pairs per step (see epi_wide_row)
+constexpr int WIDE_A_BYTES = GEMM_BM * GEMM_BK * 2;             // 16 KB
+constexpr int WIDE_B_BYTES = WIDE_BN * GEMM_BK * 2;             // 32 KB
+constexpr int WIDE_STAGE_BYTES = WIDE_A_BYTES + WIDE_B_BYTES;
+constexpr int WIDE_THREADS = 3 * 128;                           // warp 0: TMA producer (warps 1-3 idle), then 2 consumers
+constexpr int WIDE_OFF_BAR = WIDE_STAGES * WIDE_STAGE_BYTES;    // 192 KB
+constexpr int WIDE_SMEM_BYTES = WIDE_OFF_BAR + 256 + 1024 /*align slack*/;
+
+__global__ void __launch_bounds__(WIDE_THREADS, 1)
+gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + WIDE_OFF_BAR);
+  uint64_t* empty_bar = full_bar + WIDE_STAGES;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int m_blocks = (p.M + GEMM_BM - 1) / GEMM_BM;
+  const int n_blocks = p.N / WIDE_BN;
+  const int k_blocks = (p.K + GEMM_BK - 1) / GEMM_BK;
+  const int num_tiles = m_blocks * n_blocks;
+
+  if (warp == 0 && lane == 0) {
+    prefetch_tmap(&tmA);
+    prefetch_tmap(&tmB);
+    for (int i = 0; i < WIDE_STAGES; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 8);  // one arrive per consumer warp: each warpgroup releases its half of the slot
+    }
+    fence_barrier_init();
   }
-  CUtensorMap tmA, tmB;
-  if (make_tmap_bf16_2d(&tmA, a.A, a.M, a.K, a.lda, GEMM_BM)) return -1;
-  if (make_tmap_bf16_2d(&tmB, a.W, a.N, a.K, a.ldw, BN)) return -1;
+  __syncthreads();
+  pdl_wait();      // the previous kernel's outputs (A, residual) are complete and visible from here on
+  pdl_trigger();
+
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    if (warp == 0 && lane == 0) {
+      // ---------------------------------------------------------- TMA producer: tiles round-robin, N-block fastest
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m_blk = tile / n_blocks, n_blk = tile % n_blocks;
+        for (int kb = 0; kb < k_blocks; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1, 1);
+          uint8_t* sa = smem + stage * WIDE_STAGE_BYTES;
+          mbar_expect_tx(&full_bar[stage], WIDE_STAGE_BYTES);
+          tma_load_2d(sa, &tmA, &full_bar[stage], kb * GEMM_BK, m_blk * GEMM_BM);
+          tma_load_2d(sa + WIDE_A_BYTES, &tmB, &full_bar[stage], kb * GEMM_BK, n_blk * WIDE_BN);
+          if (++stage == WIDE_STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+
+  // ------------------------------------------------------------ consumer warpgroup h: rows 64 h .. 64 h + 63 of the tile
+  const int h = (warp - 4) >> 2;
+  const int wq = warp & 3;             // warp inside the warpgroup: fragment rows 16 wq .. 16 wq + 15 of the half
+  const int qr = lane >> 2, qc = 2 * (lane & 3);
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int m_blk = tile / n_blocks, n_blk = tile % n_blocks;
+    float acc[128];
+    int prev = -1;
+    for (int kb = 0; kb < k_blocks; ++kb) {
+      mbar_wait(&full_bar[stage], phase, 3);
+      const uint32_t sa = smem_u32(smem + stage * WIDE_STAGE_BYTES);
+      const uint32_t sb = sa + WIDE_A_BYTES;
+      wg_fence();
+#pragma unroll
+      for (int k = 0; k < GEMM_BK / 16; ++k)   // +32 B per K=16 step inside the 128-B swizzle atom
+        wgmma<256>(acc, make_desc_sw128(sa + 8192 * h + 32 * k, 0, 1024), make_desc_sw128(sb + 32 * k, 0, 1024), (kb | k) != 0);
+      wg_commit();
+      wg_wait<1>();   // the MMAs of the previous k-block have read their slot
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
+      prev = stage;
+      if (++stage == WIDE_STAGES) { stage = 0; phase ^= 1; }
+    }
+    wg_wait<0>();
+    wg_fence_acc(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+
+    const int row0 = m_blk * GEMM_BM + 64 * h + 16 * wq + qr;
+#pragma unroll
+    for (int rs = 0; rs < 2; ++rs) epi_wide_row<WIDE_EPI_CHUNK>(acc, rs, row0 + 8 * rs, n_blk * WIDE_BN + qc, p);
+  }
+}
+
+static GemmParams gemm_params(const GemmArgs& a) {
   GemmParams p;
   p.M = a.M; p.N = a.N; p.K = a.K;
   p.bias = a.bias;
@@ -322,23 +492,71 @@ static int launch_gemm_bn(const GemmArgs& a, int num_sms, cudaStream_t stream) {
   p.act = a.act;
   p.act_after_res = a.act_after_res;
   p.ln_gamma = a.ln_gamma; p.ln_beta = a.ln_beta; p.ln_eps = a.ln_eps;
+  return p;
+}
+
+// algorithmic bytes of a launch: A, W, the output and the residual rows, each once
+static double gemm_bytes(const GemmArgs& a) {
+  const double out_b = (double)a.M * a.N * (a.out_fp32 ? 4 : 2);
+  const double res_b = a.residual ? (double)(a.res_rows > 0 ? a.res_rows : a.M) * a.N * (a.res_bf16 ? 2 : 4) : 0.0;
+  return (double)a.M * a.K * 2 + (double)a.N * a.K * 2 + out_b + res_b;
+}
+
+static int launch_gemm_wide(const GemmArgs& a, int num_sms, cudaStream_t stream) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(gemm_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WIDE_SMEM_BYTES);
+    if (e != cudaSuccess) return set_error("gemm: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
+    attr_set = true;
+  }
+  CUtensorMap tmA, tmB;
+  if (make_tmap_bf16_2d(&tmA, a.A, a.M, a.K, a.lda, GEMM_BM)) return -1;
+  if (make_tmap_bf16_2d(&tmB, a.W, a.N, a.K, a.ldw, WIDE_BN)) return -1;
+  const GemmParams p = gemm_params(a);
+  const int tiles = ((a.M + GEMM_BM - 1) / GEMM_BM) * (a.N / WIDE_BN);
+  const int grid = tiles < num_sms ? tiles : num_sms;
+  prof_begin(stream, a.K >= 512 ? "gemm_wide plain K>=512" : "gemm_wide plain K<512", 2.0 * a.M * a.N * a.K, gemm_bytes(a));
+  launch_pdl(gemm_wide_kernel, dim3(grid), dim3(WIDE_THREADS), WIDE_SMEM_BYTES, stream, tmA, tmB, p);
+  prof_end(stream);
+  LAUNCH_CHECK("gemm_wide");
+  return 0;
+}
+
+template <int BN, int EPI>
+static int launch_gemm_bn(const GemmArgs& a, int num_sms, cudaStream_t stream) {
+  using Cfg = GemmCfg<BN>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e =
+        cudaFuncSetAttribute(gemm_bf16_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+    if (e != cudaSuccess) return set_error("gemm: cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
+    attr_set = true;
+  }
+  CUtensorMap tmA, tmB;
+  if (make_tmap_bf16_2d(&tmA, a.A, a.M, a.K, a.lda, GEMM_BM)) return -1;
+  if (make_tmap_bf16_2d(&tmB, a.W, a.N, a.K, a.ldw, BN)) return -1;
+  const GemmParams p = gemm_params(a);
   const int tiles = ((a.M + GEMM_BM - 1) / GEMM_BM) * ((a.N + BN - 1) / BN);
   const int grid = tiles < num_sms ? tiles : num_sms;
-  {
-    const double out_b = (double)a.M * a.N * (a.out_fp32 ? 4 : 2);
-    const double res_b = a.residual ? (double)(a.res_rows > 0 ? a.res_rows : a.M) * a.N * (a.res_bf16 ? 2 : 4) : 0.0;
-    const char* nm = EPI == EPI_LN256 ? "gemm_bf16<256,ln256>"
-                     : (a.K >= 512 ? "gemm_bf16 plain K>=512" : "gemm_bf16 plain K<512");
-    prof_begin(stream, nm, 2.0 * a.M * a.N * a.K, (double)a.M * a.K * 2 + (double)a.N * a.K * 2 + out_b + res_b);
-  }
+  const char* nm = EPI == EPI_LN256 ? "gemm_bf16<256,ln256>" : (a.K >= 512 ? "gemm_bf16 plain K>=512" : "gemm_bf16 plain K<512");
+  prof_begin(stream, nm, 2.0 * a.M * a.N * a.K, gemm_bytes(a));
   launch_pdl(gemm_bf16_kernel<BN, EPI>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, stream, tmA, tmB, p);
   prof_end(stream);
   LAUNCH_CHECK("gemm");
   return 0;
 }
 
+static int device_sm_count() {
+  int dev = 0, n = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+  return n;
+}
+
 int launch_gemm(const GemmArgs& a, int num_sms, cudaStream_t stream) {
   if (a.M <= 0 || a.N <= 0 || a.K <= 0) return set_error("gemm: empty problem M=%d N=%d K=%d", a.M, a.N, a.K);
+  if (a.path < GEMM_PATH_AUTO || a.path > GEMM_PATH_WIDE) return set_error("gemm: unknown path %d", a.path);
+  if (a.path == GEMM_PATH_WIDE && a.epi != EPI_PLAIN) return set_error("gemm: the wide-tile kernel has the plain epilogue only");
   if (a.N % 32 != 0) return set_error("gemm: N=%d must be a multiple of 32", a.N);
   if (a.K % 8 != 0 || a.lda % 8 != 0 || a.ldw % 8 != 0)
     return set_error("gemm: K/lda/ldw must be multiples of 8 (16-byte TMA strides)");
@@ -350,6 +568,15 @@ int launch_gemm(const GemmArgs& a, int num_sms, cudaStream_t stream) {
   }
   if (a.epi != EPI_PLAIN) return set_error("gemm: unknown epilogue %d", a.epi);
   if ((a.ldc > 0 ? a.ldc : a.N) % 2 != 0) return set_error("gemm: ldc must be even");
+  if (a.path == GEMM_PATH_WIDE) {
+    if (a.N % 256 != 0) return set_error("gemm: the wide-tile kernel needs N %% 256 == 0 (N=%d)", a.N);
+    return launch_gemm_wide(a, num_sms, stream);
+  }
+  // The wide-tile kernel for products with enough 128 x 256 tiles to give every SM of the device one (the choice depends on
+  // the device, not on the num_sms cap, so that a capped grid computes what the full one does).
+  if (a.path == GEMM_PATH_AUTO && a.N % 256 == 0 &&
+      (long)((a.M + GEMM_BM - 1) / GEMM_BM) * (a.N / 256) >= device_sm_count())
+    return launch_gemm_wide(a, num_sms, stream);
   // BN=256 reads the A tile once per 256 output columns; fall back to 128 / 64 when N is not a multiple (or is small), to
   // avoid wasted columns.
   if (a.N % 256 == 0) return launch_gemm_bn<256, EPI_PLAIN>(a, num_sms, stream);

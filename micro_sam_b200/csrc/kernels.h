@@ -50,6 +50,12 @@ struct GemmArgs {
   const float* ln_gamma = nullptr;
   const float* ln_beta = nullptr;
   float ln_eps = 1e-5f;
+  int path = 0;  // GEMM_PATH_*: which kernel runs a plain-epilogue product
+};
+enum {
+  GEMM_PATH_AUTO = 0,   // the wide-tile kernel when N % 256 == 0 and the product has a 128 x 256 tile for every SM, else the tiled one
+  GEMM_PATH_TILED = 1,  // gemm_bf16_kernel<BN, EPI> (BN = 256 / 128 / 64)
+  GEMM_PATH_WIDE = 2,   // gemm_wide_kernel (needs N % 256 == 0 and the plain epilogue)
 };
 int launch_gemm(const GemmArgs& a, int num_sms, cudaStream_t stream);
 
