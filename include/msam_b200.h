@@ -434,6 +434,40 @@ int msam_stack_slice(const int32_t* src, int64_t n, int32_t* dst, int32_t* state
  * no positive weight is left.  labels int64 [n_nodes]: elf's multicut_decomposition numbering, clusters ordered by the smallest
  * node of their component of positive edges, then by their own smallest node, from 0. */
 int msam_multicut_gaec(int64_t n_nodes, int64_t n_edges, const int64_t* uv, const double* weights, int64_t* labels);
+/* ---- decoder-based automatic instance segmentation (AIS): UNETR decoder layers and generate() on the device ----
+ * Activations are bf16 NHWC, 16-byte aligned.  Convolution as an implicit GEMM on wgmma: sources x0 [B, H, W, C0] and
+ * x1 [B, H, W, C1] (C1 = 0: none) are read as their channel concatenation; w bf16 [N][ks * ks * (C0 + C1)] with K index
+ * (ky * 3 + kx) * (C0 + C1) + c; ks 3 (pad 1, zero padding) or 1; out = bias + conv, ReLU when relu.  transposed (ks = 1):
+ * the 2x2 / stride 2 transposed convolution, N = 4 Cout with row (i * 2 + j) * Cout + co of w, out [B, 2H, 2W, Cout].
+ * C0, C1 multiples of 64, Cout a multiple of 64.  stats (optional, msam_ais_conv_stats_size bytes): per image, 64 x 2-pixel
+ * tile (and 2x2 position when transposed) and channel, the sum and sum of squares of the stored outputs, for
+ * msam_op_ais_instnorm with nchunk = size / (16 B Cout). */
+int64_t msam_ais_conv_stats_size(int B, int H, int W, int Cout, int transposed);
+int msam_op_ais_conv(const void* x0, int C0, const void* x1, int C1, int B, int H, int W, int ks, const void* w_bf16,
+                     const float* bias, int Cout, int relu, int transposed, void* out, double* stats, void* stream);
+/* InstanceNorm2d (eps, biased variance per image and channel, optional affine gamma / beta) of x [B, HW, C] -> out (bf16);
+ * C % 8 == 0.  stats: the partial sums msam_op_ais_conv wrote for x (nchunk per image), or null: computed here.  The partial
+ * sums are reduced in a fixed order.  ws: msam_ais_instnorm_workspace bytes, 8-byte aligned. */
+int64_t msam_ais_instnorm_workspace(int B, int HW, int C);
+int msam_op_ais_instnorm(const void* x, int B, int HW, int C, const double* stats, int nchunk, const float* gamma,
+                         const float* beta, float eps, void* ws, int64_t ws_bytes, void* out, void* stream);
+/* bilinear x2 (align_corners=False) of [B, H, W, C] -> [B, 2H, 2W, C]; C % 8 == 0 */
+int msam_op_ais_upsample2(const void* x, int B, int H, int W, int C, void* out, void* stream);
+/* out_conv (1x1, C -> 3, w fp32 [3][C]) + sigmoid of [B, HW, C] -> fp32 [B, 3, HW]; C % 8 == 0, C <= 512 */
+int msam_op_ais_head(const void* x, int B, int HW, int C, const float* w, const float* bias, float* out, void* stream);
+/* fp32 planes [P, Hs, Ws] cropped to [ih, iw], then bilinear (align_corners=False) to [P, oh, ow] */
+int msam_op_ais_resize(const float* x, int P, int Hs, int Ws, int ih, int iw, int oh, int ow, float* out, void* stream);
+/* generate() of one image from fp32 maps fg / cd / bd [H, W]: separable gaussian smoothing in fp64 (taps [2r + 1] on the host,
+ * r = 0: none; taps_fg for fg, taps_d for both distances), fg = fg_s > t_fg, markers = cd_s < t_cd & bd_s < t_bd & fg, their
+ * 8-connected components numbered 1.. in raster order, the seeded watershed on bd_s inside fg (DESIGN.md section 2), then ids
+ * of fewer than min_size pixels removed and the rest renumbered.  labels int32 [H, W] (device); n_ids and sweeps (host): the
+ * number of ids and of watershed sweeps.  ws: msam_ais_postprocess_workspace bytes, 256-byte aligned.  Synchronises stream. */
+int64_t msam_ais_postprocess_workspace(int H, int W);
+int msam_ais_postprocess(const float* fg, const float* cd, const float* bd, int H, int W, const double* taps_fg, int r_fg,
+                         const double* taps_d, int r_d, float t_fg, float t_cd, float t_bd, int min_size, void* ws,
+                         int64_t ws_bytes, int32_t* labels, int* n_ids, int* sweeps, void* stream);
+/* per id 1..n_ids of labels [H, W]: props int32 [n_ids][5] = area, x0, y0, x1, y1 (inclusive) */
+int msam_ais_props(const int32_t* labels, int H, int W, int n_ids, int32_t* props, void* stream);
 /* debug: device buffer of 64 x 16 uint64 %globaltimer stamps written by the window-attention kernels, NULL = off */
 int msam_debug_attn_trace(void* dev_buf);
 

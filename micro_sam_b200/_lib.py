@@ -153,6 +153,23 @@ def lib() -> ctypes.CDLL:
         L.msam_merge3d_filter_z.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p]
         L.msam_stack_slice.argtypes = [c_void_p, c_int64, c_void_p, c_void_p, c_void_p]
         L.msam_multicut_gaec.argtypes = [c_int64, c_int64, c_void_p, c_void_p, c_void_p]
+        L.msam_ais_conv_stats_size.restype = c_int64
+        L.msam_ais_conv_stats_size.argtypes = [c_int, c_int, c_int, c_int, c_int]
+        L.msam_op_ais_conv.argtypes = [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
+                                       c_int, c_int, c_void_p, c_void_p, c_void_p]
+        L.msam_ais_instnorm_workspace.restype = c_int64
+        L.msam_ais_instnorm_workspace.argtypes = [c_int, c_int, c_int]
+        L.msam_op_ais_instnorm.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_float, c_void_p,
+                                           c_int64, c_void_p, c_void_p]
+        L.msam_op_ais_upsample2.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
+        L.msam_op_ais_head.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
+        L.msam_op_ais_resize.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
+        L.msam_ais_postprocess_workspace.restype = c_int64
+        L.msam_ais_postprocess_workspace.argtypes = [c_int, c_int]
+        L.msam_ais_postprocess.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_float,
+                                           c_float, c_float, c_int, c_void_p, c_int64, c_void_p, POINTER(c_int), POINTER(c_int),
+                                           c_void_p]
+        L.msam_ais_props.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]
         _lib = L
     return _lib
 

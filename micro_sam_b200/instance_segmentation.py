@@ -643,9 +643,143 @@ class TiledAutomaticMaskGenerator(AutomaticMaskGenerator):
         self._crop_boxes = crop_boxes
 
 
+# ------------------------------------------------------------------------------------------------ AIS (UNETR decoder)
+def get_decoder(image_encoder, decoder_state, device=None):
+    """get_decoder (instance_segmentation.py:808): the UNETR decoder of `decoder_state` on the device.  The image encoder is
+    the predictor's own (the decoder runs on its embeddings); it is accepted for the reference signature."""
+    from .unetr import UNETRDecoder
+    return UNETRDecoder(decoder_state, device=util.get_device(device))
+
+
+def get_predictor_and_decoder(model_type: str, checkpoint_path, device=None):
+    """get_predictor_and_decoder (instance_segmentation.py:829): predictor and AIS decoder from one checkpoint."""
+    device = util.get_device(device)
+    predictor, state = util.get_sam_model(model_type=model_type, checkpoint_path=checkpoint_path, device=device,
+                                          return_state=True)
+    if state is None or "decoder_state" not in state:
+        raise ValueError(f"The checkpoint at {checkpoint_path} does not contain a decoder state")
+    return predictor, get_decoder(None, state["decoder_state"], device)
+
+
+class InstanceSegmentationWithDecoder:
+    """InstanceSegmentationWithDecoder (instance_segmentation.py:955): initialize() runs the UNETR decoder on the image
+    embedding and keeps the foreground, center distance and boundary distance maps on the device; generate() runs the
+    smoothing, the seeded watershed and the size filter there too (DESIGN.md section 2 fixes their rules)."""
+
+    def __init__(self, predictor, decoder):
+        self._predictor = predictor
+        self._decoder = decoder
+        self._is_initialized = False
+
+    @property
+    def is_initialized(self):
+        return self._is_initialized
+
+    def initialize(self, image: np.ndarray, image_embeddings: Optional[util.ImageEmbeddings] = None, i: Optional[int] = None,
+                   verbose: bool = False, pbar_init=None, pbar_update=None, ndim: int = 2) -> None:
+        _, pbar_init, pbar_update, pbar_close = util.handle_pbar(verbose, pbar_init, pbar_update)
+        pbar_init(1, "Initialize instance segmentation with decoder")
+        if image_embeddings is None:
+            image_embeddings = util.precompute_image_embeddings(predictor=self._predictor, input_=image, ndim=ndim,
+                                                                verbose=verbose)
+        self._predictor = util.set_precomputed(self._predictor, image_embeddings, i=i)
+        emb = self._predictor.features
+        if emb.dim() == 3:
+            emb = emb[None]
+        maps = self._decoder(emb, tuple(self._predictor.input_size), tuple(self._predictor.original_size))[0]
+        pbar_update(1)
+        pbar_close()
+        self._foreground, self._center_distances, self._boundary_distances = maps[0], maps[1], maps[2]
+        self._i = i
+        self._is_initialized = True
+
+    def _to_masks(self, labels, n_ids, output_mode):
+        if output_mode != "binary_mask":
+            raise ValueError(f"Output mode {output_mode} is not supported. Choose one of 'instance_segmentation', 'binary_masks'")
+        from .unetr import region_props
+        props = region_props(labels, n_ids)
+        seg = labels.cpu().numpy()
+        H, W = seg.shape
+        return [{"segmentation": seg == k + 1, "area": int(p[0]), "bbox": [int(p[1]), int(p[3] - p[1] + 1), int(p[2]),
+                                                                          int(p[4] - p[2] + 1)],
+                 "crop_box": [0, W, 0, H], "seg_id": k + 1} for k, p in enumerate(props) if p[0] > 0]
+
+    def generate_device(self, center_distance_threshold: float = 0.5, boundary_distance_threshold: float = 0.5,
+                        foreground_threshold: float = 0.5, foreground_smoothing: float = 1.0, distance_smoothing: float = 1.6,
+                        min_size: int = 0):
+        """generate() without the host copy: (int32 device label image, number of ids, watershed sweeps)."""
+        if not self.is_initialized:
+            raise RuntimeError("InstanceSegmentationWithDecoder has not been initialized. Call initialize first.")
+        from .unetr import postprocess
+        return postprocess(self._foreground, self._center_distances, self._boundary_distances, center_distance_threshold,
+                           boundary_distance_threshold, foreground_threshold, foreground_smoothing, distance_smoothing, min_size)
+
+    def generate(self, center_distance_threshold: float = 0.5, boundary_distance_threshold: float = 0.5,
+                 foreground_threshold: float = 0.5, foreground_smoothing: float = 1.0, distance_smoothing: float = 1.6,
+                 min_size: int = 0, output_mode: str = "instance_segmentation", tile_shape=None, halo=None,
+                 n_threads: Optional[int] = None, optimize_memory: bool = False, segmentation=None):
+        """generate (instance_segmentation.py:1081): the uint32 label image, or the list of mask records with
+        output_mode="binary_mask".  `n_threads` and `segmentation` (the tiled path's output array) are accepted and unused, as
+        in the reference's untiled path."""
+        if not self.is_initialized:
+            raise RuntimeError("InstanceSegmentationWithDecoder has not been initialized. Call initialize first.")
+        if tile_shape is not None or halo is not None:
+            raise NotImplementedError("generate(tile_shape=..., halo=...): the blockwise watershed is not built on the GPU path")
+        if optimize_memory:
+            raise NotImplementedError("generate(optimize_memory=True) is not built on the GPU path")
+        if output_mode not in ("instance_segmentation", "binary_mask"):
+            raise ValueError(f"Output mode {output_mode} is not supported. Choose one of 'instance_segmentation', 'binary_masks'")
+        labels, n_ids, _ = self.generate_device(center_distance_threshold, boundary_distance_threshold, foreground_threshold,
+                                                foreground_smoothing, distance_smoothing, min_size)
+        if output_mode == "binary_mask":
+            return self._to_masks(labels, n_ids, output_mode)
+        return labels.cpu().numpy().view(np.uint32)
+
+    def get_state(self) -> Dict[str, Any]:
+        if not self.is_initialized:
+            raise RuntimeError("The state has not been computed yet. Call initialize first.")
+        return {"foreground": self._foreground.cpu().numpy(), "center_distances": self._center_distances.cpu().numpy(),
+                "boundary_distances": self._boundary_distances.cpu().numpy()}
+
+    def set_state(self, state: Dict[str, Any]) -> None:
+        dev = self._predictor.device
+        to = lambda a: (a if torch.is_tensor(a) else torch.from_numpy(np.asarray(a))).to(dev, torch.float32).contiguous()
+        self._foreground = to(state["foreground"])
+        self._center_distances = to(state["center_distances"])
+        self._boundary_distances = to(state["boundary_distances"])
+        self._is_initialized = True
+
+    def clear_state(self):
+        self._foreground = self._center_distances = self._boundary_distances = None
+        self._is_initialized = False
+
+
+class TiledInstanceSegmentationWithDecoder(InstanceSegmentationWithDecoder):
+    """TiledInstanceSegmentationWithDecoder (instance_segmentation.py:1208): not built on the GPU path."""
+
+    def __init__(self, *args, **kwargs):
+        raise NotImplementedError("TiledInstanceSegmentationWithDecoder (tiled AIS) is not built on the GPU path")
+
+
 def get_instance_segmentation_generator(predictor, is_tiled: bool, decoder=None, segmentation_mode: Optional[str] = None,
                                         **kwargs):
-    """instance_segmentation.py:1631: only the AMG mode exists on this path (AIS/APG need the UNETR decoder, 8f-2)."""
-    if decoder is not None or segmentation_mode not in (None, "amg"):
-        raise NotImplementedError("only segmentation_mode='amg' is available on the GPU path")
-    return (TiledAutomaticMaskGenerator if is_tiled else AutomaticMaskGenerator)(predictor, **kwargs)
+    """instance_segmentation.py:1631: "amg" (the default without a decoder) or "ais" (the default with one, untiled)."""
+    if segmentation_mode is None:
+        segmentation_mode = "amg" if decoder is None else DEFAULT_SEGMENTATION_MODE_WITH_DECODER
+    mode = segmentation_mode.lower()
+    if mode == "amg":
+        return (TiledAutomaticMaskGenerator if is_tiled else AutomaticMaskGenerator)(predictor, **kwargs)
+    if mode == "ais":
+        if decoder is None:
+            raise ValueError("segmentation_mode='ais' needs a decoder")
+        return (TiledInstanceSegmentationWithDecoder if is_tiled else InstanceSegmentationWithDecoder)(predictor, decoder, **kwargs)
+    if mode == "apg":
+        raise NotImplementedError("segmentation_mode='apg' (AutomaticPromptGenerator) is not built on the GPU path")
+    raise ValueError(f"Invalid segmentation_mode: {segmentation_mode}. Choose one of 'amg', 'ais', or 'apg'.")
+
+
+class AutomaticPromptGenerator:
+    """AutomaticPromptGenerator (APG, instance_segmentation.py:1380): not built on the GPU path."""
+
+    def __init__(self, *args, **kwargs):
+        raise NotImplementedError("AutomaticPromptGenerator (segmentation_mode='apg') is not built on the GPU path")
