@@ -288,6 +288,11 @@ int msam_decoder_zero_grads(msam_handle* h, void* stream);
  * second step without a new backward applies the same gradients again, as torch.optim.AdamW does.  The packed operands of the
  * INFERENCE decoder are refreshed by load_state_dict. */
 int msam_optimizer_step(msam_handle* h, float lr, float beta1, float beta2, float eps, float weight_decay, void* stream);
+/* The same AdamW update restricted to the tensors whose key starts with `prefix` (e.g. "image_encoder."): the step of an optimizer
+ * whose other parameters have no gradient, which torch skips.  After the first such call every tensor's bias correction uses its
+ * own number of updates, as torch.optim.AdamW's per-parameter step does; without it msam_optimizer_step is unchanged. */
+int msam_optimizer_step_prefix(msam_handle* h, const char* prefix, float lr, float beta1, float beta2, float eps, float weight_decay,
+                               void* stream);
 /* Enumeration of the trainable tensors (after the first training forward passes): key, DEVICE pointers of the fp32 gradient and master
  * buffers, element count -- to read gradients and weights, and so that a data-parallel driver can all-reduce (or clip) the gradients in
  * place before msam_optimizer_step.  Each tensor is an upstream one with its upstream element count.  The key is its upstream name,
@@ -468,6 +473,56 @@ int msam_ais_postprocess(const float* fg, const float* cd, const float* bd, int 
                          int64_t ws_bytes, int32_t* labels, int* n_ids, int* sweeps, void* stream);
 /* per id 1..n_ids of labels [H, W]: props int32 [n_ids][5] = area, x0, y0, x1, y1 (inclusive) */
 int msam_ais_props(const int32_t* labels, int H, int W, int n_ids, int32_t* props, void* stream);
+/* ---- training of the AIS decoder (csrc/ais_train.cu).  Every reduction runs in a fixed order: repeats are bit-identical. ----
+ * Weight gradient of msam_op_ais_conv (ks 3 or 1, not transposed): dw fp32 [Cout][ks * ks * (C0 + C1)] (the forward's layout) =
+ * sum over the pixels of dy [B, H, W, Cout] times the sources x0 / x1 shifted by the tap, zero outside the image.  ws:
+ * msam_ais_wgrad_workspace bytes (the split-K partials), 16-byte aligned.  The data gradient is msam_op_ais_conv on dy with the
+ * weights rotated by 180 degrees and the channel roles swapped. */
+int64_t msam_ais_wgrad_workspace(int Cout, int C0, int C1, int B, int H, int W, int ks);
+int msam_op_ais_wgrad(const void* dy, int Cout, const void* x0, int C0, const void* x1, int C1, int B, int H, int W, int ks, void* ws,
+                      int64_t ws_bytes, float* dw, void* stream);
+/* Training-mode norm of x [B, HW, C] bf16: per_image 1 = InstanceNorm, 0 = BatchNorm (batch statistics over B * HW, with
+ * run_mean / run_var updated as torch does: momentum, unbiased variance).  Writes mean and rstd ([B * C] or [C]) for the
+ * backward pass and out = (relu of) the normalised x.  ws: msam_ais_norm_workspace bytes, 256-byte aligned. */
+int64_t msam_ais_norm_workspace(int B, int HW, int C);
+int msam_op_ais_norm_forward(const void* x, int B, int HW, int C, int per_image, const float* gamma, const float* beta, float eps,
+                             int relu, float momentum, float* run_mean, float* run_var, void* ws, int64_t ws_bytes, float* mean,
+                             float* rstd, void* out, void* stream);
+/* Its backward pass: g = dy (bf16, or fp32 when dy_f32; row stride ldd) times [relu_out > 0] when relu_out is given;
+ * dx = gamma rstd (g - mean(g) - xhat mean(g xhat)), times [x > 0] when in_mask; out_mode 0: bf16 store, 1: fp32 store,
+ * 2: fp32 add, row stride ldo.  dgamma / dbeta (optional): sum g xhat, sum g per channel. */
+int msam_op_ais_norm_backward(const void* x, int ldx, const void* dy, int dy_f32, int ldd, const void* relu_out, int B, int HW, int C,
+                              int per_image, const float* gamma, const float* mean, const float* rstd, int in_mask, void* ws,
+                              int64_t ws_bytes, void* dx, int out_mode, int ldo, float* dgamma, float* dbeta, void* stream);
+/* out[c] = sum over the B * HW pixels of g [B, HW, C] bf16 (a bias gradient); ws: msam_ais_norm_workspace bytes */
+int msam_op_ais_chan_sum(const void* g, int B, int HW, int C, void* ws, int64_t ws_bytes, float* out, void* stream);
+/* adjoint of msam_op_ais_upsample2: dy [B, 2H, 2W, C] -> dx [B, H, W, C], bf16 */
+int msam_op_ais_upsample2_backward(const void* dy, int B, int H, int W, int C, void* dx, void* stream);
+/* out[b, y, x, (i * 2 + j) * C + c] = dy[b, 2y + i, 2x + j, c] (bf16): the transposed convolution's output as GEMM columns */
+int msam_op_ais_space_to_depth(const void* dy, int B, int H, int W, int C, void* out, void* stream);
+/* acc[i] (fp32) += x[i] (bf16) */
+int msam_op_ais_add_bf16(float* acc, const void* x, int64_t n, void* stream);
+/* g[i] (bf16) = 0 where out[i] <= 0: the ReLU mask of the layer that wrote out */
+int msam_op_ais_relu_mask(void* g, const void* out, int64_t n, void* stream);
+/* backward of msam_op_ais_head from its input h, weights w and sigmoid maps: dh (bf16, times [h > 0]: the ReLU before the head),
+ * dw fp32 [3][C], db [3].  ws: msam_ais_head_backward_workspace bytes, 256-byte aligned. */
+int64_t msam_ais_head_backward_workspace(int B, int HW, int C);
+int msam_op_ais_head_backward(const void* h, int B, int HW, int C, const float* w, const float* maps, const float* dmaps, void* ws,
+                              int64_t ws_bytes, void* dh, float* dw, float* db, void* stream);
+/* adjoint of msam_op_ais_resize: dout [P, oh, ow] -> dsrc [P, Hs, Ws] (zero outside the crop); tmp: P * oh * iw floats */
+int msam_op_ais_resize_backward(const float* dout, int P, int Hs, int Ws, int ih, int iw, int oh, int ow, float* tmp, float* dsrc,
+                                void* stream);
+/* Distance-based Dice loss sums of prediction x and target y (fp32 [B, 3, HW]); mask: channels 1, 2 of both times y[:, 0].
+ * stats (device, fp64 [3][3]): per channel sum x y, sum x^2, sum y^2 over the batch.  The backward pass takes
+ * coef (device, fp32 [3][2]) = dL / d(sum x y), dL / d(sum x^2) per channel and writes dx. */
+int64_t msam_ais_dist_loss_workspace(int B, int HW);
+int msam_op_ais_dist_loss_stats(const float* x, const float* y, int B, int HW, int mask, void* ws, int64_t ws_bytes, double* stats,
+                                void* stream);
+int msam_op_ais_dist_loss_backward(const float* x, const float* y, int B, int HW, int mask, const float* coef, float* dx, void* stream);
+/* One AdamW step (torch.optim.AdamW) of fp32 masters w with gradients g and moments m, v at bias-correction step `step` (>= 1),
+ * for tensors kept outside the engine's table. */
+int msam_op_adamw(float* w, const float* g, float* m, float* v, int64_t n, float lr, float beta1, float beta2, float eps,
+                  float weight_decay, int step, void* stream);
 /* debug: device buffer of 64 x 16 uint64 %globaltimer stamps written by the window-attention kernels, NULL = off */
 int msam_debug_attn_trace(void* dev_buf);
 

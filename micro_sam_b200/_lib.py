@@ -122,6 +122,7 @@ def lib() -> ctypes.CDLL:
         L.msam_decoder_train_backward.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
         L.msam_decoder_zero_grads.argtypes = [c_void_p, c_void_p]
         L.msam_optimizer_step.argtypes = [c_void_p, c_float, c_float, c_float, c_float, c_float, c_void_p]
+        L.msam_optimizer_step_prefix.argtypes = [c_void_p, c_char_p, c_float, c_float, c_float, c_float, c_float, c_void_p]
         L.msam_train_tensor_count.argtypes = [c_void_p]
         L.msam_train_tensor_info.argtypes = [c_void_p, c_int, ctypes.c_char_p, c_int, POINTER(c_void_p), POINTER(c_void_p), POINTER(c_int64)]
         L.msam_mask_loss_backward.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
@@ -170,6 +171,34 @@ def lib() -> ctypes.CDLL:
                                            c_float, c_float, c_int, c_void_p, c_int64, c_void_p, POINTER(c_int), POINTER(c_int),
                                            c_void_p]
         L.msam_ais_props.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]
+        L.msam_ais_wgrad_workspace.restype = c_int64
+        L.msam_ais_wgrad_workspace.argtypes = [c_int, c_int, c_int, c_int, c_int, c_int, c_int]
+        L.msam_op_ais_wgrad.argtypes = [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                        c_int64, c_void_p, c_void_p]
+        L.msam_ais_norm_workspace.restype = c_int64
+        L.msam_ais_norm_workspace.argtypes = [c_int, c_int, c_int]
+        L.msam_op_ais_norm_forward.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_float,
+                                               c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]
+        L.msam_op_ais_norm_backward.argtypes = [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int,
+                                                c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int64, c_void_p, c_int, c_int,
+                                                c_void_p, c_void_p, c_void_p]
+        L.msam_op_ais_chan_sum.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p]
+        L.msam_op_ais_upsample2_backward.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
+        L.msam_op_ais_space_to_depth.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
+        L.msam_op_ais_relu_mask.argtypes = [c_void_p, c_void_p, c_int64, c_void_p]
+        L.msam_op_ais_add_bf16.argtypes = [c_void_p, c_void_p, c_int64, c_void_p]
+        L.msam_ais_head_backward_workspace.restype = c_int64
+        L.msam_ais_head_backward_workspace.argtypes = [c_int, c_int, c_int]
+        L.msam_op_ais_head_backward.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
+                                                c_void_p, c_void_p, c_void_p, c_void_p]
+        L.msam_op_ais_resize_backward.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                                  c_void_p]
+        L.msam_ais_dist_loss_workspace.restype = c_int64
+        L.msam_ais_dist_loss_workspace.argtypes = [c_int, c_int]
+        L.msam_op_ais_dist_loss_stats.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p]
+        L.msam_op_ais_dist_loss_backward.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]
+        L.msam_op_adamw.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_float, c_float, c_float, c_float, c_float,
+                                    c_int, c_void_p]
         _lib = L
     return _lib
 

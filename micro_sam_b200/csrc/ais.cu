@@ -56,14 +56,6 @@ struct ConvParams {
   double* stats;         // null, or [B][(N / Cout) * tiles][Cout][2]: sum and sum of squares of the stored bf16 outputs
 };
 
-__device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(
-          smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-
 template <int BN>
 __global__ void __launch_bounds__(ConvCfg<BN>::THREADS, 1)
 ais_conv_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
@@ -212,21 +204,6 @@ ais_conv_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__
   }
 }
 
-// 4-D map (C, W, H, B) of a bf16 NHWC tensor, box {64 ch, 64 x, 2 y, 1}, SWIZZLE_128B, out-of-bounds elements zero
-int make_tmap_nhwc(CUtensorMap* m, const void* x, int B, int H, int W, int C) {
-  PFN_encodeTiled enc = get_encode_tiled();
-  if (!enc) return set_error("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-  cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  cuuint32_t box[4] = {CV_BK, CV_TX, CV_TY, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return set_error("ais conv: cuTensorMapEncodeTiled failed (%d) for [%d, %d, %d, %d]", (int)r, B, H, W, C);
-  return 0;
-}
-
 // ------------------------------------------------------------------------------------------------ InstanceNorm2d
 constexpr int IN_CHUNK = 1024;   // pixels per partial sum
 
@@ -295,14 +272,6 @@ __global__ void ais_in_apply_kernel(const __nv_bfloat16* __restrict__ x, int HW,
 }
 
 // ------------------------------------------------------------------------------------------------ bilinear x2, head, resize
-// PyTorch's upsample_bilinear2d source index (align_corners=False): max(0, (dst + 0.5) * scale - 0.5)
-__device__ __forceinline__ void lin_src(int d, float scale, int n, int& i0, int& i1, float& l1) {
-  const float s = fmaxf((d + 0.5f) * scale - 0.5f, 0.f);
-  i0 = (int)s;
-  i1 = i0 + (i0 < n - 1 ? 1 : 0);
-  l1 = s - (float)i0;
-}
-
 __global__ void ais_up2_kernel(const __nv_bfloat16* __restrict__ x, int B, int H, int W, int C, __nv_bfloat16* __restrict__ out) {
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   const int C8 = C / 8;
@@ -682,6 +651,21 @@ size_t post_ws(int H, int W, char* base, PostWs* w) {
 }
 
 }  // namespace
+
+// 4-D map (C, W, H, B) of a bf16 NHWC tensor, box {64 ch, 64 x, 2 y, 1}, SWIZZLE_128B, out-of-bounds elements zero
+int make_tmap_nhwc(CUtensorMap* m, const void* x, int B, int H, int W, int C) {
+  PFN_encodeTiled enc = get_encode_tiled();
+  if (!enc) return set_error("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
+  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+  cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+  cuuint32_t box[4] = {CV_BK, CV_TX, CV_TY, 1};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x), dims, strides, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return set_error("ais conv: cuTensorMapEncodeTiled failed (%d) for [%d, %d, %d, %d]", (int)r, B, H, W, C);
+  return 0;
+}
 
 template <int BN>
 int launch_conv_bn(const CUtensorMap& t0, const CUtensorMap& t1, const CUtensorMap& tw, const ConvParams& p, int B,

@@ -26,14 +26,6 @@ constexpr int SMEM_BYTES = OFF_BAR + 128 + 1024;
 constexpr int THREADS = 256;
 }  // namespace bg
 
-__device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(
-          smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-
 struct BgParams {
   float* out;             // fp32 [outer, heads, M, ldc]
   long o_wstride, o_hstride;

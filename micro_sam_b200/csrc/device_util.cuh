@@ -46,4 +46,12 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return y;
 }
 
+// PyTorch's upsample_bilinear2d source index (align_corners=False): max(0, (dst + 0.5) * scale - 0.5)
+__device__ __forceinline__ void lin_src(int d, float scale, int n, int& i0, int& i1, float& l1) {
+  const float s = fmaxf((d + 0.5f) * scale - 0.5f, 0.f);
+  i0 = (int)s;
+  i1 = i0 + (i0 < n - 1 ? 1 : 0);
+  l1 = s - (float)i0;
+}
+
 }  // namespace msam

@@ -896,6 +896,11 @@ int msam_optimizer_step(msam_handle* h, float lr, float beta1, float beta2, floa
   if (!h) return set_error("msam_optimizer_step: null handle");
   return h->eng.optimizer_step(lr, beta1, beta2, eps, weight_decay, (cudaStream_t)stream);
 }
+int msam_optimizer_step_prefix(msam_handle* h, const char* prefix, float lr, float beta1, float beta2, float eps, float weight_decay,
+                               void* stream) {
+  if (!h || !prefix || !*prefix) return set_error("msam_optimizer_step_prefix: null handle or empty prefix");
+  return h->eng.optimizer_step(lr, beta1, beta2, eps, weight_decay, (cudaStream_t)stream, prefix);
+}
 int msam_train_tensor_count(msam_handle* h) { return h ? (int)h->eng.opt.size() : -1; }
 int msam_train_tensor_info(msam_handle* h, int i, char* key_buf, int cap, void** grad, void** master, int64_t* n) {
   if (!h || i < 0 || i >= (int)h->eng.opt.size() || !key_buf || cap < 2) return set_error("msam_train_tensor_info: bad argument");

@@ -95,6 +95,7 @@ struct OptParam {
   bool decoder = false;           // the gradient accumulates until msam_decoder_zero_grads; else msam_encode_backward overwrites it
   const bool* written = nullptr;  // non-null: AdamW skips the tensor while *written is false (no gradient since the last zeroing)
   int64_t steps = 0;              // ... and counts its own steps for the bias correction (with written only)
+  int64_t count = 0;              // updates of the tensor; the bias correction once a subset step has run (per_tensor_counts)
   Refresh refresh = Refresh::None;
   __nv_bfloat16 *dst = nullptr;
   __nv_bfloat16* dstT = nullptr;  // non-null: after the refresh, dstT [cols, rows] = dst [rows, cols]^T (W^T of the dgrad GEMMs)
@@ -125,6 +126,7 @@ struct Engine {
   std::unordered_map<std::string, HostTensor> dec_host;   // host fp32 copies of every weight, kept for the training paths (masters, decoder_train.cu operands)
   std::vector<OptParam> opt;
   int64_t opt_step_count = 0;
+  bool per_tensor_counts = false;  // set by the first subset step: from then on each tensor's bias correction uses its own count
 
   void* dalloc(size_t bytes, bool zero = false);
   const std::vector<float>* host(const std::string& name, std::initializer_list<int64_t> shape);
@@ -170,7 +172,8 @@ struct Engine {
   // train_add returns the gradient buffer of p, or null on error.  p.g null: a zeroed buffer of p.n floats is allocated.
   // p.w null: the master is an fp32 upload of p.n floats from `init`, or from the host copy dec_host[p.key] when init is null.
   float* train_add(OptParam p, const float* init = nullptr);
-  int optimizer_step(float lr, float beta1, float beta2, float eps, float weight_decay, cudaStream_t st);
+  // prefix non-null: only the tensors whose key starts with it (a subset step: torch skips the parameters without a gradient)
+  int optimizer_step(float lr, float beta1, float beta2, float eps, float weight_decay, cudaStream_t st, const char* prefix = nullptr);
   int set_image_embedding(const float* feat, cudaStream_t st);  // decoder.cu
   int decode(const float* points, const float* labels, int np, const float* boxes, const float* mask_in, int P, int multimask,
              float* low_res, float* iou, cudaStream_t st);  // decoder.cu

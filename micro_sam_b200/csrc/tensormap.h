@@ -21,4 +21,8 @@ int make_tmap_2d(CUtensorMap* out, const void* gptr, int elem_bytes, uint64_t ro
 // fp16 variant of make_tmap_bf16_2d
 int make_tmap_f16_2d(CUtensorMap* out, const void* gptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows);
 
+// bf16 NHWC tensor [B, H, W, C] as a 4-D map (C, W, H, B), box {64 ch, 64 x, 2 y, 1 image}, SWIZZLE_128B, out-of-bounds
+// elements zero (ais.cu)
+int make_tmap_nhwc(CUtensorMap* m, const void* x, int B, int H, int W, int C);
+
 }  // namespace msam

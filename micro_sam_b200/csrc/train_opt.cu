@@ -5,6 +5,7 @@
 #include "engine.h"
 
 #include <cmath>
+#include <cstring>
 
 namespace msam {
 
@@ -56,16 +57,23 @@ float* Engine::train_add(OptParam p, const float* init) {
   return p.g;
 }
 
-int Engine::optimizer_step(float lr, float b1, float b2, float eps, float wd, cudaStream_t st) {
+int Engine::optimizer_step(float lr, float b1, float b2, float eps, float wd, cudaStream_t st, const char* prefix) {
   if (opt.empty()) return set_error("msam_optimizer_step: no trainable tensors registered (run a training forward / backward first)");
-  ++opt_step_count;
+  if (prefix) per_tensor_counts = true;
+  else ++opt_step_count;
   const float c1 = 1.f - powf(b1, (float)opt_step_count), c2 = 1.f - powf(b2, (float)opt_step_count);
+  const size_t plen = prefix ? strlen(prefix) : 0;
   for (OptParam& p : opt) {
+    if (prefix && p.key.compare(0, plen, prefix) != 0) continue;
     float c1p = c1, c2p = c2;
     if (p.written) {
       if (!*p.written) continue;
       ++p.steps;
       c1p = 1.f - powf(b1, (float)p.steps); c2p = 1.f - powf(b2, (float)p.steps);
+    }
+    ++p.count;
+    if (per_tensor_counts) {   // torch.optim.AdamW: a parameter's step counts only the steps that updated it
+      c1p = 1.f - powf(b1, (float)p.count); c2p = 1.f - powf(b2, (float)p.count);
     }
     if (!p.m) {
       p.m = (float*)dalloc((size_t)p.n * 4, true);
@@ -97,3 +105,14 @@ int Engine::optimizer_step(float lr, float b1, float b2, float eps, float wd, cu
 }
 
 }  // namespace msam
+
+extern "C" int msam_op_adamw(float* w, const float* g, float* m, float* v, int64_t n, float lr, float beta1, float beta2, float eps,
+                             float weight_decay, int step, void* stream) {
+  using namespace msam;
+  if (!w || !g || !m || !v) return set_error("msam_op_adamw: null argument");
+  if (n <= 0 || step <= 0) return set_error("msam_op_adamw: %lld elements, step %d", (long long)n, step);
+  const float c1 = 1.f - powf(beta1, (float)step), c2 = 1.f - powf(beta2, (float)step);
+  adamw_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(w, g, m, v, n, lr, beta1, beta2, eps, weight_decay, c1, c2);
+  LAUNCH_CHECK("adamw");
+  return 0;
+}

@@ -472,6 +472,14 @@ class B200Sam:
         from .distributed import allreduce_average_
         return allreduce_average_([v for _, v in self.grad_views()])
 
+    def optimizer_step_prefix(self, prefix: str, lr: float = 1e-5, betas=(0.9, 0.999), eps: float = 1e-8,
+                              weight_decay: float = 0.01) -> None:
+        """`optimizer_step` over the tensors whose upstream key starts with `prefix` only (msam_optimizer_step_prefix): the step
+        of a torch optimizer in which the other parameters have no gradient.  From then on every tensor's bias correction counts
+        its own updates, as torch.optim.AdamW does."""
+        _lib.check(_lib.lib().msam_optimizer_step_prefix(self._h, prefix.encode(), lr, betas[0], betas[1], eps, weight_decay,
+                                                         _lib.cur_stream()))
+
     def optimizer_step(self, lr: float = 1e-5, betas=(0.9, 0.999), eps: float = 1e-8, weight_decay: float = 0.01) -> None:
         """One AdamW update (torch.optim.AdamW semantics, the reference trainer's default) of every tensor that has gradients, on the
         device (csrc/train_opt.cu): fp32 master weights + moments, then the operands of the training paths are refreshed.  The fused

@@ -464,3 +464,216 @@ def interactive_train_iteration(model: TrainableSAM, x, y, iteration: int, n_obj
     loss, mask_loss, iou_loss, model_iou = compute_iterative_loss(model, batched_inputs, y_one_hot, n_sub_iteration, multimask_output,
                                                                   update, full_masks=False)
     return loss, mask_loss, iou_loss, model_iou, y_one_hot
+
+
+# ---------------------------------------------------------------------------------------------------------------------------------
+# Instance-segmentation (UNETR decoder) training: micro_sam/training/training.py:train_instance_segmentation with the image encoder
+# frozen, JointSamTrainer._instance_iteration (joint_sam_trainer.py:73-131) and export_instance_segmentation_model (training.py:378)
+
+class _UNETRDecoderFn(torch.autograd.Function):
+    """TrainableUNETRDecoder.forward, then crop + resize to the original size (postprocess_masks); backward fills the decoder's
+    gradients and returns d embedding."""
+
+    @staticmethod
+    def forward(ctx, emb, anchor, dec, input_size, original_size):
+        from .unetr import resize_maps
+        maps = dec.forward(emb)
+        ctx.dec, ctx.geom = dec, (tuple(maps.shape), tuple(input_size), tuple(original_size))
+        if tuple(maps.shape[-2:]) == tuple(original_size) and tuple(input_size) == tuple(original_size):
+            return maps
+        return resize_maps(maps, input_size, original_size)
+
+    @staticmethod
+    def backward(ctx, d_out):
+        (B, P, Hs, Ws), (ih, iw), (oh, ow) = ctx.geom
+        d = d_out.to(torch.float32).contiguous()
+        if (Hs, Ws) != (oh, ow) or (ih, iw) != (oh, ow):
+            tmp = torch.empty(B * P * oh * iw, device=d.device, dtype=torch.float32)
+            dm = torch.empty(B, P, Hs, Ws, device=d.device, dtype=torch.float32)
+            _lib.check(_lib.lib().msam_op_ais_resize_backward(_lib.ptr(d), B * P, Hs, Ws, ih, iw, oh, ow, _lib.ptr(tmp), _lib.ptr(dm),
+                                                              _lib.cur_stream()))
+            d = dm
+        return ctx.dec.backward(d), torch.zeros((), device=d.device), None, None, None
+
+
+class UNETR:
+    """micro-sam's get_unetr model (torch_em UNETR with use_skip_connection=False, resize_input=True, Sigmoid) on the device:
+    `__call__(x)` takes images (B, 3, H, W) in [0, 255] and returns the foreground / center distance / boundary distance maps
+    (B, 3, H, W).  preprocess (TrainableSAM.preprocess) -> image encoder (frozen) -> decoder -> crop and resize back; the result
+    is differentiable with respect to the decoder's parameters."""
+
+    def __init__(self, sam: B200Sam, decoder):
+        self.sam = sam
+        self.decoder = decoder
+        self._trainable = TrainableSAM(sam)
+        self._anchor = torch.zeros((), device=decoder.device, requires_grad=True)
+
+    def embed(self, x: torch.Tensor, train_encoder: bool = False):
+        """(embeddings (B, 256, 64, 64), input_size).  With `train_encoder` (and grad mode) the embeddings come from the encoder's
+        training forward (`_EncoderFn`) and are part of the autograd graph: a backward pass fills the encoder's gradients.
+        Otherwise the frozen encoder runs in eval mode without a graph."""
+        with torch.no_grad():
+            images, input_size = self._trainable.preprocess(x)
+        was = self.sam.training
+        if train_encoder and torch.is_grad_enabled():
+            self.sam.train()
+            try:
+                return self.sam.image_encoder(images), input_size
+            finally:
+                if not was:
+                    self.sam.eval()
+        with torch.no_grad():
+            self.sam.eval()
+            try:
+                emb = self.sam.image_encoder(images)
+            finally:
+                if was:
+                    self.sam.train()
+        return emb, input_size
+
+    def __call__(self, x: torch.Tensor) -> torch.Tensor:
+        """preprocess -> image encoder -> decoder -> crop and resize back.  In train() mode of the SAM model and grad mode the
+        encoder runs its training forward, so the result is differentiable w.r.t. the encoder and the decoder."""
+        emb, input_size = self.embed(x, train_encoder=bool(self.sam.training))
+        return self.decode(emb, input_size, tuple(x.shape[-2:]))
+
+    def decode(self, emb: torch.Tensor, input_size, original_size) -> torch.Tensor:
+        if torch.is_grad_enabled():
+            return _UNETRDecoderFn.apply(emb, self._anchor, self.decoder, tuple(input_size), tuple(original_size))
+        with torch.no_grad():
+            return _UNETRDecoderFn.forward(_Ctx(), emb, None, self.decoder, tuple(input_size), tuple(original_size))
+
+    def decoder_grads(self) -> Dict[str, torch.Tensor]:
+        return dict(self.decoder.grads)
+
+    def optimizer_step(self, lr: float = 1e-5, betas=(0.9, 0.999), eps: float = 1e-8, weight_decay: float = 0.01) -> None:
+        self.decoder.optimizer_step(lr, betas, eps, weight_decay)
+
+    def decoder_state_dict(self) -> Dict[str, torch.Tensor]:
+        return self.decoder.state_dict()
+
+
+class _Ctx:
+    pass
+
+
+def _sam_of(image_encoder) -> B200Sam:
+    for cand in (image_encoder, getattr(image_encoder, "_sam", None), getattr(image_encoder, "model", None)):
+        if isinstance(cand, B200Sam):
+            return cand
+    raise TypeError("get_unetr takes a B200Sam, its image_encoder or a predictor built on one")
+
+
+def get_unetr(image_encoder, decoder_state=None, device=None, out_channels: int = 3, flexible_load_checkpoint: bool = False,
+              final_activation: str = "Sigmoid") -> UNETR:
+    """get_unetr (instance_segmentation.py:765): a trainable UNETR on `image_encoder`'s model.  Without `decoder_state` the
+    decoder is the production plan with the bilinear upsampler, freshly initialised (`unetr.default_decoder_state`, seed 0)."""
+    from .unetr import TrainableUNETRDecoder, default_decoder_state
+    if out_channels != 3:
+        raise NotImplementedError(f"out_channels={out_channels}: the decoder head has 3 output channels")
+    if final_activation != "Sigmoid":
+        raise NotImplementedError(f"final_activation={final_activation!r}: only 'Sigmoid' is implemented")
+    if flexible_load_checkpoint:
+        raise NotImplementedError("flexible_load_checkpoint=True is not implemented")
+    sam = _sam_of(image_encoder)
+    if sam.image_size != 1024:
+        raise NotImplementedError(f"image_size {sam.image_size}: the UNETR decoder is built for 1024")
+    state = default_decoder_state() if decoder_state is None else decoder_state
+    return UNETR(sam, TrainableUNETRDecoder(state, device=device if device is not None else sam.device))
+
+
+class _DistLossStatsFn(torch.autograd.Function):
+    """msam_op_ais_dist_loss_stats with its adjoint: per channel (sum x y, sum x^2, sum y^2), fp64 [3, 3]"""
+
+    @staticmethod
+    def forward(ctx, x, y, mask):
+        B, _, H, W = x.shape
+        L = _lib.lib()
+        ws = torch.empty(int(L.msam_ais_dist_loss_workspace(B, H * W)), device=x.device, dtype=torch.uint8)
+        st = torch.empty(3, 3, device=x.device, dtype=torch.float64)
+        _lib.check(L.msam_op_ais_dist_loss_stats(_lib.ptr(x), _lib.ptr(y), B, H * W, int(mask), _lib.ptr(ws), ws.numel(), _lib.ptr(st),
+                                                 _lib.cur_stream()))
+        ctx.save_for_backward(x, y)
+        ctx.mask = mask
+        return st
+
+    @staticmethod
+    def backward(ctx, d_st):
+        x, y = ctx.saved_tensors
+        B, _, H, W = x.shape
+        coef = d_st[:, :2].to(torch.float32).contiguous()
+        dx = torch.empty_like(x)
+        _lib.check(_lib.lib().msam_op_ais_dist_loss_backward(_lib.ptr(x), _lib.ptr(y), B, H * W, int(ctx.mask), _lib.ptr(coef),
+                                                             _lib.ptr(dx), _lib.cur_stream()))
+        return dx, None, None
+
+
+def dice_from_stats(st: torch.Tensor, eps: float = 1e-7) -> torch.Tensor:
+    """sum over the channels of 1 - 2 sum(x y) / max(sum x^2 + sum y^2, eps) (compute_loss's Dice convention)"""
+    return (1.0 - 2.0 * st[:, 0] / (st[:, 1] + st[:, 2]).clamp(min=eps)).sum()
+
+
+class DiceBasedDistanceLoss:
+    """torch_em's DiceBasedDistanceLoss as DESIGN.md section 2 restates it (unpinned): prediction and target (B, 3, H, W) =
+    foreground, center distances, boundary distances; the loss is the Dice loss of each channel, each reduced over the whole
+    batch, summed.  With `mask_distances_in_bg` the two distance channels of both are multiplied by the foreground target."""
+
+    def __init__(self, mask_distances_in_bg: bool = True):
+        self.mask_distances_in_bg = mask_distances_in_bg
+
+    def __call__(self, input_: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
+        if input_.shape != target.shape or input_.dim() != 4 or input_.shape[1] != 3:
+            raise ValueError(f"DiceBasedDistanceLoss takes (B, 3, H, W) prediction and target, got {tuple(input_.shape)} and "
+                             f"{tuple(target.shape)}")
+        x = input_.to(torch.float32).contiguous()
+        y = target.to(x.device, torch.float32).contiguous()
+        return dice_from_stats(_DistLossStatsFn.apply(x, y, self.mask_distances_in_bg)).to(torch.float32)
+
+
+def instance_train_iteration(unetr: UNETR, x, y, freeze_encoder: bool = True, loss=None, lr: float = 1e-5, betas=(0.9, 0.999),
+                             eps: float = 1e-8, weight_decay: float = 0.01) -> torch.Tensor:
+    """JointSamTrainer._instance_iteration (joint_sam_trainer.py:73-89) + its backward and AdamW step: x images (B, 3, H, W) in
+    [0, 255], y targets (B, 3, H, W) (foreground, center and boundary distances).  Returns the loss (detached).
+    `freeze_encoder=True` is train_instance_segmentation(freeze=["image_encoder"]): no encoder backward, the encoder untouched.
+    Otherwise the loss is back-propagated through the encoder too and the step updates the encoder's tensors and the decoder's;
+    the optimizer's other parameters (prompt encoder, mask decoder) have no gradient in this step and are skipped, as
+    torch.optim.AdamW skips them after zero_grad()."""
+    loss_fn = DiceBasedDistanceLoss() if loss is None else loss
+    emb, input_size = unetr.embed(x, train_encoder=not freeze_encoder)
+    pred = unetr.decode(emb, input_size, tuple(x.shape[-2:]))
+    value = loss_fn(pred, y.to(pred.device))
+    value.backward()
+    if not freeze_encoder:
+        unetr.sam.optimizer_step_prefix("image_encoder.", lr, betas, eps, weight_decay)
+    unetr.optimizer_step(lr, betas, eps, weight_decay)
+    return value.detach()
+
+
+def joint_train_iteration(model: TrainableSAM, unetr: UNETR, x, y, y_instance, iteration: int, n_objects_per_batch: int = 25,
+                          n_sub_iteration: int = 8, mask_prob: float = 0.5, convert_inputs: Optional[ConvertToSamInputs] = None,
+                          lr: float = 1e-5, betas=(0.9, 0.999), eps: float = 1e-8, weight_decay: float = 0.01):
+    """One iteration of JointSamTrainer._train_epoch_impl (joint_sam_trainer.py:99-114): the interactive iteration on the label
+    images `y` (`interactive_train_iteration`), its backward and AdamW step over the SAM model; then the instance iteration on
+    the UNETR targets `y_instance` through the encoder, its backward and a step over the encoder and the UNETR decoder.  `unetr`
+    must be built on `model.sam`.  Returns (interactive loss, instance loss), detached."""
+    if unetr.sam is not model.sam:
+        raise ValueError("joint training: the UNETR must share the SAM model's image encoder")
+    sam = model.sam
+    sam.train()
+    sam.zero_decoder_grads()
+    loss = interactive_train_iteration(model, x, y, iteration, n_objects_per_batch, n_sub_iteration, mask_prob, convert_inputs)[0]
+    loss.backward()
+    sam.optimizer_step(lr, betas, eps, weight_decay)
+    sam.zero_decoder_grads()   # optimizer.zero_grad(): the prompt encoder and mask decoder get no gradient in the instance step
+    unetr_loss = instance_train_iteration(unetr, x, y_instance, freeze_encoder=False, lr=lr, betas=betas, eps=eps,
+                                          weight_decay=weight_decay)
+    return loss.detach(), unetr_loss
+
+
+def export_instance_segmentation_model(unetr: UNETR, output_path) -> None:
+    """export_instance_segmentation_model (training.py:378) with a different signature: the reference reads a trainer checkpoint
+    (trained_model_path, output_path, model_type, initial_checkpoint_path); this writes the in-memory model.  The file is the same:
+    {"model_state": the SAM weights ("sam."-prefixed; the optimizer's masters where it trained them), "decoder_state": the UNETR
+    decoder}, loadable by get_predictor_and_decoder."""
+    model_state = {"sam." + k: v.detach().cpu() for k, v in unetr.sam.trained_state_dict().items()}
+    torch.save({"model_state": model_state, "decoder_state": unetr.decoder_state_dict()}, output_path)
