@@ -52,6 +52,69 @@ def _dec(sd):
     return unetr.TrainableUNETRDecoder(sd, device=DEV)
 
 
+def wgrad_plan(cout, cin, B, H, W, ks):
+    """(splits, k-blocks per split, k-blocks in all) of msam_op_ais_wgrad (wgrad_plan in csrc/ais_train.cu)"""
+    mh, nb = (2 if cout % 128 == 0 else 1), (2 if cin % 128 == 0 else 1)
+    kb_total = B * ((W + 63) // 64) * ((H + 1) // 2)
+    ctas = (cout // (64 * mh)) * ks * ks * (cin // (64 * nb))
+    splits = max(min(-(-264 // ctas), -(-kb_total // 8)), 1)
+    per = -(-kb_total // splits)
+    return -(-kb_total // per), per, kb_total
+
+
+def production_wgrad_cases():
+    """every (Cout, C0, C1, B, H, W, ks) the production decoder's backward passes to _wgrad, both samplers, B = 1 and 2, on a
+    64 x 64 embedding (1024^2 maps)"""
+    cases = set()
+    for transposed in (False, True):
+        d = _dec(unetr.default_decoder_state(transposed=transposed))
+        real = d._wgrad
+
+        def record(dy, x0, x1, ks):
+            cases.add((dy.shape[3], x0.shape[3], 0 if x1 is None else x1.shape[3], *dy.shape[:3], ks))
+            return real(dy, x0, x1, ks)
+
+        d._wgrad = record
+        for B in (1, 2):
+            d.forward(torch.zeros(B, 256, 64, 64, device=DEV))
+            d.backward(torch.zeros(B, 3, 1024, 1024, device=DEV))
+        del d
+    return sorted(cases)
+
+
+def test_wgrad_at_production_shapes():
+    """the weight gradient of every convolution the production decoder trains, at its own shape, against a float64 conv2d
+    weight gradient on the GPU: long k-loops per split, short last splits, and single-split grids.  The fp32 accumulation
+    error grows with the k-blocks per split: 1e-6 .. 1e-5 up to 70 of them, and about 1.5e-7 per k-block beyond (8.1e-5 at
+    547 k-blocks of 128 pixels, the head block's 3x3 convolutions at B = 2, H100); bound max(1e-5, 3e-7 per k-block)."""
+    L = _lib.lib()
+    g = torch.Generator(device=DEV).manual_seed(17)
+    bad = []
+    for cout, C0, C1, B, H, W, ks in production_wgrad_cases():
+        splits, per, kb_total = wgrad_plan(cout, C0 + C1, B, H, W, ks)
+        nbytes = int(L.msam_ais_wgrad_workspace(cout, C0, C1, B, H, W, ks))
+        assert nbytes == splits * cout * ks * ks * (C0 + C1) * 4
+        x = torch.randn(B, H, W, C0 + C1, generator=g, device=DEV).to(torch.bfloat16)
+        dy = torch.randn(B, H, W, cout, generator=g, device=DEV).to(torch.bfloat16)
+        x0, x1 = x[..., :C0].contiguous(), (x[..., C0:].contiguous() if C1 else None)
+        ws = torch.empty(nbytes, device=DEV, dtype=torch.uint8)
+        dw = torch.empty(cout, ks * ks * (C0 + C1), device=DEV)
+        _lib.check(L.msam_op_ais_wgrad(_lib.ptr(dy), cout, _lib.ptr(x0), C0, _lib.ptr(x1), C1, B, H, W, ks, _lib.ptr(ws), ws.numel(),
+                                       _lib.ptr(dw), _lib.cur_stream()))
+        del x0, x1, ws
+        want = torch.nn.grad.conv2d_weight(x.permute(0, 3, 1, 2).double(), (cout, C0 + C1, ks, ks), dy.permute(0, 3, 1, 2).double(),
+                                           padding=ks // 2).permute(0, 2, 3, 1).reshape(cout, -1)
+        err = ref.rel_l2(dw, want)
+        print(f"wgrad Cout={cout} C0={C0} C1={C1} B={B} {H}x{W} ks={ks}: splits={splits} per={per} "
+              f"last={kb_total - (splits - 1) * per} rel-L2 {err:.2e}")
+        if not err < max(1e-5, 3e-7 * per):
+            bad.append(((cout, C0, C1, B, H, W, ks), err))
+        del x, dy, dw, want
+    assert not bad, bad
+
+
+
+
 def test_dgrad_through_rotated_weights():
     g = torch.Generator().manual_seed(3)
     w = torch.randn(64, 128, 3, 3, generator=g) * 0.05
@@ -65,19 +128,17 @@ def test_dgrad_through_rotated_weights():
     assert ref.rel_l2(got.permute(0, 3, 1, 2).float(), x.grad) < 8e-3
 
 
-@pytest.mark.parametrize("per_image,affine", [(True, False), (True, True), (False, True)])
-def test_norm_forward_backward_against_float64(per_image, affine):
-    g = torch.Generator().manual_seed(4)
-    B, C, H, W = 2, 64, 33, 40
-    x = torch.relu(torch.randn(B, C, H, W, generator=g) + 0.3).to(torch.bfloat16).double().requires_grad_(True)
-    gam = (1 + 0.2 * torch.randn(C, generator=g)).double().requires_grad_(True) if affine else None
-    bet = (0.2 * torch.randn(C, generator=g)).double().requires_grad_(True) if affine else None
-    rm, rv = torch.zeros(C, dtype=torch.float64), torch.ones(C, dtype=torch.float64)
+def _check_norm(per_image, affine, B, C, H, W, g, dev="cpu"):
+    """training-mode norm forward (with BatchNorm's running statistics) and backward against float64 autograd on `dev`"""
+    x = torch.relu(torch.randn(B, C, H, W, generator=g, device=dev) + 0.3).to(torch.bfloat16).double().requires_grad_(True)
+    gam = (1 + 0.2 * torch.randn(C, generator=g, device=dev)).double().requires_grad_(True) if affine else None
+    bet = (0.2 * torch.randn(C, generator=g, device=dev)).double().requires_grad_(True) if affine else None
+    rm, rv = torch.zeros(C, dtype=torch.float64, device=dev), torch.ones(C, dtype=torch.float64, device=dev)
     if per_image:
         y = F.instance_norm(x, weight=gam, bias=bet, eps=1e-5)
     else:
         y = torch.relu(F.batch_norm(x, rm, rv, gam, bet, training=True, momentum=0.1, eps=1e-5))
-    dy = torch.randn(B, C, H, W, generator=g).to(torch.bfloat16).double()
+    dy = torch.randn(B, C, H, W, generator=g, device=dev).to(torch.bfloat16).double()
     (y * dy).sum().backward()
     d = _dec(unetr_ref.seeded_state(seed=1, **REDUCED))
     xd = _bf(_nhwc(x.detach()))
@@ -93,6 +154,18 @@ def test_norm_forward_backward_against_float64(per_image, affine):
     assert ref.rel_l2(dx.permute(0, 3, 1, 2), x.grad) < 1e-2
     if affine:
         assert ref.rel_l2(dg, gam.grad) < 1e-3 and ref.rel_l2(db, bet.grad) < 1e-3
+
+
+@pytest.mark.parametrize("per_image,affine", [(True, False), (True, True), (False, True)])
+def test_norm_forward_backward_against_float64(per_image, affine):
+    _check_norm(per_image, affine, 2, 64, 33, 40, torch.Generator().manual_seed(4))
+
+
+@pytest.mark.parametrize("per_image", [True, False])
+def test_norm_forward_backward_at_1024(per_image):
+    """the head block's InstanceNorm and deconv4's BatchNorm at their production size: 1024 chunks of NT_CHUNK pixels per
+    image, and BatchNorm's statistics over two images"""
+    _check_norm(per_image, True, 2, 64, 1024, 1024, torch.Generator(device=DEV).manual_seed(4), dev=DEV)
 
 
 def test_upsample_space_to_depth_head_resize_and_loss_backward():
@@ -145,6 +218,54 @@ def test_upsample_space_to_depth_head_resize_and_loss_backward():
         want.backward()
         xg = xl.detach().float().to(DEV).requires_grad_(True)
         got = training.DiceBasedDistanceLoss(mask)(xg, yl.float().to(DEV))
+        got.backward()
+        assert abs(float(got) - float(want)) < 1e-5
+        assert ref.rel_l2(xg.grad, xl.grad) < 1e-4
+
+
+def test_head_resize_and_loss_backward_at_1024():
+    """out_conv + sigmoid backward, the crop + resize backward and the distance loss at the decoder's output size, B = 2: 2048
+    chunks of NT_CHUNK pixels in the head's weight gradient, 256 chunks of DL_CHUNK per image in the loss statistics"""
+    g = torch.Generator(device=DEV).manual_seed(6)
+    L = _lib.lib()
+    B, C, HW = 2, 64, 1024 * 1024
+    h = torch.relu(torch.randn(B, C, 1024, 1024, generator=g, device=DEV)).to(torch.bfloat16).double().requires_grad_(True)
+    w = (torch.randn(3, C, generator=g, device=DEV) * 0.1).double().requires_grad_(True)
+    b = torch.randn(3, generator=g, device=DEV).double().requires_grad_(True)
+    s = torch.sigmoid(F.conv2d(h, w[:, :, None, None], b))
+    dm = torch.randn(s.shape, generator=g, device=DEV).double()
+    (s * dm).sum().backward()
+    hd = _bf(_nhwc(h.detach()))
+    wd, bdv = w.detach().float().contiguous(), b.detach().float()
+    maps = torch.empty(B, 3, 1024, 1024, device=DEV)
+    _lib.check(L.msam_op_ais_head(_lib.ptr(hd), B, HW, C, _lib.ptr(wd), _lib.ptr(bdv), _lib.ptr(maps), _lib.cur_stream()))
+    assert ref.rel_l2(maps, s.detach()) < 1e-5
+    ws = torch.empty(int(L.msam_ais_head_backward_workspace(B, HW, C)), device=DEV, dtype=torch.uint8)
+    dh, dw, db = torch.empty_like(hd), torch.empty(3, C, device=DEV), torch.empty(3, device=DEV)
+    _lib.check(L.msam_op_ais_head_backward(_lib.ptr(hd), B, HW, C, _lib.ptr(wd), _lib.ptr(maps), _lib.ptr(dm.float()), _lib.ptr(ws),
+                                           ws.numel(), _lib.ptr(dh), _lib.ptr(dw), _lib.ptr(db), _lib.cur_stream()))
+    assert ref.rel_l2(dw, w.grad) < 1e-4 and ref.rel_l2(db, b.grad) < 1e-4
+    assert ref.rel_l2(dh.permute(0, 3, 1, 2), h.grad * (h.detach() > 0)) < 5e-3
+    del h, s, hd, dh, ws
+    # crop + resize to a few original sizes, as postprocess_masks after the decoder
+    for (ih, iw), (oh, ow) in [((1024, 768), (1536, 1152)), ((768, 1024), (600, 800)), ((1024, 1024), (1024, 1024))]:
+        m = torch.zeros(B, 3, 1024, 1024, dtype=torch.float64, device=DEV, requires_grad=True)
+        do = torch.randn(B, 3, oh, ow, generator=g, device=DEV).double()
+        (ref.crop_resize(m, (ih, iw), (oh, ow)) * do).sum().backward()
+        tmp = torch.empty(B * 3 * oh * iw, device=DEV)
+        dm2 = torch.empty(B, 3, 1024, 1024, device=DEV)
+        _lib.check(L.msam_op_ais_resize_backward(_lib.ptr(do.float()), B * 3, 1024, 1024, ih, iw, oh, ow, _lib.ptr(tmp), _lib.ptr(dm2),
+                                                 _lib.cur_stream()))
+        assert ref.rel_l2(dm2, m.grad) < 1e-4, (ih, iw, oh, ow)   # fp32 interpolation weights: 4.6e-5 at 1024 -> 1536
+    # distance-based Dice loss: statistics and backward
+    for mask in (True, False):
+        xl = torch.rand(B, 3, 1024, 1024, generator=g, device=DEV).double().requires_grad_(True)
+        yl = torch.rand(B, 3, 1024, 1024, generator=g, device=DEV).double()
+        yl[:, 0] = (yl[:, 0] > 0.4).double()
+        want = ref.dice_based_distance_loss(xl, yl, mask)
+        want.backward()
+        xg = xl.detach().float().requires_grad_(True)
+        got = training.DiceBasedDistanceLoss(mask)(xg, yl.float())
         got.backward()
         assert abs(float(got) - float(want)) < 1e-5
         assert ref.rel_l2(xg.grad, xl.grad) < 1e-4
