@@ -255,7 +255,9 @@ int msam_op_dec_upscale(msam_handle* h, const void* keys, const float* hyper_in,
  * the mask decoder).  Every trainable tensor has one fp32 gradient buffer and one fp32 master buffer in the engine, listed by
  * msam_train_tensor_count / _info (below); that list is the only way to read gradients and master weights.
  * msam_encode_train = msam_encode_f32 that keeps the activations of B <= max_batch images (ViT encoders only);
- * msam_encode_backward takes dL/d(embedding) (B,256,64,64) fp32 NCHW and overwrites the gradient of every encoder parameter. */
+ * msam_encode_backward takes dL/d(embedding) (B,256,64,64) fp32 NCHW and overwrites the gradient of every encoder parameter.  It
+ * needs the latest forward pass to be that training forward: an inference encode (msam_encode_f32 / _u8 / _u8_blocks) or an
+ * optimizer step in between discards the saved pass, and the backward then fails. */
 int msam_encode_train(msam_handle* h, const float* nchw, int B, float* out, void* stream);
 int msam_encode_backward(msam_handle* h, const float* d_out_nchw, void* stream);
 /* Mask decoder + prompt encoder in training mode (micro_sam/training/trainable_sam.py:62-114): MaskDecoder.forward for the P prompts of

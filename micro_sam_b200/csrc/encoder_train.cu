@@ -1,7 +1,9 @@
 // ViT image encoder, training mode (BASELINE.json configs[4] "vit_b fine-tuning step: encoder fwd/bwd"): a forward pass that keeps
 // what the backward pass needs, and the backward pass itself.  Reference: torch autograd over ImageEncoderViT (oracle/sam_ref.py)
 // as driven by micro_sam/training/sam_trainer.py:393 (loss.backward()); gradients are checked tensor by tensor against it in
-// tests/test_gpu_backward.py.
+// tests/test_gpu_backward.py, and against a float64 mirror that rounds to bf16 where this file does in
+// tests/test_gpu_encoder_train_mirror.py.  The backward pass reads the workspace of the inference forward (patches, neck
+// activations), so any inference encode discards the saved forward pass (Engine::encode -> train_invalidate).
 //
 // Saved per block (bf16 unless noted): x_in (fp32), qkv, attention output, x_mid (fp32), fc1 pre-activation.  LayerNorm outputs and
 // GELU(fc1) are recomputed (HBM-bound, cheaper than keeping them).  Per block, in reverse:

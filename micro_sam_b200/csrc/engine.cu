@@ -255,6 +255,9 @@ int Engine::alloc_encoder_ws() {
 // ------------------------------------------------------------------------------------------------ encoder forward
 int Engine::encode(const uint8_t* u8, const float* f32, int B, int hh, int ww, float* out, cudaStream_t st, int stop_after,
                    float* x_out) {
+  // the inference forward writes the workspace that msam_encode_backward reads (patches, neck activations): a saved training
+  // forward pass does not survive it
+  train_invalidate();
   if (is_tinyvit()) return encode_tinyvit(u8, f32, B, hh, ww, out, st, stop_after, x_out);
   if (!finalized) return set_error("msam_encode: weights not finalized");
   if (B <= 0) return set_error("msam_encode: empty batch");

@@ -94,18 +94,24 @@ class ResizeLongestSide:
 class _EncoderFn(torch.autograd.Function):
     """image_encoder with a backward pass (cfg 5): forward = msam_encode_train (keeps the activations in the engine), backward =
     msam_encode_backward, which fills the engine's per-parameter gradients (read them with `B200Sam.encoder_grads()`); the image
-    itself gets no gradient (trainable_sam.py never asks for one)."""
+    itself gets no gradient (trainable_sam.py never asks for one).  The engine keeps the activations of one forward pass only, so
+    the backward pass of an output is refused once another encoder forward (training or inference) has run on the same model."""
 
     @staticmethod
     def forward(ctx, x, anchor, sam):
         x = x.to(device=sam.device, dtype=torch.float32).contiguous()
         out = torch.empty(x.shape[0], 256, 64, 64, device=sam.device, dtype=torch.float32)
+        ctx.serial = sam._encoder_forward_started()
         _lib.check(_lib.lib().msam_encode_train(sam._h, _lib.ptr(x), x.shape[0], _lib.ptr(out), _lib.cur_stream()))
         ctx.sam = sam
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
+        if ctx.sam._encoder_forwards != ctx.serial:
+            raise RuntimeError("image_encoder backward: another encoder forward pass ran on this model after the training forward "
+                               "that produced this output, and the engine keeps the activations of the latest one only; run "
+                               "backward() before the next image_encoder(...) call")
         g = grad_out.to(torch.float32).contiguous()
         _lib.check(_lib.lib().msam_encode_backward(ctx.sam._h, _lib.ptr(g), _lib.cur_stream()))
         ctx.sam._encoder_grads_valid = True
@@ -194,6 +200,7 @@ class _ImageEncoder:
             return _EncoderFn.apply(x, sam._grad_anchor, sam)
         x = x.to(device=sam.device, dtype=torch.float32).contiguous()
         out = torch.empty(x.shape[0], 256, 64, 64, device=sam.device, dtype=torch.float32)
+        sam._encoder_forward_started()
         _lib.check(_lib.lib().msam_encode_f32(sam._h, _lib.ptr(x), x.shape[0], _lib.ptr(out), _lib.cur_stream()))
         return out
 
@@ -336,6 +343,7 @@ class B200Sam:
         self._bound_key = self._bound_src = self._bound_tensor = None
         self._encoder_grads_valid = self._decoder_grads_valid = False   # a rebuilt engine has no training state yet
         self._mask_grads_valid = False   # mask_downscaling joins the trained tensors with the first masked backward
+        self._encoder_forward_started()   # a pending encoder backward belongs to the old engine
         with torch.cuda.device(self.device):
             _lib.check(L.msam_create(ctypes.byref(self._cfg), self.device.index, ctypes.byref(self._h)))
             self._state = {}
@@ -500,6 +508,14 @@ class B200Sam:
             raise RuntimeError("no encoder gradients: run image_encoder(x) in train() mode and call backward() first")
         return self._upstream(lambda k: k.startswith("image_encoder.") and (names is None or k in names), master=False)
 
+    _encoder_forwards = 0
+
+    def _encoder_forward_started(self) -> int:
+        """Counts the encoder forward passes run on this model (training and inference) and returns the new count: a training
+        forward's backward pass is only valid while its count is the latest (`_EncoderFn`)."""
+        self._encoder_forwards += 1
+        return self._encoder_forwards
+
     def bind_embedding(self, f: torch.Tensor) -> None:
         """Bind a (1,256,64,64) image embedding as the decoder's current image (SamPredictor.features assignment).  The
         engine caches prompt-independent decoder state per bound embedding; the cache key lives HERE, with the engine it
@@ -538,6 +554,7 @@ class B200Sam:
         if x.dtype != torch.uint8 or x.ndim != 4 or x.shape[-1] != 3:
             raise ValueError("encode_u8 expects uint8 [B,h,w,3]")
         out = torch.empty(x.shape[0], 256, 64, 64, device=self.device, dtype=torch.float32)
+        self._encoder_forward_started()
         _lib.check(_lib.lib().msam_encode_u8(self._h, _lib.ptr(x), x.shape[0], x.shape[1], x.shape[2], _lib.ptr(out),
                                              _lib.cur_stream()))
         return out
