@@ -525,6 +525,26 @@ int msam_op_ais_dist_loss_backward(const float* x, const float* y, int B, int HW
  * for tensors kept outside the engine's table. */
 int msam_op_adamw(float* w, const float* g, float* m, float* v, int64_t n, float lr, float beta1, float beta2, float eps,
                   float weight_decay, int step, void* stream);
+/* ---- object centres, bounding boxes and one-hot masks of a label image (csrc/centers.cu; micro_sam/util.py:1283-1396) ----
+ * labels: int32 ids in [0, 2^31), 0 background, C order, ndim 2 ([H, W]) or 3 ([Z, H, W]) with host extents dims; the grid padded
+ * by one pixel per side must have fewer than 2^31 pixels.  ws: msam_centers_workspace bytes of device memory, 256-byte aligned.
+ * msam_centers_boxes: for the n_ids objects of ids (int32, sorted ascending, unique, non-zero; pixels with other ids are ignored)
+ * boxes int32 [n_ids][2 ndim] = (min per axis, max + 1 per axis) and centers [n_ids][ndim]: mode 'v' int32, the object pixel of
+ * largest Euclidean distance to the inner boundaries of the padded labels (the first in raster order on ties); mode 'p' fp64,
+ * the mean pixel coordinate (int64 sums divided once).  Integer atomics only: bit-identical from run to run. */
+int64_t msam_centers_workspace(int ndim, const int* dims, int n_ids);
+int msam_centers_boxes(const int32_t* labels, int ndim, const int* dims, int mode, void* ws, int64_t ws_bytes, const int32_t* ids,
+                       int n_ids, void* centers, int32_t* boxes, void* stream);
+/* out uint8 over the padded grid ([H + 2, W + 2] or [Z + 2, H + 2, W + 2]): 1 where skimage's find_boundaries(np.pad(labels, 1),
+ * mode="inner") is true (foreground with a different label among its in-grid cross / 6-neighbours) */
+int msam_op_label_boundaries(const int32_t* labels, int ndim, const int* dims, uint8_t* out, void* stream);
+/* out int32 = scipy's distance_transform_edt(mask)^2 exactly, for a uint8 mask of 1 to 3 dims (< 2^31 pixels): the squared
+ * distance of every pixel to the nearest zero of mask (0 on the zeros), saturated at INT32_MAX (also where mask has no zero).
+ * ws: 3 x (4 n bytes rounded up to 256) of device memory, 256-byte aligned. */
+int msam_op_edt_squared(const uint8_t* mask, int ndim, const int* dims, void* ws, int64_t ws_bytes, int32_t* out, void* stream);
+/* segmentation_to_one_hot's planes: out fp32 [n_planes, n], plane p = (plane(labels[i]) == p).  ids NULL: plane(v) = v - 1;
+ * else ids int32 [n_tab] sorted ascending and unique, plane(v) = the index of v in ids (none when absent or v == 0). */
+int msam_segmentation_one_hot(const int32_t* labels, int64_t n, const int32_t* ids, int n_tab, int n_planes, float* out, void* stream);
 /* debug: device buffer of 64 x 16 uint64 %globaltimer stamps written by the window-attention kernels, NULL = off */
 int msam_debug_attn_trace(void* dev_buf);
 

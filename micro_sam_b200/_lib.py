@@ -199,6 +199,13 @@ def lib() -> ctypes.CDLL:
         L.msam_op_ais_dist_loss_backward.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]
         L.msam_op_adamw.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_float, c_float, c_float, c_float, c_float,
                                     c_int, c_void_p]
+        L.msam_centers_workspace.restype = c_int64
+        L.msam_centers_workspace.argtypes = [c_int, POINTER(c_int), c_int]
+        L.msam_centers_boxes.argtypes = [c_void_p, c_int, POINTER(c_int), c_int, c_void_p, c_int64, c_void_p, c_int, c_void_p, c_void_p,
+                                         c_void_p]
+        L.msam_op_label_boundaries.argtypes = [c_void_p, c_int, POINTER(c_int), c_void_p, c_void_p]
+        L.msam_op_edt_squared.argtypes = [c_void_p, c_int, POINTER(c_int), c_void_p, c_int64, c_void_p, c_void_p]
+        L.msam_segmentation_one_hot.argtypes = [c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p]
         _lib = L
     return _lib
 

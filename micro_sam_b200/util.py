@@ -11,6 +11,7 @@ Out of scope: pooch downloads.
 """
 from __future__ import annotations
 
+import ctypes
 import hashlib
 import os
 import warnings
@@ -625,6 +626,120 @@ def compute_iou(mask1: np.ndarray, mask2: np.ndarray) -> float:
     overlap = np.logical_and(mask1 == 1, mask2 == 1).sum()
     union = np.logical_or(mask1 == 1, mask2 == 1).sum()
     return float(overlap) / (float(union) + 1e-7)
+
+
+# ------------------------------------------------------------------------------------------------ centres, boxes and one-hot
+def _check_label_shape(shape) -> None:
+    if len(shape) not in (2, 3):
+        raise ValueError(f"segmentation must be 2-D or 3-D, got {len(shape)} dimensions")
+    padded = int(np.prod([int(v) + 2 for v in shape]))
+    if min(shape) == 0 or padded >= 2 ** 31:
+        raise ValueError(f"segmentation of shape {tuple(shape)}: the image padded by one pixel per side must have fewer than 2^31 "
+                         f"pixels (int32 linear indices), got {padded}, and no axis may be empty")
+
+
+def _labels_for_centers(segmentation):
+    """A 2-D or 3-D integer label image (numpy or torch, host or device) -> (int32 labels on the device, C order; the sorted
+    unique ids present, int64 on the device, 0 included when present; the largest id).  Refuses non-integer labels, negative
+    labels, ids >= 2^31 and images whose grid padded by one pixel per side has 2^31 pixels or more."""
+    wrapped = False   # unsigned values reinterpreted as signed: a negative value is one >= 2^31 (uint32) or >= 2^63 (uint64)
+    if torch.is_tensor(segmentation):
+        t = segmentation
+        if t.is_floating_point() or t.is_complex():
+            raise ValueError(f"segmentation must hold integer labels, got {t.dtype}")
+        _check_label_shape(t.shape)
+        if t.dtype in (torch.uint32, torch.uint64):
+            t = t.to(torch.int64)   # uint32 widens exactly; uint64 >= 2^63 wraps negative
+            wrapped = True
+        dev = t.device if t.is_cuda else torch.device("cuda", torch.cuda.current_device())
+        t = t.to(dev)
+    else:
+        a = np.asarray(segmentation)
+        if a.dtype.kind not in "biu":
+            raise ValueError(f"segmentation must hold integer labels, got {a.dtype}")
+        _check_label_shape(a.shape)
+        if a.dtype == np.uint32:
+            a, wrapped = a.view(np.int32), True
+        elif a.dtype == np.uint64:
+            a, wrapped = a.view(np.int64), True
+        dev = torch.device("cuda", torch.cuda.current_device())
+        t = torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    if t.dtype == torch.bool:
+        t = t.to(torch.uint8)
+    ids = torch.unique(t)
+    lo, hi = (int(v) for v in ids[[0, -1]].tolist())
+    if lo < 0:
+        raise ValueError("segmentation ids must be below 2^31" if wrapped else "segmentation labels must be non-negative")
+    if hi >= 2 ** 31:
+        raise ValueError(f"segmentation ids must be below 2^31, got {hi}")
+    return t.to(torch.int32).contiguous(), ids.to(torch.int64), hi
+
+
+def get_centers_and_bounding_boxes(segmentation, mode: str = "v", device_result: bool = False):
+    """util.get_centers_and_bounding_boxes (micro_sam/util.py:1283-1331) on the device (csrc/centers.cu), 2-D and 3-D.
+
+    Returns (centers, boxes): two dicts keyed by object id in ascending order.  mode "v": the object pixel of largest distance to
+    the object boundary (ties: the first in raster order), as a tuple of ints; "p": the centroid, a tuple of float64.  Boxes are
+    skimage's bbox tuples (min per axis, then max + 1 per axis).  `segmentation` holds integer labels (numpy or torch, host or
+    device; 0 is background, ids below 2^31).  The rules are restated in DESIGN.md section 2.
+
+    `device_result=True` (extension): returns device tensors (ids int64 (n,), centers (n, ndim) int32 for "v" / float64 for "p",
+    boxes int32 (n, 2 ndim)) and builds no dicts.
+    """
+    if mode not in ("p", "v"):
+        raise AssertionError("Choose either 'p' for regionprops centroids or 'v' for distance-based centers")
+    labels, ids, _ = _labels_for_centers(segmentation)
+    dev, ndim = labels.device, labels.ndim
+    ids = ids[ids != 0]
+    n = int(ids.numel())
+    centers = torch.empty((n, ndim), dtype=torch.int32 if mode == "v" else torch.float64, device=dev)
+    boxes = torch.empty((n, 2 * ndim), dtype=torch.int32, device=dev)
+    if n:
+        L = _lib.lib()
+        dims = (ctypes.c_int * ndim)(*labels.shape)
+        ws = torch.empty(int(L.msam_centers_workspace(ndim, dims, n)), dtype=torch.uint8, device=dev)
+        ids32 = ids.to(torch.int32)
+        with torch.cuda.device(dev):
+            _lib.check(L.msam_centers_boxes(_lib.ptr(labels), ndim, dims, ord(mode), _lib.ptr(ws), ws.numel(), _lib.ptr(ids32), n,
+                                            _lib.ptr(centers), _lib.ptr(boxes), _lib.cur_stream()))
+    if device_result:
+        return ids, centers, boxes
+    keys = ids.cpu().tolist()
+    cast = int if mode == "v" else float
+    center_coordinates = {k: tuple(cast(v) for v in c) for k, c in zip(keys, centers.cpu().tolist())}
+    bbox_coordinates = {k: tuple(b) for k, b in zip(keys, boxes.cpu().tolist())}
+    return center_coordinates, bbox_coordinates
+
+
+def segmentation_to_one_hot(segmentation, segmentation_ids: Optional[np.ndarray] = None) -> torch.Tensor:
+    """util.segmentation_to_one_hot (micro_sam/util.py:1356-1396) on the device (csrc/centers.cu), 2-D and 3-D.
+
+    Returns float32 masks (n_ids, 1, *shape) as a device tensor (the reference returns a CPU tensor).  Without
+    `segmentation_ids`, n_ids = segmentation.max() and plane k holds label k + 1.  With them (not empty, no 0), n_ids =
+    len(segmentation_ids) and the selected ids present in the image fill the planes in ascending order, as the reference's
+    relabel_sequential does: a selected id that is absent shifts the later ones forward and leaves an empty plane at the end.
+    """
+    if segmentation_ids is not None:
+        sel = np.asarray(segmentation_ids).ravel()
+        if len(sel) == 0 or 0 in sel:
+            raise RuntimeError("No foreground objects were found.")
+    labels, present, hi = _labels_for_centers(segmentation)
+    dev = labels.device
+    table, n_tab = None, 0
+    if segmentation_ids is None:
+        n_planes = hi
+    else:
+        n_planes = len(sel)
+        wanted = torch.as_tensor(np.sort(sel).astype(np.int64), device=dev)
+        table = present[torch.isin(present, wanted) & (present != 0)].to(torch.int32)
+        n_tab = int(table.numel())
+        if n_tab == 0:   # no selected id is present: every plane is empty, but the table pointer must still be set
+            table = torch.zeros(1, dtype=torch.int32, device=dev)
+    out = torch.empty((n_planes, 1) + tuple(labels.shape), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().msam_segmentation_one_hot(_lib.ptr(labels), labels.numel(), _lib.ptr(table), n_tab,
+                                                        n_planes, _lib.ptr(out), _lib.cur_stream()))
+    return out
 
 
 # ------------------------------------------------------------------------------------------------ label image assembly
