@@ -521,6 +521,20 @@ int64_t msam_ais_dist_loss_workspace(int B, int HW);
 int msam_op_ais_dist_loss_stats(const float* x, const float* y, int B, int HW, int mask, void* ws, int64_t ws_bytes, double* stats,
                                 void* stream);
 int msam_op_ais_dist_loss_backward(const float* x, const float* y, int B, int HW, int mask, const float* coef, float* dx, void* stream);
+/* ---- loss of semantic fine-tuning (csrc/semantic_loss.cu; micro_sam/training/semantic_sam_trainer.py:11-86) ----
+ * low_res fp32 [B, C, 256, 256] logits (1 <= C <= 15), labels [B, H, W] (label_dtype 0 int32, 1 int64), (in_h, in_w) the
+ * input_size and (H, W) the original_size of Sam.postprocess_masks, evaluated per pixel and never materialised.  With
+ * p = softmax over the C full-resolution logits, stats (device, fp64 [3 C + 3]) = per class c { sum p_c [l == c], sum p_c^2,
+ * sum [l == c] }, then { sum of -log p_l over the labels l in [0, C), their count, the count of labels outside [0, C) other
+ * than -100 }.  Label -100 is ignored by the cross entropy and in no class.  The backward pass takes d_stats (device, fp64, the
+ * layout of stats; reads dL/d sum p_c t_c, dL/d sum p_c^2 and dL/d ce sum) and WRITES d_low_res.  fp64 partials reduced in a
+ * fixed order and no float atomics: repeats are bit-identical.  ws: msam_semantic_loss_workspace(..., backward) bytes of
+ * device memory, 256-byte aligned (backward = 1 sizes it for both calls). */
+int64_t msam_semantic_loss_workspace(int B, int C, int in_h, int in_w, int H, int W, int backward);
+int msam_semantic_loss_stats(const float* low_res, const void* labels, int label_dtype, int B, int C, int in_h, int in_w, int H, int W,
+                             void* ws, int64_t ws_bytes, double* stats, void* stream);
+int msam_semantic_loss_backward(const float* low_res, const void* labels, int label_dtype, const double* d_stats, int B, int C, int in_h,
+                                int in_w, int H, int W, void* ws, int64_t ws_bytes, float* d_low_res, void* stream);
 /* One AdamW step (torch.optim.AdamW) of fp32 masters w with gradients g and moments m, v at bias-correction step `step` (>= 1),
  * for tensors kept outside the engine's table. */
 int msam_op_adamw(float* w, const float* g, float* m, float* v, int64_t n, float lr, float beta1, float beta2, float eps,

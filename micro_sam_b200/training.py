@@ -670,6 +670,147 @@ def joint_train_iteration(model: TrainableSAM, unetr: UNETR, x, y, y_instance, i
     return loss.detach(), unetr_loss
 
 
+# ---------------------------------------------------------------------------------------------------------------------------------
+# Semantic segmentation loss: micro_sam/training/semantic_sam_trainer.py:11-86 (CustomDiceLoss, SemanticSamTrainer._compute_loss)
+# and micro_sam/training/util.py:268-280 (ConvertToSemanticSamInputs)
+
+MAX_SEMANTIC_CLASSES = 15
+
+
+class ConvertToSemanticSamInputs:
+    """micro_sam.training.util.ConvertToSemanticSamInputs: one record {"image", "original_size"} per image, with no prompts."""
+
+    def __call__(self, x, y):
+        return [{"image": image, "original_size": image.shape[-2:]} for image in x]
+
+
+class _SemanticStatsFn(torch.autograd.Function):
+    """msam_semantic_loss_stats with its adjoint (msam_semantic_loss_backward): the loss depends on the logits only through the
+    per-class sums (sum p t, sum p^2) and the cross-entropy sum; the counts are piecewise constant."""
+
+    @staticmethod
+    def forward(ctx, lr, labels, in_h, in_w):
+        B, C = lr.shape[:2]
+        H, W = labels.shape[-2:]
+        L = _lib.lib()
+        label64 = int(labels.dtype == torch.int64)
+        ws = torch.empty(int(L.msam_semantic_loss_workspace(B, C, in_h, in_w, H, W, 0)), device=lr.device, dtype=torch.uint8)
+        st = torch.empty(3 * C + 3, device=lr.device, dtype=torch.float64)
+        _lib.check(L.msam_semantic_loss_stats(_lib.ptr(lr), _lib.ptr(labels), label64, B, C, in_h, in_w, H, W, _lib.ptr(ws), ws.numel(),
+                                              _lib.ptr(st), _lib.cur_stream()))
+        ctx.save_for_backward(lr, labels)
+        ctx.geom = (in_h, in_w)
+        return st
+
+    @staticmethod
+    def backward(ctx, d_st):
+        lr, labels = ctx.saved_tensors
+        B, C = lr.shape[:2]
+        H, W = labels.shape[-2:]
+        in_h, in_w = ctx.geom
+        L = _lib.lib()
+        ws = torch.empty(int(L.msam_semantic_loss_workspace(B, C, in_h, in_w, H, W, 1)), device=lr.device, dtype=torch.uint8)
+        ds = d_st.to(torch.float64).contiguous()
+        d_lr = torch.empty_like(lr)
+        _lib.check(L.msam_semantic_loss_backward(_lib.ptr(lr), _lib.ptr(labels), int(labels.dtype == torch.int64), _lib.ptr(ds), B, C,
+                                                 in_h, in_w, H, W, _lib.ptr(ws), ws.numel(), _lib.ptr(d_lr), _lib.cur_stream()))
+        return d_lr, None, None, None
+
+
+def _semantic_inputs(pred, y, num_classes: int, input_size=None, original_size=None):
+    """(low-res logits fp32 (B, C, 256, 256), labels int32 / int64 (B, H, W), input_size) from either the batched outputs of
+    `TrainableSAM.forward` (records with "low_res_masks" (1, C, 256, 256) or (C, 256, 256), "input_size", "original_size") or the
+    low-res logits themselves; `input_size` defaults to the resized shape of the original size (ResizeLongestSide(1024))."""
+    from .sam import get_preprocess_shape
+    if isinstance(pred, (list, tuple)):
+        if not pred:
+            raise ValueError("semantic loss: no outputs")
+        lows = [o["low_res_masks"] for o in pred]
+        lows = [lo.squeeze(0) if lo.dim() == 4 else lo for lo in lows]
+        low = torch.stack(lows)
+        sizes = {tuple(int(s) for s in o["input_size"]) for o in pred}
+        origs = {tuple(int(s) for s in o["original_size"]) for o in pred}
+        if len(sizes) != 1 or len(origs) != 1:
+            raise ValueError("semantic loss: every image of the batch needs the same input_size and original_size")
+        input_size, original_size = sizes.pop(), origs.pop()
+    else:
+        low = pred
+    if low.dim() != 4 or tuple(low.shape[-2:]) != (256, 256):
+        raise ValueError(f"semantic loss: takes the low-res logits (B, C, 256, 256), got {tuple(low.shape)}; the full-resolution "
+                         "logits are evaluated per pixel from them and never materialised")
+    B, C = int(low.shape[0]), int(low.shape[1])
+    if C != num_classes:
+        raise ValueError(f"semantic loss: {C} logit channels for num_classes={num_classes}")
+    if not 1 <= C <= MAX_SEMANTIC_CLASSES:
+        raise ValueError(f"semantic loss: num_classes={C}; the loss kernels take 1..{MAX_SEMANTIC_CLASSES} classes")
+    lab = torch.as_tensor(y)
+    if lab.dim() == 4 and lab.shape[1] == 1:
+        lab = lab[:, 0]
+    if lab.dim() != 3 or lab.shape[0] != B:
+        raise ValueError(f"semantic loss: labels (B, 1, H, W) or (B, H, W) with B={B}, got {tuple(lab.shape)}")
+    H, W = int(lab.shape[-2]), int(lab.shape[-1])
+    if original_size is not None and tuple(int(s) for s in original_size) != (H, W):
+        raise ValueError(f"semantic loss: original_size {tuple(original_size)} but labels of size {(H, W)}")
+    if input_size is None:
+        input_size = get_preprocess_shape(H, W, 1024)
+    lab = lab.to(low.device)
+    if lab.dtype not in (torch.int32, torch.int64):
+        lab = lab.long()            # nn.CrossEntropyLoss takes target.long()
+    return low.to(torch.float32).contiguous(), lab.contiguous(), (int(input_size[0]), int(input_size[1]))
+
+
+def semantic_loss_stats(pred, y, num_classes: int, input_size=None, original_size=None) -> torch.Tensor:
+    """`msam_semantic_loss_stats` (fp64 (3 C + 3,)), differentiable w.r.t. the low-res logits; raises ValueError when a label lies
+    outside [0, num_classes) and is not -100 (nn.CrossEntropyLoss's ignore_index), as torch refuses such a target."""
+    low, lab, (in_h, in_w) = _semantic_inputs(pred, y, num_classes, input_size, original_size)
+    st = _SemanticStatsFn.apply(low, lab, in_h, in_w)
+    n_bad = int(st[3 * num_classes + 2].item())
+    if n_bad:
+        raise ValueError(f"semantic loss: {n_bad} labels outside [0, {num_classes}) (only -100, the ignore index, is allowed)")
+    return st
+
+
+def _semantic_dice(st: torch.Tensor, C: int, eps: float = 1e-7) -> torch.Tensor:
+    pt, pp, t = st[:3 * C].view(C, 3).unbind(-1)
+    return (1.0 - 2.0 * pt / (pp + t).clamp(min=eps)).sum()       # one-hot targets: sum t^2 = sum t
+
+
+class CustomDiceLoss:
+    """micro_sam.training.semantic_sam_trainer.CustomDiceLoss: softmax over the classes, one-hot targets (label == c; -100 in no
+    class), torch_em's DiceLoss() = sum over the classes of 1 - 2 sum(p t) / max(sum p^2 + sum t^2, 1e-7), each sum over the whole
+    batch.  `__call__(pred, target)` takes the batched outputs of `TrainableSAM.forward` or the low-res logits (B, C, 256, 256)
+    (with `input_size` / `original_size` keywords); the full-resolution logits are evaluated per pixel and never materialised."""
+
+    def __init__(self, num_classes: int, softmax: bool = True) -> None:
+        if not softmax:
+            raise NotImplementedError("CustomDiceLoss(softmax=False): the loss kernels take the softmax of the logits")
+        self.num_classes = num_classes
+        self.softmax = softmax
+
+    def __call__(self, pred, target, input_size=None, original_size=None) -> torch.Tensor:
+        st = semantic_loss_stats(pred, target, self.num_classes, input_size, original_size)
+        return _semantic_dice(st, self.num_classes).to(torch.float32)
+
+
+def _check_dice_weight(dice_weight) -> None:
+    if dice_weight is not None and (dice_weight < 0 or dice_weight > 1):
+        raise ValueError("The weight factor should lie between 0 and 1.")
+
+
+def compute_semantic_loss(pred, y, num_classes: int, dice_weight: Optional[float] = None, input_size=None,
+                          original_size=None) -> torch.Tensor:
+    """SemanticSamTrainer._compute_loss: CustomDiceLoss + nn.CrossEntropyLoss() (the mean over the pixels whose label is not -100)
+    of the full-resolution logits, or w * dice + (1 - w) * CE for `dice_weight` w in [0, 1].  `pred`: the batched outputs of
+    `TrainableSAM.forward` or the low-res logits (B, C, 256, 256); `y`: labels (B, 1, H, W) or (B, H, W).  Both terms come from one
+    pass of msam_semantic_loss_stats and are combined in fp64; the result is fp32 and differentiable w.r.t. the low-res logits."""
+    _check_dice_weight(dice_weight)
+    st = semantic_loss_stats(pred, y, num_classes, input_size, original_size)
+    dice = _semantic_dice(st, num_classes)
+    ce = st[3 * num_classes] / st[3 * num_classes + 1]
+    loss = dice + ce if dice_weight is None else dice_weight * dice + (1 - dice_weight) * ce
+    return loss.to(torch.float32)
+
+
 def export_instance_segmentation_model(unetr: UNETR, output_path) -> None:
     """export_instance_segmentation_model (training.py:378) with a different signature: the reference reads a trainer checkpoint
     (trained_model_path, output_path, model_type, initial_checkpoint_path); this writes the in-memory model.  The file is the same:

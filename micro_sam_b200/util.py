@@ -74,6 +74,31 @@ def _load_checkpoint(checkpoint_path):
     return state, model_state
 
 
+SUPPORTED_MULTIMASK_OUTPUTS = 3   # the mask decoder has 4 mask tokens: the single mask and 3 multimask outputs
+
+
+def _check_model_kwargs(kwargs) -> None:
+    """The model keywords of micro-sam's get_sam_model (util.py:434-476) that this port cannot honour are refused, not ignored:
+    a mask decoder with another mask-token count (semantic models, `num_multimask_outputs=C`) is not built, and
+    `flexible_load_checkpoint` only matters for such models."""
+    n = kwargs.get("num_multimask_outputs")
+    if n is not None and n != SUPPORTED_MULTIMASK_OUTPUTS:
+        raise NotImplementedError(f"get_sam_model(num_multimask_outputs={n}): only {SUPPORTED_MULTIMASK_OUTPUTS} is supported (the "
+                                  "mask decoder is built with 4 mask tokens; semantic models with other class counts are not)")
+    if kwargs.get("flexible_load_checkpoint"):
+        raise NotImplementedError("get_sam_model(flexible_load_checkpoint=True) is not implemented: checkpoints load strictly")
+
+
+def check_mask_token_count(state_dict) -> None:
+    """A checkpoint whose mask decoder has another mask-token count than 4 (a semantic model trained with
+    num_multimask_outputs = C has C + 1) is refused with the limit named, before the weight loader's shape check."""
+    w = state_dict.get("mask_decoder.mask_tokens.weight")
+    if w is not None and tuple(w.shape)[:1] != (SUPPORTED_MULTIMASK_OUTPUTS + 1,):
+        raise NotImplementedError(f"checkpoint has {tuple(w.shape)[0]} mask tokens (a model with num_multimask_outputs="
+                                  f"{tuple(w.shape)[0] - 1}); only {SUPPORTED_MULTIMASK_OUTPUTS + 1} mask tokens "
+                                  f"(num_multimask_outputs={SUPPORTED_MULTIMASK_OUTPUTS}) are supported")
+
+
 def get_sam_model(model_type: str = "vit_b", device: Optional[Union[str, torch.device]] = None,
                   checkpoint_path: Optional[Union[str, os.PathLike]] = None, return_sam: bool = False,
                   return_state: bool = False, state_dict: Optional[Dict[str, torch.Tensor]] = None,
@@ -83,6 +108,7 @@ def get_sam_model(model_type: str = "vit_b", device: Optional[Union[str, torch.d
     for k in ("peft_kwargs", "decoder_path"):
         if unsupported.get(k) is not None:
             raise NotImplementedError(f"get_sam_model({k}=...) is outside the GPU hot path (SURVEY.md 8f)")
+    _check_model_kwargs(unsupported)
     device = get_device(device)
     state = None
     if state_dict is None:
@@ -95,6 +121,7 @@ def get_sam_model(model_type: str = "vit_b", device: Optional[Union[str, torch.d
         raise RuntimeError(f"model_type {model_type!r} does not match the checkpoint ({detected!r})")
     if detected == "vit_t" and abbrev in ("vit_b", "vit_l", "vit_h"):
         raise RuntimeError(f"model_type {model_type!r} does not match the checkpoint (MobileSAM 'vit_t')")
+    check_mask_token_count(state_dict)
     sam = B200Sam(detected, state_dict, device=device, max_batch=max_batch, max_prompts=max_prompts)
     predictor = B200SamPredictor(sam)
     predictor.model_type = model_type
