@@ -559,6 +559,18 @@ int msam_op_edt_squared(const uint8_t* mask, int ndim, const int* dims, void* ws
 /* segmentation_to_one_hot's planes: out fp32 [n_planes, n], plane p = (plane(labels[i]) == p).  ids NULL: plane(v) = v - 1;
  * else ids int32 [n_tab] sorted ascending and unique, plane(v) = the index of v in ids (none when absent or v == 0). */
 int msam_segmentation_one_hot(const int32_t* labels, int64_t n, const int32_t* ids, int n_tab, int n_planes, float* out, void* stream);
+/* ---- the UNETR decoder's training targets: torch_em's PerObjectDistanceTransform for B 2-D label images (csrc/distance_targets.cu;
+ * DESIGN.md section 2) ----
+ * labels [B, H, W] C order, label_dtype 0 int32 / 1 int64, ids in [0, 2^31) (0 background); H, W <= 32768 and B H W < 2^31 - 1024.
+ * apply_label 1: objects are the 8-connected components of equal ids (skimage.measure.label), numbered in raster order of their
+ * first pixel; 0: the distinct ids in ascending order.  Objects of fewer than min_size pixels become background.  channels: bit
+ * 1 instances (per-image object number), 2 foreground, 4 centre distances, 8 boundary distances, each normalised within its
+ * object; out fp32 [B, popcount(channels), H, W] in that order, fill at background pixels of the distance channels.
+ * ws: msam_distance_targets_workspace bytes of device memory, 256-byte aligned (-1: shape refused).  Integer atomics only:
+ * bit-identical from run to run. */
+int64_t msam_distance_targets_workspace(int B, int H, int W, int apply_label);
+int msam_distance_targets(const void* labels, int label_dtype, int B, int H, int W, int apply_label, int min_size, int channels,
+                          float fill, void* ws, int64_t ws_bytes, float* out, void* stream);
 /* debug: device buffer of 64 x 16 uint64 %globaltimer stamps written by the window-attention kernels, NULL = off */
 int msam_debug_attn_trace(void* dev_buf);
 

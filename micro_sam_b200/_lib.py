@@ -206,6 +206,10 @@ def lib() -> ctypes.CDLL:
         L.msam_op_label_boundaries.argtypes = [c_void_p, c_int, POINTER(c_int), c_void_p, c_void_p]
         L.msam_op_edt_squared.argtypes = [c_void_p, c_int, POINTER(c_int), c_void_p, c_int64, c_void_p, c_void_p]
         L.msam_segmentation_one_hot.argtypes = [c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p]
+        L.msam_distance_targets_workspace.restype = c_int64
+        L.msam_distance_targets_workspace.argtypes = [c_int, c_int, c_int, c_int]
+        L.msam_distance_targets.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_int64,
+                                            c_void_p, c_void_p]
         L.msam_semantic_loss_workspace.restype = c_int64
         L.msam_semantic_loss_workspace.argtypes = [c_int, c_int, c_int, c_int, c_int, c_int, c_int]
         L.msam_semantic_loss_stats.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int64,

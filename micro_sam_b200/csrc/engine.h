@@ -213,8 +213,17 @@ int post_finish_segmentation(const int32_t* seg, int h, int w, int min_size, int
                              int32_t* ws, cudaStream_t st);
 // Connected components of equal non-zero labels of seg int32 [h, w] (4-connectivity): parent [h * w] = the component's root,
 // its first pixel in raster order (-1 on label 0); size [h * w] = pixel count at the roots; *bg_count += count of label 0.
-// The caller zeroes *bg_count.  h * w < 2^31 - 1024.
-int post_label_components(const int32_t* seg, int h, int w, int* parent, int* size, int* bg_count, cudaStream_t st);
+// The caller zeroes *bg_count.  h * w < 2^31 - 1024.  img_h > 0: no links between rows of different blocks of img_h rows (a
+// batch of images); conn8: 8-connectivity.
+int post_label_components(const int32_t* seg, int h, int w, int* parent, int* size, int* bg_count, cudaStream_t st, int img_h = 0,
+                          int conn8 = 0);
+// Objects of B label images seg int32 [B, h, w] (ids >= 0, 0 background): apply_label = 1 the 8-connected components of equal
+// non-zero ids, 0 the distinct non-zero ids of each image.  Objects of fewer than min_size pixels become 0; the others are
+// numbered 1.. over the whole batch, image by image, within an image by first pixel in raster order (apply_label = 1) or by
+// ascending id (0).  out int32 [B, h, w]; *n_objects (device) = their count.  ws: post_label_objects_ws bytes, 8-byte aligned.
+int64_t post_label_objects_ws(int B, int h, int w, int apply_label);
+int post_label_objects(const int32_t* seg, int B, int h, int w, int apply_label, int min_size, int32_t* out, int* n_objects, void* ws,
+                       cudaStream_t st);
 // Inclusive prefix sum of in [n]: the sum up to i is out[i] + block_sums[i >> 10]; block_sums holds ceil(n / 1024) ints.
 int post_inclusive_scan(const int* in, int n, int* out, int* block_sums, cudaStream_t st);
 int post_mask_nms(const uint8_t* masks, int n, int h, int w, const float* boxes_xyxy, const float* scores, float thresh,

@@ -898,16 +898,25 @@ __global__ void cc_init_kernel(const int32_t* __restrict__ seg, int n, int w, in
 // Unions: horizontally only across warp-segment boundaries (inside a segment the run already shares a parent); vertically
 // only where the link is not implied by the left neighbours (i-1 ~ i and i-1+w ~ i+w by their runs, i-1 ~ i-1+w by the left
 // pixel's own link), i.e. at the first column of every vertical contact between two runs.
-__global__ void cc_merge_kernel(const int32_t* __restrict__ seg, int h, int w, int* __restrict__ parent) {
+// conn8 adds the diagonal links that the horizontal and vertical ones do not imply.  Rows y and y + 1 are linked only inside
+// one image of img_h rows (a batch of images stacked along the rows).
+__global__ void cc_merge_kernel(const int32_t* __restrict__ seg, int h, int w, int img_h, int conn8, int* __restrict__ parent) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= h * w) return;
   const int s = seg[i];
   if (s == 0) return;
   const int x = i % w, y = i / w;
   if ((threadIdx.x & 31) == 0 && x > 0 && seg[i - 1] == s) uf_union(parent, i - 1, i);
-  if (y + 1 < h && seg[i + w] == s) {
-    const bool implied = x > 0 && seg[i - 1] == s && seg[i + w - 1] == s;
-    if (!implied) uf_union(parent, i, i + w);
+  if (y + 1 < h && (y + 1) % img_h != 0) {
+    const bool down = seg[i + w] == s;
+    if (down) {
+      const bool implied = x > 0 && seg[i - 1] == s && seg[i + w - 1] == s;
+      if (!implied) uf_union(parent, i, i + w);
+    }
+    if (conn8 && !down) {
+      if (x > 0 && seg[i - 1] != s && seg[i + w - 1] == s) uf_union(parent, i, i + w - 1);
+      if (x + 1 < w && seg[i + 1] != s && seg[i + w + 1] == s) uf_union(parent, i, i + w + 1);
+    }
   }
 }
 __global__ void cc_flatten_count_kernel(int n, int* __restrict__ parent, int* __restrict__ size, int* __restrict__ bg_count) {
@@ -1008,12 +1017,13 @@ __global__ void cc_relabel_kernel(int n, const int* __restrict__ parent, const i
   out[i] = v;
 }
 
-int post_label_components(const int32_t* seg, int h, int w, int* parent, int* size, int* bg_count, cudaStream_t st) {
+int post_label_components(const int32_t* seg, int h, int w, int* parent, int* size, int* bg_count, cudaStream_t st, int img_h,
+                          int conn8) {
   const int n = h * w;
   const unsigned blocks = (unsigned)((n + 255) / 256);
   cc_init_kernel<<<blocks, 256, 0, st>>>(seg, n, w, parent, size);
   LAUNCH_CHECK("cc_init");
-  cc_merge_kernel<<<blocks, 256, 0, st>>>(seg, h, w, parent);
+  cc_merge_kernel<<<blocks, 256, 0, st>>>(seg, h, w, img_h > 0 ? img_h : h, conn8, parent);
   LAUNCH_CHECK("cc_merge");
   cc_flatten_count_kernel<<<blocks, 256, 0, st>>>(n, parent, size, bg_count);
   LAUNCH_CHECK("cc_flatten");
@@ -1053,6 +1063,104 @@ int post_finish_segmentation(const int32_t* seg, int h, int w, int min_size, int
   cc_relabel_kernel<<<blocks, 256, 0, st>>>(n, parent, flag, scan, bsums, out);
   prof_end(st);
   LAUNCH_CHECK("cc_relabel");
+  return 0;
+}
+
+// Objects of a batch for the distance targets (DESIGN.md section 2).  apply_label = 0: the distinct ids of each image in
+// ascending order, found by sorting the per-pixel keys (image << 31 | id) with a bitonic network (background keys sort last)
+// and numbering the first entry of each run of equal keys; a pixel's object is the lower bound of its key.
+constexpr unsigned long long kNoKey = ~0ull;
+__global__ void obj_keys_kernel(const int32_t* __restrict__ seg, int n, int img_n, long cap, unsigned long long* __restrict__ keys) {
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < cap; i += (long)gridDim.x * blockDim.x) {
+    const int32_t v = i < n ? seg[i] : 0;
+    keys[i] = v != 0 ? ((unsigned long long)(i / img_n) << 31) | (unsigned)v : kNoKey;
+  }
+}
+__global__ void bitonic_step_kernel(unsigned long long* __restrict__ a, long cap, long j, long k) {
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < cap; i += (long)gridDim.x * blockDim.x) {
+    const long l = i ^ j;
+    if (l <= i) continue;
+    const unsigned long long x = a[i], y = a[l];
+    if ((x > y) == ((i & k) == 0)) { a[i] = y; a[l] = x; }
+  }
+}
+__device__ __forceinline__ long key_bound(const unsigned long long* __restrict__ a, long n, unsigned long long v, bool upper) {
+  long lo = 0, hi = n;
+  while (lo < hi) {
+    const long mid = (lo + hi) >> 1;
+    if (upper ? a[mid] <= v : a[mid] < v) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+// flag the first entry of each run of equal keys whose run has at least min_size entries
+__global__ void obj_run_flag_kernel(const unsigned long long* __restrict__ keys, int n, int min_size, int* __restrict__ flag) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const unsigned long long v = keys[j];
+  flag[j] = v != kNoKey && (j == 0 || keys[j - 1] != v) && key_bound(keys, n, v, true) - j >= min_size;
+}
+__global__ void obj_parent_kernel(const int32_t* __restrict__ seg, int n, int img_n, const unsigned long long* __restrict__ keys,
+                                  int* __restrict__ parent) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int32_t v = seg[i];
+  parent[i] = v != 0 ? (int)key_bound(keys, n, ((unsigned long long)(i / img_n) << 31) | (unsigned)v, false) : -1;
+}
+__global__ void obj_count_kernel(int n, const int* __restrict__ scan, const int* __restrict__ bsums, int* __restrict__ n_objects) {
+  *n_objects = scan[n - 1] + bsums[(n - 1) >> 10];
+}
+
+long post_label_objects_cap(int B, int h, int w) {
+  long cap = 1;
+  while (cap < (long)B * h * w) cap <<= 1;
+  return cap;
+}
+
+int64_t post_label_objects_ws(int B, int h, int w, int apply_label) {
+  const long n = (long)B * h * w, nb = (n + 1023) / 1024;
+  const long ints = 4 * n + std::max(4096l, nb) + 8;
+  return ((4 * ints + 255) & ~255l) + (apply_label ? 0 : 8 * post_label_objects_cap(B, h, w));
+}
+
+int post_label_objects(const int32_t* seg, int B, int h, int w, int apply_label, int min_size, int32_t* out, int* n_objects, void* ws,
+                       cudaStream_t st) {
+  const long nl = (long)B * h * w;
+  if (nl >= (1l << 31) - 1024) return set_error("label_objects: batch too large (%d x %d x %d)", B, h, w);
+  const int n = (int)nl, nb = (n + 1023) / 1024;
+  int* parent = (int*)ws;
+  int* size = parent + n;
+  int* flag = parent + 2 * (size_t)n;
+  int* scan = parent + 3 * (size_t)n;
+  int* bsums = parent + 4 * (size_t)n;
+  int* bg = bsums + (nb > 4096 ? nb : 4096);
+  const unsigned blocks = (unsigned)((n + 255) / 256);
+  if (apply_label) {
+    cudaMemsetAsync(bg, 0, sizeof(int), st);
+    RUN(post_label_components(seg, B * h, w, parent, size, bg, st, h, 1));
+    cc_flag_kernel<<<blocks, 256, 0, st>>>(n, parent, size, min_size, 0, nullptr, nullptr, flag);
+    LAUNCH_CHECK("label_objects_flag");
+  } else {
+    unsigned long long* keys = (unsigned long long*)((char*)ws + post_label_objects_ws(B, h, w, 1));
+    const long cap = post_label_objects_cap(B, h, w);
+    const int kb = (int)std::min<long>((cap + 255) / 256, 1 << 16);
+    obj_keys_kernel<<<kb, 256, 0, st>>>(seg, n, h * w, cap, keys);
+    LAUNCH_CHECK("label_objects_keys");
+    for (long k = 2; k <= cap; k <<= 1)
+      for (long j = k >> 1; j > 0; j >>= 1) {
+        bitonic_step_kernel<<<kb, 256, 0, st>>>(keys, cap, j, k);
+        LAUNCH_CHECK("label_objects_sort");
+      }
+    obj_run_flag_kernel<<<blocks, 256, 0, st>>>(keys, n, std::max(min_size, 1), flag);
+    LAUNCH_CHECK("label_objects_flag");
+    obj_parent_kernel<<<blocks, 256, 0, st>>>(seg, n, h * w, keys, parent);
+    LAUNCH_CHECK("label_objects_parent");
+  }
+  RUN(post_inclusive_scan(flag, n, scan, bsums, st));
+  cc_relabel_kernel<<<blocks, 256, 0, st>>>(n, parent, flag, scan, bsums, (uint32_t*)out);
+  LAUNCH_CHECK("label_objects_relabel");
+  obj_count_kernel<<<1, 1, 0, st>>>(n, scan, bsums, n_objects);
+  LAUNCH_CHECK("label_objects_count");
   return 0;
 }
 

@@ -25,6 +25,7 @@ from __future__ import annotations
 
 from typing import Any, Dict, List, Optional, Tuple
 
+import math
 import random
 
 import numpy as np
@@ -628,6 +629,126 @@ class DiceBasedDistanceLoss:
         x = input_.to(torch.float32).contiguous()
         y = target.to(x.device, torch.float32).contiguous()
         return dice_from_stats(_DistLossStatsFn.apply(x, y, self.mask_distances_in_bg)).to(torch.float32)
+
+
+_DT_CHANNELS = (("instances", 1), ("foreground", 2), ("distances", 4), ("boundary_distances", 8))
+
+
+class PerObjectDistanceTransform:
+    """torch_em's PerObjectDistanceTransform (the UNETR decoder's targets) on the device (csrc/distance_targets.cu), as DESIGN.md
+    section 2 restates it (unpinned): float32 channels instances, foreground, centre distances and boundary distances (the
+    selected ones, in that order), each distance normalised within its object, `distance_fill_value` on the background.
+
+    A numpy (H, W) label image gives numpy (C, H, W), as torch_em does.  A CUDA tensor (H, W) or (B, H, W) gives a device tensor
+    (C, H, W) or (B, C, H, W): the batched form, meant for the batch a DataLoader returns (forked loader workers cannot use CUDA).
+    Labels are integers in [0, 2^31) (whole-number floats accepted), 0 background; sides up to 32768.  3-D labels, directed
+    distances and `sampling` are not supported.
+    """
+
+    def __init__(self, distances: bool = True, boundary_distances: bool = True, directed_distances: bool = False,
+                 foreground: bool = True, instances: bool = False, apply_label: bool = True, min_size: int = 0,
+                 distance_fill_value: float = 1.0, sampling=None):
+        if directed_distances:
+            raise NotImplementedError("PerObjectDistanceTransform: directed distances are not supported (vigra's vector sign "
+                                      "convention is not restated)")
+        if sampling is not None:
+            raise NotImplementedError("PerObjectDistanceTransform: sampling is not supported (isotropic pixels only)")
+        if min_size < 0:
+            raise ValueError(f"PerObjectDistanceTransform: min_size must be >= 0, got {min_size}")
+        self.distances, self.boundary_distances, self.directed_distances = distances, boundary_distances, directed_distances
+        self.foreground, self.instances, self.apply_label = foreground, instances, apply_label
+        self.min_size, self.distance_fill_value, self.sampling = int(min_size), float(distance_fill_value), sampling
+        self._channels = sum(bit for name, bit in _DT_CHANNELS if getattr(self, name))
+        if self._channels == 0:
+            raise ValueError("PerObjectDistanceTransform: no output channel selected")
+
+    def _device_labels(self, t: torch.Tensor) -> torch.Tensor:
+        if t.is_complex():
+            raise ValueError(f"PerObjectDistanceTransform: labels must be integers, got {t.dtype}")
+        if t.numel() == 0:
+            raise ValueError(f"PerObjectDistanceTransform: empty labels of shape {tuple(t.shape)}")
+        if t.dtype in (torch.bool, torch.uint8, torch.int8, torch.uint16, torch.int16):
+            t = t.to(torch.int32)
+        elif t.dtype in (torch.uint32, torch.uint64):
+            t = t.to(torch.float64 if t.dtype == torch.uint64 else torch.int64)
+        lo, hi = (v.item() for v in torch.aminmax(t))
+        if t.is_floating_point():
+            if not bool(torch.all(t == torch.floor(t))):
+                raise ValueError("PerObjectDistanceTransform: float labels must hold whole numbers")
+        if lo < 0:
+            raise ValueError(f"PerObjectDistanceTransform: labels must be non-negative, got {lo}")
+        if hi >= 2 ** 31:
+            raise ValueError(f"PerObjectDistanceTransform: label ids must be below 2^31, got {hi}")
+        if t.dtype not in (torch.int32, torch.int64):
+            t = t.to(torch.int32)
+        return t.contiguous()
+
+    def _run(self, t: torch.Tensor) -> torch.Tensor:
+        batched = t.dim() == 3
+        lab = self._device_labels(t if batched else t.unsqueeze(0))
+        B, H, W = lab.shape
+        L = _lib.lib()
+        nbytes = int(L.msam_distance_targets_workspace(B, H, W, int(self.apply_label)))
+        if nbytes < 0:
+            raise ValueError(f"PerObjectDistanceTransform: {B} label images of {H} x {W} (sides up to 32768, fewer than "
+                             f"2^31 - 1024 pixels in all)")
+        dev = lab.device
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        out = torch.empty((B, bin(self._channels).count("1"), H, W), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(L.msam_distance_targets(_lib.ptr(lab), 1 if lab.dtype == torch.int64 else 0, B, H, W, int(self.apply_label),
+                                               self.min_size, self._channels, self.distance_fill_value, _lib.ptr(ws), nbytes,
+                                               _lib.ptr(out), _lib.cur_stream()))
+        return out if batched else out[0]
+
+    def __call__(self, labels):
+        if torch.is_tensor(labels):
+            if not labels.is_cuda:
+                raise ValueError("PerObjectDistanceTransform: pass a CUDA tensor (H, W) / (B, H, W) or a numpy (H, W) array")
+            if labels.dim() not in (2, 3):
+                raise ValueError(f"PerObjectDistanceTransform: a label tensor is (H, W) or (B, H, W), got {tuple(labels.shape)}")
+            return self._run(labels)
+        a = np.asarray(labels)
+        if a.ndim == 3:
+            raise NotImplementedError("PerObjectDistanceTransform: 3-D label volumes (26-connectivity) are not supported; pass "
+                                      "2-D images, or a CUDA tensor (B, H, W) for a batch")
+        if a.ndim != 2:
+            raise ValueError(f"PerObjectDistanceTransform: labels must be 2-D, got shape {a.shape}")
+        if a.dtype.kind not in "biuf":
+            raise ValueError(f"PerObjectDistanceTransform: labels must be integers, got {a.dtype}")
+        if a.dtype == np.uint32:
+            a = a.astype(np.int64)
+        elif a.dtype == np.uint64:
+            a = a.astype(np.float64)
+        t = torch.from_numpy(np.ascontiguousarray(a)).to(torch.device("cuda", torch.cuda.current_device()))
+        return self._run(t).cpu().numpy()
+
+
+class ResizeLabelTrafo:
+    """micro_sam.training.util.ResizeLabelTrafo: PerObjectDistanceTransform with instances (4 channels: instances, foreground,
+    centre and boundary distances), then a centred zero pad of H and W to desired_shape[0] (ceil before, floor after).  As in
+    micro-sam both axes are padded to desired_shape[0], so a non-square desired_shape fails the final shape check.  Takes what
+    PerObjectDistanceTransform takes; a batch (B, H, W) on the device comes back as (B, 4, H', W')."""
+
+    def __init__(self, desired_shape: Tuple[int, ...], min_size: int = 0, padding: str = "constant"):
+        if padding != "constant":
+            raise NotImplementedError(f"ResizeLabelTrafo: padding mode {padding!r} is not supported (only 'constant')")
+        self.desired_shape, self.min_size, self.padding = desired_shape, min_size, padding
+
+    def __call__(self, labels):
+        trafo = PerObjectDistanceTransform(distances=True, boundary_distances=True, directed_distances=False, foreground=True,
+                                           instances=True, min_size=self.min_size)
+        out = trafo(labels)
+        dy, dx = (self.desired_shape[0] - out.shape[-2]) / 2, (self.desired_shape[0] - out.shape[-1]) / 2
+        if min(dy, dx) < 0:
+            raise ValueError(f"ResizeLabelTrafo: labels of {tuple(out.shape[-2:])} exceed the desired shape {self.desired_shape}")
+        pads = (math.ceil(dy), math.floor(dy), math.ceil(dx), math.floor(dx))
+        if torch.is_tensor(out):
+            out = torch.nn.functional.pad(out, (pads[2], pads[3], pads[0], pads[1]))
+        else:
+            out = np.pad(out, ((0, 0), pads[:2], pads[2:]), mode="constant")
+        assert tuple(out.shape[-2:]) == tuple(self.desired_shape), out.shape
+        return out
 
 
 def instance_train_iteration(unetr: UNETR, x, y, freeze_encoder: bool = True, loss=None, lr: float = 1e-5, betas=(0.9, 0.999),
