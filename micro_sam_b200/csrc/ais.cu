@@ -369,55 +369,14 @@ __global__ void ais_smooth_kernel(const Tin* __restrict__ in, int H, int W, int 
   out[i] = (Tout)acc;
 }
 
-// fg = fg_s > t_fg; marker = cd_s < t_cd && bd_s < t_bd && fg; parent init of the marker components
+// fg = fg_s > t_fg; marker = cd_s < t_cd && bd_s < t_bd && fg, as an int32 0/1 image for the component labelling
 __global__ void ais_masks_kernel(const float* __restrict__ fg, const float* __restrict__ cd, const float* __restrict__ bd, int n,
-                                 float t_fg, float t_cd, float t_bd, uint8_t* __restrict__ fmask, int* __restrict__ parent) {
+                                 float t_fg, float t_cd, float t_bd, uint8_t* __restrict__ fmask, int* __restrict__ marker) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const bool f = fg[i] > t_fg;
   fmask[i] = f;
-  parent[i] = (f && cd[i] < t_cd && bd[i] < t_bd) ? i : -1;
-}
-
-__device__ __forceinline__ int uf_find(volatile int* par, int x) {
-  while (par[x] != x) x = par[x];
-  return x;
-}
-__device__ void uf_unite(int* par, int a, int b) {   // links the larger root under the smaller: every root is its component's
-  while (true) {                                    // first pixel in raster order
-    a = uf_find(par, a);
-    b = uf_find(par, b);
-    if (a == b) return;
-    if (a < b) {
-      const int t = a;
-      a = b;
-      b = t;
-    }
-    if (atomicCAS(par + a, a, b) == a) return;
-  }
-}
-
-__global__ void ais_cc_merge_kernel(int* parent, int H, int W) {   // 8-connectivity through the W, NW, N, NE neighbours
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= H * W || parent[i] < 0) return;
-  const int x = i % W, y = i / W;
-  if (x > 0 && parent[i - 1] >= 0) uf_unite(parent, i, i - 1);
-  if (y > 0) {
-    if (x > 0 && parent[i - W - 1] >= 0) uf_unite(parent, i, i - W - 1);
-    if (parent[i - W] >= 0) uf_unite(parent, i, i - W);
-    if (x < W - 1 && parent[i - W + 1] >= 0) uf_unite(parent, i, i - W + 1);
-  }
-}
-
-__global__ void ais_cc_flatten_kernel(int* parent, int n, int* __restrict__ root_flag) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  int r = parent[i];
-  if (r >= 0) {
-    r = uf_find(parent, i);
-    parent[i] = r;
-  }
-  root_flag[i] = r == i;
+  marker[i] = f && cd[i] < t_cd && bd[i] < t_bd;
 }
 
 // seeds: B = h, label = component id; other foreground pixels: B = +inf, label = INT_MAX; background: B = +inf, label = 0
@@ -840,12 +799,12 @@ int msam_ais_postprocess(const float* fg, const float* cd, const float* bd, int 
   RUN(smooth(bd, H, W, w.taps + MAX_TAPS, r_d, w.tmp, w.bd, st));
   prof_end(st);
   prof_begin(st, "ais markers", 0.0, 0.0);
-  ais_masks_kernel<<<nblk(n), 256, 0, st>>>(w.fg, w.cd, w.bd, n, t_fg, t_cd, t_bd, w.fmask, w.parent);
+  ais_masks_kernel<<<nblk(n), 256, 0, st>>>(w.fg, w.cd, w.bd, n, t_fg, t_cd, t_bd, w.fmask, w.flag);
   LAUNCH_CHECK("ais masks");
-  ais_cc_merge_kernel<<<nblk(n), 256, 0, st>>>(w.parent, H, W);
-  LAUNCH_CHECK("ais cc merge");
-  ais_cc_flatten_kernel<<<nblk(n), 256, 0, st>>>(w.parent, n, w.flag);
-  LAUNCH_CHECK("ais cc flatten");
+  // 8-connected marker components (roots in raster order); the sizes go to cnt and the unread background count to dflag,
+  // both rewritten before their own use below, and flag changes from the marker image to the root flags
+  RUN(post_label_components(w.flag, H, W, w.parent, w.cnt, w.dflag, st, H, 1));
+  RUN(post_flag_components(n, w.parent, w.cnt, 0, w.flag, st));
   RUN(post_inclusive_scan(w.flag, n, w.scan, w.bsums, st));
   ais_ws_init_kernel<<<nblk(n), 256, 0, st>>>(w.parent, w.fmask, w.bd, w.scan, w.bsums, n, w.Bv, w.lab);
   LAUNCH_CHECK("ais watershed init");

@@ -1,4 +1,5 @@
-// Small device helpers shared by the kernel files: bf16 packing, float warp reductions, exact GELU and its derivative, ex2.
+// Small device helpers shared by the kernel files: bf16 packing, float warp reductions, exact GELU and its derivative, ex2,
+// bilinear source indices and a block-local bitonic sort.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -52,6 +53,24 @@ __device__ __forceinline__ void lin_src(int d, float scale, int n, int& i0, int&
   i0 = (int)s;
   i1 = i0 + (i0 < n - 1 ? 1 : 0);
   l1 = s - (float)i0;
+}
+
+// Bitonic sort of keys [npow2] (a power of two) by the nthreads threads of a block, thread tid striding over the keys;
+// descending or ascending.  One __syncthreads() after every merge step, the last of them before the return.
+template <bool kDescending>
+__device__ __forceinline__ void block_bitonic_sort(unsigned long long* keys, int npow2, int tid, int nthreads) {
+  for (int k = 2; k <= npow2; k <<= 1)
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int i = tid; i < npow2; i += nthreads) {
+        const int l = i ^ j;
+        if (l > i) {
+          const unsigned long long a = keys[i], b = keys[l];
+          const bool first = (i & k) == 0;
+          if (kDescending ? (first ? a < b : a > b) : (first ? a > b : a < b)) { keys[i] = b; keys[l] = a; }
+        }
+      }
+      __syncthreads();
+    }
 }
 
 }  // namespace msam

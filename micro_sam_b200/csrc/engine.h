@@ -217,6 +217,8 @@ int post_finish_segmentation(const int32_t* seg, int h, int w, int min_size, int
 // batch of images); conn8: 8-connectivity.
 int post_label_components(const int32_t* seg, int h, int w, int* parent, int* size, int* bg_count, cudaStream_t st, int img_h = 0,
                           int conn8 = 0);
+// flag [n] = 1 at the roots of the components of post_label_components with at least min_size pixels, else 0.
+int post_flag_components(int n, const int* parent, const int* size, int min_size, int* flag, cudaStream_t st);
 // Objects of B label images seg int32 [B, h, w] (ids >= 0, 0 background): apply_label = 1 the 8-connected components of equal
 // non-zero ids, 0 the distinct non-zero ids of each image.  Objects of fewer than min_size pixels become 0; the others are
 // numbered 1.. over the whole batch, image by image, within an image by first pixel in raster order (apply_label = 1) or by

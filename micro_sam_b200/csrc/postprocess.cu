@@ -7,6 +7,7 @@
 //   filter_nms   : AMGBase._postprocess_batch (instance_segmentation.py:99-132): pred-IoU / stability / crop-edge
 //                  filters + torchvision-semantics greedy box NMS, one CTA
 //   paint        : mask_data_to_segmentation's painting loop (util.py:1799-1829)
+#include "device_util.cuh"
 #include "engine.h"
 #include "postgeom.cuh"
 
@@ -323,20 +324,7 @@ filter_nms_kernel(const int32_t* __restrict__ boxes, const float* __restrict__ s
     skey[i] = key;
   }
   __syncthreads();
-  // bitonic sort, descending
-  for (int k = 2; k <= npow2; k <<= 1) {
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int i = tid; i < npow2; i += nt) {
-        const int ixj = i ^ j;
-        if (ixj > i) {
-          const unsigned long long a = skey[i], b = skey[ixj];
-          const bool desc = (i & k) == 0;
-          if (desc ? (a < b) : (a > b)) { skey[i] = b; skey[ixj] = a; }
-        }
-      }
-      __syncthreads();
-    }
-  }
+  block_bitonic_sort<true>(skey, npow2, tid, nt);
   if (tid == 0) { s_cnt = 0; }
   __syncthreads();
   // candidates are the non-zero keys at the front
@@ -682,18 +670,7 @@ paint_min_area_kernel(const float* __restrict__ low_res, const int32_t* __restri
     for (int k = threadIdx.x; k < npow2; k += 256)
       skey[k] = k < n_sel ? (((unsigned long long)(unsigned)area[sel[k]] << 32) | (unsigned)(0xFFFFFFFFu - (unsigned)k)) : ~0ull;
     __syncthreads();
-    for (int kk = 2; kk <= npow2; kk <<= 1) {
-      for (int j = kk >> 1; j > 0; j >>= 1) {
-        for (int i = threadIdx.x; i < npow2; i += 256) {
-          const int ixj = i ^ j;
-          if (ixj > i) {
-            const unsigned long long a = skey[i], b = skey[ixj];
-            if (((i & kk) == 0) ? (a > b) : (a < b)) { skey[i] = b; skey[ixj] = a; }
-          }
-        }
-        __syncthreads();
-      }
-    }
+    block_bitonic_sort<false>(skey, npow2, threadIdx.x, 256);
     if (x >= g.out_w) return;
     int best_pos = -1;
     for (int k = 0; k < n_sel; ++k) {
@@ -745,18 +722,7 @@ paint_min_area_x4_kernel(const float* __restrict__ low_res, const int32_t* __res
     for (int k = tid; k < npow2; k += 256)
       skey[k] = k < n_sel ? (((unsigned long long)(unsigned)area[sel[k]] << 32) | (unsigned)(0xFFFFFFFFu - (unsigned)k)) : ~0ull;
     __syncthreads();
-    for (int kk = 2; kk <= npow2; kk <<= 1) {
-      for (int j = kk >> 1; j > 0; j >>= 1) {
-        for (int i = tid; i < npow2; i += 256) {
-          const int ixj = i ^ j;
-          if (ixj > i) {
-            const unsigned long long a = skey[i], b = skey[ixj];
-            if (((i & kk) == 0) ? (a > b) : (a < b)) { skey[i] = b; skey[ixj] = a; }
-          }
-        }
-        __syncthreads();
-      }
-    }
+    block_bitonic_sort<false>(skey, npow2, tid, 256);
     // Candidates of THIS region, in sorted order: survivors whose box misses the 32 x 32 region are dropped up front (with
     // localised masks a region sees a handful of the survivors instead of all of them).  Order-preserving compaction:
     // ballot words -> exclusive scan of their popcounts by warp 0 -> scatter.
@@ -862,6 +828,18 @@ int post_paint_min_area(const float* low_res, const int32_t* sel, const int32_t*
 // (4-connectivity; union-find with atomicMin roots, so a component's root is its first pixel in raster order), size
 // filter, optional removal of the largest segment (`with_background`; the unlabelled area counts as segment 0 exactly
 // like np.unique), consecutive relabelling in raster order of the roots.
+// The labelling kernels read pixels through one of two accessors: an int32 label image, or a uint8 mask whose non-zero
+// pixels (invert = 0) or zero pixels (invert = 1) are labelled as 1.  __ldg: the pixels are read-only for the kernel's life
+// (__restrict__ on a struct member would not be honoured).
+struct LabelPixels {
+  const int32_t* p;
+  __device__ __forceinline__ int operator[](int i) const { return __ldg(p + i); }
+};
+struct MaskPixels {
+  const uint8_t* p;
+  int invert;
+  __device__ __forceinline__ int operator[](int i) const { return (__ldg(p + i) != 0) != invert; }
+};
 __device__ __forceinline__ int uf_find(int* parent, int i) {
   int p = parent[i];
   while (p != i) { i = p; p = parent[i]; }
@@ -881,7 +859,8 @@ __device__ __forceinline__ void uf_union(int* parent, int a, int b) {
 // Initial forest: every pixel points at the first pixel of its horizontal run inside the warp's 32-pixel segment (found with
 // one ballot), so the union phase starts from runs instead of single pixels: the chains that uf_find walks are 32x shorter
 // and most horizontal unions disappear.  (Roots stay the smallest index of their set, as the relabelling order requires.)
-__global__ void cc_init_kernel(const int32_t* __restrict__ seg, int n, int w, int* __restrict__ parent, int* __restrict__ size) {
+template <class Pixels>
+__global__ void cc_init_kernel(Pixels seg, int n, int w, int* __restrict__ parent, int* __restrict__ size) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int lane = threadIdx.x & 31;
   const int s = i < n ? seg[i] : 0;
@@ -900,7 +879,8 @@ __global__ void cc_init_kernel(const int32_t* __restrict__ seg, int n, int w, in
 // pixel's own link), i.e. at the first column of every vertical contact between two runs.
 // conn8 adds the diagonal links that the horizontal and vertical ones do not imply.  Rows y and y + 1 are linked only inside
 // one image of img_h rows (a batch of images stacked along the rows).
-__global__ void cc_merge_kernel(const int32_t* __restrict__ seg, int h, int w, int img_h, int conn8, int* __restrict__ parent) {
+template <class Pixels>
+__global__ void cc_merge_kernel(Pixels seg, int h, int w, int img_h, int conn8, int* __restrict__ parent) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= h * w) return;
   const int s = seg[i];
@@ -1017,8 +997,8 @@ __global__ void cc_relabel_kernel(int n, const int* __restrict__ parent, const i
   out[i] = v;
 }
 
-int post_label_components(const int32_t* seg, int h, int w, int* parent, int* size, int* bg_count, cudaStream_t st, int img_h,
-                          int conn8) {
+template <class Pixels>
+int label_components(Pixels seg, int h, int w, int* parent, int* size, int* bg_count, cudaStream_t st, int img_h, int conn8) {
   const int n = h * w;
   const unsigned blocks = (unsigned)((n + 255) / 256);
   cc_init_kernel<<<blocks, 256, 0, st>>>(seg, n, w, parent, size);
@@ -1027,6 +1007,16 @@ int post_label_components(const int32_t* seg, int h, int w, int* parent, int* si
   LAUNCH_CHECK("cc_merge");
   cc_flatten_count_kernel<<<blocks, 256, 0, st>>>(n, parent, size, bg_count);
   LAUNCH_CHECK("cc_flatten");
+  return 0;
+}
+int post_label_components(const int32_t* seg, int h, int w, int* parent, int* size, int* bg_count, cudaStream_t st, int img_h,
+                          int conn8) {
+  return label_components(LabelPixels{seg}, h, w, parent, size, bg_count, st, img_h, conn8);
+}
+
+int post_flag_components(int n, const int* parent, const int* size, int min_size, int* flag, cudaStream_t st) {
+  cc_flag_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, parent, size, min_size, 0, nullptr, nullptr, flag);
+  LAUNCH_CHECK("cc_flag");
   return 0;
 }
 
@@ -1138,8 +1128,7 @@ int post_label_objects(const int32_t* seg, int B, int h, int w, int apply_label,
   if (apply_label) {
     cudaMemsetAsync(bg, 0, sizeof(int), st);
     RUN(post_label_components(seg, B * h, w, parent, size, bg, st, h, 1));
-    cc_flag_kernel<<<blocks, 256, 0, st>>>(n, parent, size, min_size, 0, nullptr, nullptr, flag);
-    LAUNCH_CHECK("label_objects_flag");
+    RUN(post_flag_components(n, parent, size, min_size, flag, st));
   } else {
     unsigned long long* keys = (unsigned long long*)((char*)ws + post_label_objects_ws(B, h, w, 1));
     const long cap = post_label_objects_cap(B, h, w);
@@ -1282,17 +1271,7 @@ matrix_nms_kernel(const float* __restrict__ m, const float* __restrict__ scores,
   for (int i = tid; i < npow2; i += nt)
     skey[i] = i < n ? (((unsigned long long)orderable(scores[i]) << 32) | (unsigned long long)(0xFFFFFFFFu - (uint32_t)i)) : 0ull;
   __syncthreads();
-  for (int k = 2; k <= npow2; k <<= 1)
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int i = tid; i < npow2; i += nt) {
-        const int ixj = i ^ j;
-        if (ixj > i) {
-          const unsigned long long a = skey[i], b = skey[ixj];
-          if (((i & k) == 0) ? (a < b) : (a > b)) { skey[i] = b; skey[ixj] = a; }
-        }
-      }
-      __syncthreads();
-    }
+  block_bitonic_sort<true>(skey, npow2, tid, nt);
   for (int i = tid; i < n; i += nt) alive[i] = 1;
   if (tid == 0) s_cnt = 0;
   __syncthreads();
@@ -1455,54 +1434,22 @@ int post_local_otsu(const float* low_res, int n, float* thr_out, cudaStream_t st
 // min_mask_region_area > 0 (AMGBase._postprocess_small_regions, instance_segmentation.py:146-186; the per-mask work is
 // segment_anything.utils.amg.remove_small_regions: cv2.connectedComponentsWithStats(8-connectivity) on the mask ("islands")
 // or its complement ("holes"), components below `area_thresh` are removed / filled; if every island is small the largest
-// one (first in raster order on ties, like np.argmax over cv2's raster-ordered labels) is kept).  Batched over masks
-// (blockIdx.y), union-find with atomicMin roots as in the label-image CC above, 8-connectivity.
+// one (first in raster order on ties, like np.argmax over cv2's raster-ordered labels) is kept).  The masks of a pass are
+// labelled as one image of n * h rows by label_components (8-connectivity, no links between masks), so mask m's roots
+// are its first pixels in raster order offset by m * h * w, and the per-mask kernels below run on blockIdx.y = m.
 namespace msam {
 
-__global__ void rsr_init_kernel(const uint8_t* __restrict__ masks, long npix, int holes, int* __restrict__ parent,
-                                int* __restrict__ size) {
-  const long m = blockIdx.y;
-  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= npix) return;
-  const bool working = (masks[m * npix + i] != 0) != (holes != 0);
-  parent[m * npix + i] = working ? (int)i : -1;
-  size[m * npix + i] = 0;
-}
-__global__ void rsr_merge_kernel(int h, int w, int* __restrict__ parent_all) {
-  const long m = blockIdx.y;
-  const long npix = (long)h * w;
-  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= npix) return;
-  int* parent = parent_all + m * npix;
-  if (parent[i] < 0) return;
-  const int x = (int)(i % w), y = (int)(i / w);
-  if (x + 1 < w && parent[i + 1] >= 0) uf_union(parent, (int)i, (int)i + 1);
-  if (y + 1 < h) {
-    if (parent[i + w] >= 0) uf_union(parent, (int)i, (int)(i + w));
-    if (x + 1 < w && parent[i + w + 1] >= 0) uf_union(parent, (int)i, (int)(i + w + 1));
-    if (x > 0 && parent[i + w - 1] >= 0) uf_union(parent, (int)i, (int)(i + w - 1));
-  }
-}
-__global__ void rsr_flatten_kernel(long npix, int* __restrict__ parent_all, int* __restrict__ size_all) {
-  const long m = blockIdx.y;
-  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= npix) return;
-  int* parent = parent_all + m * npix;
-  if (parent[i] < 0) return;
-  const int r = uf_find(parent, (int)i);
-  parent[i] = r;
-  atomicAdd(&size_all[m * npix + r], 1);
-}
 // per-mask statistics: st[0] = #small components, st[1] = #large components, best = packed (size, ~root) maximum
 __global__ void rsr_stats_kernel(long npix, const int* __restrict__ parent_all, const int* __restrict__ size_all, int area_thresh,
                                  int* __restrict__ st, unsigned long long* __restrict__ best) {
   const long m = blockIdx.y;
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= npix) return;
-  if (parent_all[m * npix + i] != (int)i) return;
-  const int s = size_all[m * npix + i];
+  const long r = m * npix + i;
+  if (parent_all[r] != (int)r) return;
+  const int s = size_all[r];
   atomicAdd(&st[2 * m + (s < area_thresh ? 0 : 1)], 1);
-  atomicMax(&best[m], ((unsigned long long)(unsigned)s << 32) | (unsigned)(~(unsigned)i));
+  atomicMax(&best[m], ((unsigned long long)(unsigned)s << 32) | (unsigned)(~(unsigned)r));
 }
 __global__ void rsr_apply_kernel(uint8_t* __restrict__ masks, long npix, int holes, const int* __restrict__ parent_all,
                                  const int* __restrict__ size_all, int area_thresh, const int* __restrict__ st,
@@ -1513,43 +1460,45 @@ __global__ void rsr_apply_kernel(uint8_t* __restrict__ masks, long npix, int hol
   if (i >= npix || st[2 * m] == 0) return;  // no small component: the mask is returned unchanged
   const int r = parent_all[m * npix + i];
   if (holes) {
-    if (r >= 0 && size_all[m * npix + r] < area_thresh) masks[m * npix + i] = 1;   // fill the small holes
+    if (r >= 0 && size_all[r] < area_thresh) masks[m * npix + i] = 1;   // fill the small holes
   } else {
     bool keep = false;
     if (r >= 0) {
-      if (st[2 * m + 1] > 0) keep = size_all[m * npix + r] >= area_thresh;
-      else keep = r == (int)(~(unsigned)(best[m] & 0xffffffffu));                  // every island is small: keep the largest
+      if (st[2 * m + 1] > 0) keep = size_all[r] >= area_thresh;
+      else keep = r == (int)(~(unsigned)(best[m] & 0xffffffffu));        // every island is small: keep the largest
     }
     masks[m * npix + i] = keep ? 1 : 0;
   }
 }
 
-// masks [n, h, w] uint8 (0/1) in place; changed [n]; ws: n * (2*h*w) ints + n * 4 ints
+// masks [n, h, w] uint8 (0/1) in place; changed [n]; ws: n * (2*h*w) ints + n * 4 ints.  The labeller indexes with int32,
+// so the masks go in passes of at most `group` masks.
 int post_remove_small_regions(uint8_t* masks, int n, int h, int w, int area_thresh, int holes, int32_t* changed, int32_t* ws,
                               cudaStream_t st) {
   if (n <= 0) return 0;
-  const long npix = (long)h * w;
-  if (npix >= (1l << 31)) return set_error("remove_small_regions: image too large");
+  const long npix = (long)h * w, lim = (1l << 31) - 1024;
+  if (h <= 0 || w <= 0 || npix >= lim) return set_error("remove_small_regions: image of %d x %d pixels", h, w);
+  const int group = (int)std::min<long>(n, (lim - 1) / npix);
   int* parent = ws;
   int* size = ws + (size_t)n * npix;
   int* stats = ws + 2 * (size_t)n * npix;
   unsigned long long* best = reinterpret_cast<unsigned long long*>(stats + 2 * n);  // 2n ints: 8-byte aligned with ws
+  // stats[0] takes the labeller's background count, which nothing reads, before the block is zeroed
+  for (int m0 = 0; m0 < n; m0 += group)
+    RUN(label_components(MaskPixels{masks + m0 * npix, holes != 0}, std::min(group, n - m0) * h, w, parent + m0 * npix,
+                         size + m0 * npix, stats, st, h, 1));
   cudaMemsetAsync(stats, 0, (size_t)n * 4 * sizeof(int), st);
-  const dim3 grid((unsigned)((npix + 255) / 256), n);
-  rsr_init_kernel<<<grid, 256, 0, st>>>(masks, npix, holes, parent, size);
-  LAUNCH_CHECK("rsr_init");
-  rsr_merge_kernel<<<grid, 256, 0, st>>>(h, w, parent);
-  LAUNCH_CHECK("rsr_merge");
-  rsr_flatten_kernel<<<grid, 256, 0, st>>>(npix, parent, size);
-  LAUNCH_CHECK("rsr_flatten");
-  rsr_stats_kernel<<<grid, 256, 0, st>>>(npix, parent, size, area_thresh, stats, best);
-  LAUNCH_CHECK("rsr_stats");
-  rsr_apply_kernel<<<grid, 256, 0, st>>>(masks, npix, holes, parent, size, area_thresh, stats, best, changed);
-  LAUNCH_CHECK("rsr_apply");
+  for (int m0 = 0; m0 < n; m0 += group) {
+    const dim3 grid((unsigned)((npix + 255) / 256), std::min(group, n - m0));
+    rsr_stats_kernel<<<grid, 256, 0, st>>>(npix, parent + m0 * npix, size + m0 * npix, area_thresh, stats + 2 * m0, best + m0);
+    LAUNCH_CHECK("rsr_stats");
+    rsr_apply_kernel<<<grid, 256, 0, st>>>(masks + m0 * npix, npix, holes, parent + m0 * npix, size + m0 * npix, area_thresh,
+                                           stats + 2 * m0, best + m0, changed + m0);
+    LAUNCH_CHECK("rsr_apply");
+  }
   return 0;
 }
 
-// batched_mask_to_box (_vendored.py:33-85) + area for materialised uint8 masks [n, h, w]: one CTA per mask
 __global__ void __launch_bounds__(256)
 mask_box_kernel(const uint8_t* __restrict__ masks, int h, int w, int32_t* __restrict__ boxes, int32_t* __restrict__ area) {
   const long m = blockIdx.x;

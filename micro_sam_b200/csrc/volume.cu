@@ -18,6 +18,7 @@
 #include <cmath>
 #include <utility>
 
+#include "device_util.cuh"
 #include "engine.h"
 
 namespace msam {
@@ -358,18 +359,7 @@ __global__ void peak_thin_kernel(const int64_t* st, int32_t* ctr, unsigned long 
   const unsigned long long* cand = cand_all + (long)which * kMaxCand;
   for (int i = threadIdx.x; i < np2; i += blockDim.x) s_k[i] = i < n ? cand[i] : 0ull;
   __syncthreads();
-  for (int k = 2; k <= np2; k <<= 1)            // bitonic sort, descending
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int i = threadIdx.x; i < np2; i += blockDim.x) {
-        const int l = i ^ j;
-        if (l > i) {
-          const bool desc = (i & k) == 0;
-          const unsigned long long a = s_k[i], b = s_k[l];
-          if (desc ? a < b : a > b) { s_k[i] = b; s_k[l] = a; }
-        }
-      }
-      __syncthreads();
-    }
+  block_bitonic_sort<true>(s_k, np2, threadIdx.x, blockDim.x);
   int32_t* kept = kept_all + (long)which * kMaxCand;
   __shared__ int s_nk;
   __shared__ int s_ok;
