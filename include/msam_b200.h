@@ -265,9 +265,19 @@ int msam_encode_backward(msam_handle* h, const float* d_out_nchw, void* stream);
  * [P, n_sparse, 256] (msam_prompt_encode), emb_index [P, n_sparse] int32 = the embedding-table row behind each sparse token (0..3 =
  * point_embeddings.{0..3}, 4 = not_a_point_embed) so that their gradients can be formed; the dense prompt is no_mask_embed.
  * backward: d_low_res [P, M, 256, 256] / d_iou [P, M] (either may be NULL) -> parameter gradients ACCUMULATE (msam_decoder_zero_grads),
- * d_emb_nchw [256, 64, 64] = dL/d(image embedding) is overwritten. */
+ * d_emb_nchw = dL/d(image embedding) is overwritten: [256, 64, 64] for a slot of msam_decoder_train_forward(_ex), [B, 256, 64, 64]
+ * (one gradient per image, not summed) for a slot of msam_decoder_train_forward_images. */
 int msam_decoder_train_forward(msam_handle* h, int slot, const float* emb_nchw, const float* sparse, const int32_t* emb_index, int n_sparse,
                                int P, int multimask, float* low_res, float* iou, void* stream);
+/* Prompt-free training decode of B images in one slot (micro_sam's SemanticSamTrainer: no prompts, so the sparse embeddings are
+ * empty and the dense prompt is no_mask_embed): emb_nchw [B, 256, 64, 64] -> low_res [B, M, 256, 256], iou [B, M], one prompt of the
+ * 5 output tokens per image, image b keyed by its own embedding.  Its backward gives no_mask_embed a gradient and none to
+ * point_embeddings.*, not_a_point_embed or mask_downscaling.*.  While only such backwards have run since the last
+ * msam_decoder_zero_grads, msam_optimizer_step skips (masters, moments and update counts untouched) the tensors a prompt-free loss
+ * cannot reach: iou_prediction_head.*, point_embeddings.*, not_a_point_embed and mask_downscaling.*; once any other backward has
+ * run, the step updates every tensor as before. */
+int msam_decoder_train_forward_images(msam_handle* h, int slot, const float* emb_nchw, int B, int multimask, float* low_res, float* iou,
+                                      void* stream);
 int msam_decoder_train_backward(msam_handle* h, int slot, const float* d_low_res, const float* d_iou, float* d_emb_nchw, void* stream);
 /* msam_decoder_train_forward with mask prompts: mask_input [P, 1, 256, 256] fp32 low-res logits (PromptEncoder._embed_masks), or NULL
  * (= msam_decoder_train_forward).  The dense prompt is then mask_downscaling(mask_input) instead of no_mask_embed.  The first call with

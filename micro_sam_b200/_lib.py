@@ -118,6 +118,7 @@ def lib() -> ctypes.CDLL:
                                                  c_void_p]
         L.msam_decoder_train_forward_ex.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p,
                                                     c_void_p, c_void_p]
+        L.msam_decoder_train_forward_images.argtypes = [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]
         L.msam_op_mask_downscaling_train.argtypes = [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
         L.msam_decoder_train_backward.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
         L.msam_decoder_zero_grads.argtypes = [c_void_p, c_void_p]

@@ -10,7 +10,9 @@
 // and pushes its backward closure; backward() replays the closures in reverse.  Tensors carry an fp32 value, an fp32 gradient
 // (accumulated: every consumer ADDS) and a bf16 copy (the GEMM operand).  Parameter gradients accumulate across calls (images,
 // sub-iterations) until msam_decoder_zero_grads.  Prompts: points and / or boxes, with the dense prompt no_mask_embed or, for mask
-// prompts, mask_downscaling(mask) (md_* kernels: fp32, taped by keeping the mask; no gradient w.r.t. the mask itself).
+// prompts, mask_downscaling(mask) (md_* kernels: fp32, taped by keeping the mask; no gradient w.r.t. the mask itself).  A
+// prompt-free batch (semantic training, micro_sam/training/semantic_sam_trainer.py) runs B images as B prompts of 5 tokens in one
+// slot, prompt p keyed by image p (src_images_* kernels); its backward writes dL/d embedding per image.
 #include "device_util.cuh"
 #include "engine.h"
 
@@ -140,6 +142,32 @@ __global__ void src_grad_kernel(const float* __restrict__ g, int P, float* __res
   }
   __syncthreads();
   for (int i = threadIdx.y; i < 32; i += blockDim.y) d_emb_nchw[(long)(c0 + i) * 4096 + pix0 + threadIdx.x] = tile[threadIdx.x][i];
+  if (threadIdx.y == 0) {
+    float s = 0.f;
+    for (int i = 0; i < 32; ++i) s += tile[i][threadIdx.x];
+    atomicAdd(g_no_mask + c0 + threadIdx.x, s);
+  }
+}
+// Prompt-free batches (one prompt per image): keys0[p, pix, c] = emb_nchw[p, c, pix] + no_mask[c].  grid = (128, 8, P)
+__global__ void src_images_kernel(const float* __restrict__ emb_nchw, const float* __restrict__ no_mask, float* __restrict__ out) {
+  __shared__ float tile[32][33];
+  const int pix0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
+  const long p = blockIdx.z;
+  const float* e = emb_nchw + p * 256 * 4096;
+  for (int i = threadIdx.y; i < 32; i += blockDim.y) tile[i][threadIdx.x] = e[(long)(c0 + i) * 4096 + pix0 + threadIdx.x];
+  __syncthreads();
+  for (int i = threadIdx.y; i < 32; i += blockDim.y)
+    out[(p * 4096 + pix0 + i) * 256 + c0 + threadIdx.x] = tile[threadIdx.x][i] + no_mask[c0 + threadIdx.x];
+}
+// d_emb_nchw[p, c, pix] = g[p, pix, c] (per image, not summed);  g_no_mask[c] += sum_{p, pix} g[p, pix, c].  grid = (128, 8, P)
+__global__ void src_images_grad_kernel(const float* __restrict__ g, float* __restrict__ d_emb_nchw, float* __restrict__ g_no_mask) {
+  __shared__ float tile[32][33];
+  const int pix0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
+  const long p = blockIdx.z;
+  for (int i = threadIdx.y; i < 32; i += blockDim.y) tile[i][threadIdx.x] = g[(p * 4096 + pix0 + i) * 256 + c0 + threadIdx.x];
+  __syncthreads();
+  float* d = d_emb_nchw + p * 256 * 4096;
+  for (int i = threadIdx.y; i < 32; i += blockDim.y) d[(long)(c0 + i) * 4096 + pix0 + threadIdx.x] = tile[threadIdx.x][i];
   if (threadIdx.y == 0) {
     float s = 0.f;
     for (int i = 0; i < 32; ++i) s += tile[i][threadIdx.x];
@@ -528,6 +556,7 @@ struct DecSlot {
   size_t cap = 0, used = 0;
   std::vector<std::function<int(cudaStream_t)>> tape;
   int P = 0, T = 0, Ts = 0, nm = 0, m0 = 0;
+  bool images = false;               // prompt-free batch: prompt p is image p with no sparse tokens (msam_decoder_train_forward_images)
   Ten low4, iou32, keys0, tok;
   int* emb_index = nullptr;
   __nv_bfloat16* dmask8 = nullptr;
@@ -549,6 +578,9 @@ struct DecTrain {
   float *md_w = nullptr, *md_g = nullptr;
   bool md_registered = false;
   bool md_written = false;           // a masked backward added to md_g since the last msam_decoder_zero_grads
+  // Since the last msam_decoder_zero_grads: a backward of a prompt-free batch / of a prompted slot has run.  unreached = only
+  // prompt-free ones: the IoU head and the sparse-prompt tables then have no gradient, and AdamW skips them (OptParam::skip).
+  bool free_written = false, prompted_written = false, unreached = false;
 };
 
 namespace {
@@ -888,6 +920,12 @@ int Engine::dec_train_setup() {
     p.key = m + "iou_token.weight"; p.w = d.out_tokens; p.g = d.g_out_tokens; p.n = 256; CHK(train_add(p));
     p.key = m + "mask_tokens.weight"; p.w = d.out_tokens + 256; p.g = d.g_out_tokens + 256; p.n = 4 * 256; CHK(train_add(p));
     p.key = "prompt_encoder.no_mask_embed.weight"; p.w = d.no_mask; p.g = nullptr; p.n = 256; CHK(d.g_no_mask = train_add(p));
+    // what a prompt-free batch cannot reach (its loss ignores the IoU predictions; no sparse tokens): torch leaves their .grad None
+    // after such backwards only, and AdamW skips them (mask_downscaling is skipped through md_written)
+    for (OptParam& q : opt)
+      if (q.key.rfind(m + "iou_prediction_head.", 0) == 0 || q.key.rfind("prompt_encoder.point_embeddings.", 0) == 0 ||
+          q.key == "prompt_encoder.not_a_point_embed.weight")
+        q.skip = &d.unreached;
     return 0;
   };
   rc = go();
@@ -964,6 +1002,21 @@ int Engine::decoder_train_forward(int slot, const float* emb_nchw, const float* 
   if (slot < 0 || slot >= 8) return set_error("decoder training: slot %d outside [0, 8)", slot);
   if (P <= 0 || Ts <= 0 || !sparse || !emb_index) return set_error("decoder training: needs sparse prompt embeddings (points and / or boxes)");
   if (5 + Ts > 64) return set_error("decoder training: %d tokens per prompt exceeds the supported 64", 5 + Ts);
+  return dec_train_run(slot, emb_nchw, sparse, emb_index, Ts, P, mask_in, false, multimask, low_res, iou, st);
+}
+
+int Engine::decoder_train_forward_images(int slot, const float* emb_nchw, int B, int multimask, float* low_res, float* iou,
+                                         cudaStream_t st) {
+  if (slot < 0 || slot >= 8) return set_error("decoder training: slot %d outside [0, 8)", slot);
+  if (B <= 0) return set_error("decoder training: B = %d images", B);
+  return dec_train_run(slot, emb_nchw, nullptr, nullptr, 0, B, nullptr, true, multimask, low_res, iou, st);
+}
+
+// The tape of one slot.  images = false: P prompts of ONE image (Ts sparse tokens each, dense prompt no_mask_embed or
+// mask_downscaling(mask_in)); images = true: P images with no prompt (T = 5 output tokens, dense prompt no_mask_embed), prompt p
+// reading image p.  Every op after the keys is per prompt either way.
+int Engine::dec_train_run(int slot, const float* emb_nchw, const float* sparse, const int* emb_index, int Ts, int P,
+                          const float* mask_in, bool images, int multimask, float* low_res, float* iou, cudaStream_t st) {
   RUN(dec_train_setup());
   if (mask_in) RUN(md_register());
   DecTrain& d = *dtrain;
@@ -981,11 +1034,13 @@ int Engine::decoder_train_forward(int slot, const float* emb_nchw, const float* 
     }
   }
   s.used = 0; s.tape.clear(); s.live = false; s.mask = nullptr;
-  s.P = P; s.T = T; s.Ts = Ts; s.nm = multimask ? 3 : 1; s.m0 = multimask ? 1 : 0;
+  s.P = P; s.T = T; s.Ts = Ts; s.nm = multimask ? 3 : 1; s.m0 = multimask ? 1 : 0; s.images = images; s.emb_index = nullptr;
   Ctx c{*this, d, s, st};
-  s.emb_index = (int*)c.take((size_t)P * Ts * 4);
-  if (c.err) return -1;
-  if (cudaMemcpyAsync(s.emb_index, emb_index, (size_t)P * Ts * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess) return set_error("decoder training: copy failed");
+  if (Ts > 0) {
+    s.emb_index = (int*)c.take((size_t)P * Ts * 4);
+    if (c.err) return -1;
+    if (cudaMemcpyAsync(s.emb_index, emb_index, (size_t)P * Ts * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess) return set_error("decoder training: copy failed");
+  }
   // tokens and image-side source
   Ten tok = c.ten(Rt, 256, true, true, true);
   Ten keys0 = c.ten(Ri, 256, true, true, true);
@@ -1001,6 +1056,10 @@ int Engine::decoder_train_forward(int slot, const float* emb_nchw, const float* 
     if (cudaMemcpyAsync(s.mask, mask_in, (size_t)P * 65536 * 4, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
       return set_error("decoder training: copy failed");
     RUN(md_forward(s.mask, P, d.md_w, emb_nchw, keys0.v, keys0.b, s.md, st));
+  } else if (images) {
+    src_images_kernel<<<dim3(128, 8, P), dim3(32, 8), 0, st>>>(emb_nchw, d.no_mask, keys0.v);
+    LAUNCH_CHECK("src_images");
+    RUN(launch_cast_bf16(keys0.v, keys0.n(), keys0.b, st));
   } else {
     src_broadcast_kernel<<<dim3(128, 8), dim3(32, 8), 0, st>>>(emb_nchw, d.no_mask, P, keys0.v);
     LAUNCH_CHECK("src_broadcast");
@@ -1133,10 +1192,15 @@ int Engine::decoder_train_backward(int slot, const float* d_low_res, const float
   if (s.mask) {
     RUN(md_backward(s.keys0.g, s.mask, P, d.md_w, d_emb_nchw, s.md, d.md_g, 1, st));
     d.md_written = true;
+  } else if (s.images) {
+    src_images_grad_kernel<<<dim3(128, 8, P), dim3(32, 8), 0, st>>>(s.keys0.g, d_emb_nchw, d.g_no_mask);
+    LAUNCH_CHECK("src_images_grad");
   } else {
     src_grad_kernel<<<dim3(128, 8), dim3(32, 8), 0, st>>>(s.keys0.g, P, d_emb_nchw, d.g_no_mask);
     LAUNCH_CHECK("src_grad");
   }
+  (s.images ? d.free_written : d.prompted_written) = true;
+  d.unreached = d.free_written && !d.prompted_written;
   s.live = false;   // gradients of the activations are consumed: one backward per forward
   return 0;
 }
@@ -1153,7 +1217,7 @@ int Engine::decoder_zero_grads(cudaStream_t st) {
   if (!dtrain) return 0;
   for (const OptParam& p : opt)
     if (p.decoder && cudaMemsetAsync(p.g, 0, (size_t)p.n * 4, st) != cudaSuccess) return set_error("decoder training: memset failed");
-  dtrain->md_written = false;
+  dtrain->md_written = dtrain->free_written = dtrain->prompted_written = dtrain->unreached = false;
   return 0;
 }
 

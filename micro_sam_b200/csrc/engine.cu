@@ -878,6 +878,11 @@ int msam_decoder_train_forward_ex(msam_handle* h, int slot, const float* emb_nch
   return h->eng.decoder_train_forward(slot, emb_nchw, sparse, emb_index, n_sparse, P, mask_input, multimask, low_res, iou,
                                       (cudaStream_t)stream);
 }
+int msam_decoder_train_forward_images(msam_handle* h, int slot, const float* emb_nchw, int B, int multimask, float* low_res, float* iou,
+                                      void* stream) {
+  if (!h || !emb_nchw || !low_res || !iou) return set_error("msam_decoder_train_forward_images: null argument");
+  return h->eng.decoder_train_forward_images(slot, emb_nchw, B, multimask, low_res, iou, (cudaStream_t)stream);
+}
 int msam_op_mask_downscaling_train(msam_handle* h, const float* mask, int P, const float* d_dense, float* dense_out, float* grads_out,
                                    void* stream) {
   if (!h || !mask || !d_dense || !dense_out || !grads_out) return set_error("msam_op_mask_downscaling_train: null argument");

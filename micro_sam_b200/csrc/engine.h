@@ -95,6 +95,7 @@ struct OptParam {
   bool decoder = false;           // the gradient accumulates until msam_decoder_zero_grads; else msam_encode_backward overwrites it
   const bool* written = nullptr;  // non-null: AdamW skips the tensor while *written is false (no gradient since the last zeroing)
   int64_t steps = 0;              // ... and counts its own steps for the bias correction (with written only)
+  const bool* skip = nullptr;     // non-null: AdamW skips the tensor while *skip is true (its upstream .grad would be None)
   int64_t count = 0;              // updates of the tensor; the bias correction once a subset step has run (per_tensor_counts)
   Refresh refresh = Refresh::None;
   __nv_bfloat16 *dst = nullptr;
@@ -160,6 +161,10 @@ struct Engine {
   int dec_train_setup();
   int decoder_train_forward(int slot, const float* emb_nchw, const float* sparse, const int* emb_index, int Ts, int P,
                             const float* mask_in, int multimask, float* low_res, float* iou, cudaStream_t st);
+  // B images with no prompts in one slot (one prompt of 5 tokens per image)
+  int decoder_train_forward_images(int slot, const float* emb_nchw, int B, int multimask, float* low_res, float* iou, cudaStream_t st);
+  int dec_train_run(int slot, const float* emb_nchw, const float* sparse, const int* emb_index, int Ts, int P, const float* mask_in,
+                    bool images, int multimask, float* low_res, float* iou, cudaStream_t st);
   int decoder_train_backward(int slot, const float* d_low_res, const float* d_iou, float* d_emb_nchw, cudaStream_t st);
   int decoder_zero_grads(cudaStream_t st);
   int dec_train_refresh_prompt_tables(cudaStream_t st);   // the inference prompt encoder's tables <- the training masters

@@ -63,8 +63,11 @@ int Engine::optimizer_step(float lr, float b1, float b2, float eps, float wd, cu
   else ++opt_step_count;
   const float c1 = 1.f - powf(b1, (float)opt_step_count), c2 = 1.f - powf(b2, (float)opt_step_count);
   const size_t plen = prefix ? strlen(prefix) : 0;
+  for (const OptParam& p : opt)   // a skipped tensor falls behind the step count: from now on each tensor counts its own updates
+    if (p.skip && *p.skip) per_tensor_counts = true;
   for (OptParam& p : opt) {
     if (prefix && p.key.compare(0, plen, prefix) != 0) continue;
+    if (p.skip && *p.skip) continue;
     float c1p = c1, c2p = c2;
     if (p.written) {
       if (!*p.written) continue;

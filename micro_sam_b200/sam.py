@@ -183,6 +183,33 @@ class _DecoderFn(torch.autograd.Function):
         return d_emb, None, None, None, None, None, None
 
 
+class _ImagesDecoderFn(torch.autograd.Function):
+    """mask decoder of B images with no prompts in one slot (msam_decoder_train_forward_images): embeddings [B,256,64,64] ->
+    (low-res logits [B,M,256,256], IoU predictions [B,M]).  backward accumulates the decoder parameter gradients in the engine and
+    returns dL/d embedding per image."""
+
+    @staticmethod
+    def forward(ctx, embs, sam, slot, multimask):
+        embs = embs.to(device=sam.device, dtype=torch.float32).contiguous()
+        B, M = embs.shape[0], 3 if multimask else 1
+        low = torch.empty(B, M, 256, 256, device=sam.device, dtype=torch.float32)
+        iou = torch.empty(B, M, device=sam.device, dtype=torch.float32)
+        _lib.check(_lib.lib().msam_decoder_train_forward_images(sam._h, slot, _lib.ptr(embs), B, int(bool(multimask)), _lib.ptr(low),
+                                                                _lib.ptr(iou), _lib.cur_stream()))
+        ctx.sam, ctx.slot, ctx.B = sam, slot, B
+        return low, iou
+
+    @staticmethod
+    def backward(ctx, d_low, d_iou):
+        sam = ctx.sam
+        d_low = None if d_low is None else d_low.to(torch.float32).contiguous()
+        d_iou = None if d_iou is None else d_iou.to(torch.float32).contiguous()
+        d_emb = torch.empty(ctx.B, 256, 64, 64, device=sam.device, dtype=torch.float32)
+        _lib.check(_lib.lib().msam_decoder_train_backward(sam._h, ctx.slot, _lib.ptr(d_low), _lib.ptr(d_iou), _lib.ptr(d_emb), _lib.cur_stream()))
+        sam._decoder_grads_valid = True
+        return d_emb, None, None, None
+
+
 class _ImageEncoder:
     """Callable stand-in for `sam.image_encoder`: (B,3,1024,1024) fp32 preprocessed -> (B,256,64,64) fp32."""
 
@@ -414,6 +441,24 @@ class B200Sam:
         emb_index = prompt_table_index(None if points is None else points[1], boxes is not None, P).to(self.device)
         assert emb_index.shape == sparse.shape[:2], (emb_index.shape, sparse.shape)
         return _DecoderFn.apply(emb, sparse, emb_index, self, int(slot), bool(multimask_output), masks)
+
+    def decoder_train_images(self, embs: torch.Tensor, multimask_output: bool, slot: int = 0):
+        """mask_decoder(prompt_encoder()) of B images with no prompts, in training mode and in ONE decoder slot: differentiable
+        w.r.t. `embs` (B,256,64,64) and the decoder parameters.  Each image is one prompt of the 5 output tokens with the dense
+        prompt no_mask_embed, keyed by its own embedding, as the reference decodes each prompt-free record on its own.  Returns
+        (low (B,M,256,256), iou (B,M))."""
+        if not self.training:
+            raise RuntimeError("decoder_train_images needs train() mode")
+        if embs.dim() != 4 or tuple(embs.shape[1:]) != (256, 64, 64) or embs.shape[0] == 0:
+            raise ValueError(f"decoder_train_images: embeddings must have shape (B, 256, 64, 64) with B >= 1, got {tuple(embs.shape)}")
+        return _ImagesDecoderFn.apply(embs, self, int(slot), bool(multimask_output))
+
+    def decode_images_with_training_decoder(self, embs: torch.Tensor, multimask_output: bool, slot: int = 0):
+        """Forward pass only of `decoder_train_images` (no autograd record, any mode).  It reads the optimizer's current weights,
+        which the inference decoder only sees after `load_state_dict`, so validation between training steps decodes here.  Uses
+        decoder slot `slot` (a pending backward pass of that slot is lost)."""
+        with torch.no_grad():
+            return _ImagesDecoderFn.forward(types.SimpleNamespace(), embs.detach(), self, int(slot), bool(multimask_output))
 
     def decode_with_training_decoder(self, emb: torch.Tensor, points, boxes, multimask_output: bool, slot: int = 0, masks=None):
         """Forward pass only of `decoder_train` (no autograd record, any mode): the inference decoder takes at most 16 tokens per

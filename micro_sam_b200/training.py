@@ -47,6 +47,27 @@ def _sparse_tokens(points, boxes) -> int:
     return (n_points + (0 if boxes is not None else 1) if n_points else 0) + (2 if boxes is not None else 0)
 
 
+_PROMPT_KEYS = ("point_coords", "boxes", "mask_inputs")
+
+
+def decoder_slots(batched_inputs: List[Dict[str, Any]]) -> List[Optional[int]]:
+    """The training decoder slot of each record: the prompted records (points, boxes or mask inputs) take slots 0, 1, ... in batch
+    order; a record with no prompt gets None, and all of those are decoded together in the next slot.  A slot holds its
+    activations until its backward pass has run, and there are 8."""
+    slots, n = [], 0
+    for rec in batched_inputs:
+        if any(k in rec for k in _PROMPT_KEYS):
+            slots.append(n)
+            n += 1
+        else:
+            slots.append(None)
+    used = n + (1 if n < len(slots) else 0)
+    if used > 8:
+        raise ValueError(f"training forward: {n} prompted images need {used} decoder slots, and there are 8 (one slot per prompted "
+                         "image, one for all images without prompts, each held until its backward pass has run)")
+    return slots
+
+
 class TrainableSAM:
     """micro_sam.training.TrainableSAM on a `B200Sam` (trainable_sam.py:12-114)."""
 
@@ -73,8 +94,9 @@ class TrainableSAM:
                 return_masks: bool = True) -> List[Dict[str, Any]]:
         """trainable_sam.py:62-114.  `return_masks=False` skips the (n_obj, M, H, W) up-sampled logits (the loss does not need
         them: `compute_loss` works from `low_res_masks`).  In train() mode with grad enabled the outputs are part of the autograd
-        graph (point, box and `mask_inputs` prompts; the mask inputs get no gradient): image i of the batch uses decoder slot i,
-        which holds its activations until its backward pass has run."""
+        graph (point, box and `mask_inputs` prompts; the mask inputs get no gradient): each prompted image uses a decoder slot of
+        its own, and the images without prompts (semantic training) are decoded together in one more slot (`decoder_slots`); a
+        slot holds its activations until its backward pass has run."""
         if getattr(self.sam, "training", False) and torch.is_grad_enabled():
             return self._forward_train(batched_inputs, image_embeddings, multimask_output, return_masks)
         with torch.no_grad():
@@ -82,14 +104,21 @@ class TrainableSAM:
 
     def _forward_train(self, batched_inputs, image_embeddings, multimask_output, return_masks):
         sam, dev = self.sam, self.sam.device
-        if len(batched_inputs) > 8:
-            raise ValueError("training forward: at most 8 images per call (one decoder slot per image until its backward pass has run)")
+        slots = decoder_slots(batched_inputs)
+        free = [i for i, s in enumerate(slots) if s is None]
+        decoded = {}
+        if free:   # every prompt-free image in one call and one slot, after the prompted ones
+            low, iou = sam.decoder_train_images(image_embeddings[free], multimask_output, slot=len(batched_inputs) - len(free))
+            decoded = {i: (low[b:b + 1], iou[b:b + 1]) for b, i in enumerate(free)}
         outputs = []
         for i, (rec, emb) in enumerate(zip(batched_inputs, image_embeddings)):
-            points = (rec["point_coords"].to(dev), rec["point_labels"].to(dev)) if "point_coords" in rec else None
-            boxes = rec["boxes"].to(dev) if "boxes" in rec else None
-            masks = rec["mask_inputs"].to(dev) if "mask_inputs" in rec else None
-            low, iou = sam.decoder_train(emb, points, boxes, multimask_output, slot=i % 8, masks=masks)
+            if slots[i] is None:
+                low, iou = decoded[i]
+            else:
+                points = (rec["point_coords"].to(dev), rec["point_labels"].to(dev)) if "point_coords" in rec else None
+                boxes = rec["boxes"].to(dev) if "boxes" in rec else None
+                masks = rec["mask_inputs"].to(dev) if "mask_inputs" in rec else None
+                low, iou = sam.decoder_train(emb, points, boxes, multimask_output, slot=slots[i], masks=masks)
             out = {"low_res_masks": low, "iou_predictions": iou, "input_size": tuple(rec["input_size"]),
                    "original_size": tuple(rec["original_size"])}
             if return_masks:
@@ -930,6 +959,65 @@ def compute_semantic_loss(pred, y, num_classes: int, dice_weight: Optional[float
     ce = st[3 * num_classes] / st[3 * num_classes + 1]
     loss = dice + ce if dice_weight is None else dice_weight * dice + (1 - dice_weight) * ce
     return loss.to(torch.float32)
+
+
+def get_trainable_sam_model(model_type: str = "vit_b", device=None, checkpoint_path=None, freeze=None, return_state: bool = False,
+                            peft_kwargs=None, flexible_load_checkpoint: bool = False, **model_kwargs):
+    """micro_sam.training.util.get_trainable_sam_model (util.py:77): a `TrainableSAM` in train() mode (and the checkpoint state
+    with `return_state`).  `model_kwargs` go to `util.get_sam_model` (e.g. `state_dict=`, `max_batch=`), which refuses
+    `num_multimask_outputs` other than 3 and `flexible_load_checkpoint`.  A semantic model with 3 classes is this model with
+    `multimask_output=True`."""
+    from . import util
+    if freeze is not None:
+        raise NotImplementedError("get_trainable_sam_model(freeze=...): frozen parameter groups are not implemented; every "
+                                  "parameter of the model is trained")
+    if peft_kwargs:
+        raise NotImplementedError("get_trainable_sam_model(peft_kwargs=...): parameter-efficient fine-tuning (LoRA and the other "
+                                  "PEFT wrappers) is not implemented")
+    _, sam, state = util.get_sam_model(model_type=model_type, device=device, checkpoint_path=checkpoint_path, return_sam=True,
+                                       return_state=True, flexible_load_checkpoint=flexible_load_checkpoint, **model_kwargs)
+    sam.train()
+    model = TrainableSAM(sam)
+    return (model, state) if return_state else model
+
+
+def semantic_train_iteration(model: TrainableSAM, x, y, num_classes: int, dice_weight: Optional[float] = None,
+                             convert_inputs=None) -> torch.Tensor:
+    """The body of SemanticSamTrainer._train_epoch_impl (semantic_sam_trainer.py:113-140): records without prompts
+    (`ConvertToSemanticSamInputs`), one encoder pass, one prompt-free decode of the whole batch with `multimask_output=True`, and
+    `compute_semantic_loss` from the low-res logits.  Returns the loss; the caller zeroes the gradients
+    (`sam.zero_decoder_grads()`), calls `loss.backward()` and then `sam.optimizer_step()` (after `sam.allreduce_grads(...)` when
+    training on several GPUs).  The decoder gives 3 channels, so `num_classes` must be 3."""
+    convert_inputs = ConvertToSemanticSamInputs() if convert_inputs is None else convert_inputs
+    batched_inputs = convert_inputs(x, y)
+    image_embeddings, batched_inputs = model.image_embeddings_oft(batched_inputs)
+    outputs = model(batched_inputs, image_embeddings, multimask_output=True, return_masks=False)
+    return compute_semantic_loss(outputs, y, num_classes, dice_weight)
+
+
+def semantic_validation(model: TrainableSAM, loader, num_classes: int, dice_weight: Optional[float] = None,
+                        convert_inputs=None) -> Tuple[float, float]:
+    """SemanticSamTrainer._validate_impl (semantic_sam_trainer.py:143-170): eval() mode and no_grad, the mean loss over `loader`
+    (an iterable of (x, y) batches with a length) as both metric and loss.  The model's previous mode is restored afterwards.
+    The batch is decoded by the training decoder's forward pass (`decode_images_with_training_decoder`, slot 0), so that
+    validation between optimizer steps sees the weights trained so far.  Returns (metric, loss)."""
+    convert_inputs = ConvertToSemanticSamInputs() if convert_inputs is None else convert_inputs
+    was_training = bool(model.sam.training)
+    model.sam.eval()
+    try:
+        total = 0.0
+        with torch.no_grad():
+            for x, y in loader:
+                batched_inputs = convert_inputs(x, y)
+                image_embeddings, batched_inputs = model.image_embeddings_oft(batched_inputs)
+                low, _ = model.sam.decode_images_with_training_decoder(image_embeddings, True)
+                outputs = [{"low_res_masks": low[b:b + 1], "input_size": tuple(rec["input_size"]),
+                            "original_size": tuple(rec["original_size"])} for b, rec in enumerate(batched_inputs)]
+                total += float(compute_semantic_loss(outputs, y, num_classes, dice_weight).item())
+    finally:
+        model.sam.train(was_training)
+    loss = total / len(loader)
+    return loss, loss
 
 
 def export_instance_segmentation_model(unetr: UNETR, output_path) -> None:
