@@ -458,16 +458,10 @@ int msam_multicut_gaec(int64_t n_nodes, int64_t n_edges, const int64_t* uv, cons
  * the 2x2 / stride 2 transposed convolution, N = 4 Cout with row (i * 2 + j) * Cout + co of w, out [B, 2H, 2W, Cout].
  * C0, C1 multiples of 64, Cout a multiple of 64.  stats (optional, msam_ais_conv_stats_size bytes): per image, 64 x 2-pixel
  * tile (and 2x2 position when transposed) and channel, the sum and sum of squares of the stored outputs, for
- * msam_op_ais_instnorm with nchunk = size / (16 B Cout). */
+ * msam_op_ais_norm_forward with nchunk = size / (16 B Cout). */
 int64_t msam_ais_conv_stats_size(int B, int H, int W, int Cout, int transposed);
 int msam_op_ais_conv(const void* x0, int C0, const void* x1, int C1, int B, int H, int W, int ks, const void* w_bf16,
                      const float* bias, int Cout, int relu, int transposed, void* out, double* stats, void* stream);
-/* InstanceNorm2d (eps, biased variance per image and channel, optional affine gamma / beta) of x [B, HW, C] -> out (bf16);
- * C % 8 == 0.  stats: the partial sums msam_op_ais_conv wrote for x (nchunk per image), or null: computed here.  The partial
- * sums are reduced in a fixed order.  ws: msam_ais_instnorm_workspace bytes, 8-byte aligned. */
-int64_t msam_ais_instnorm_workspace(int B, int HW, int C);
-int msam_op_ais_instnorm(const void* x, int B, int HW, int C, const double* stats, int nchunk, const float* gamma,
-                         const float* beta, float eps, void* ws, int64_t ws_bytes, void* out, void* stream);
 /* bilinear x2 (align_corners=False) of [B, H, W, C] -> [B, 2H, 2W, C]; C % 8 == 0 */
 int msam_op_ais_upsample2(const void* x, int B, int H, int W, int C, void* out, void* stream);
 /* out_conv (1x1, C -> 3, w fp32 [3][C]) + sigmoid of [B, HW, C] -> fp32 [B, 3, HW]; C % 8 == 0, C <= 512 */
@@ -493,13 +487,15 @@ int msam_ais_props(const int32_t* labels, int H, int W, int n_ids, int32_t* prop
 int64_t msam_ais_wgrad_workspace(int Cout, int C0, int C1, int B, int H, int W, int ks);
 int msam_op_ais_wgrad(const void* dy, int Cout, const void* x0, int C0, const void* x1, int C1, int B, int H, int W, int ks, void* ws,
                       int64_t ws_bytes, float* dw, void* stream);
-/* Training-mode norm of x [B, HW, C] bf16: per_image 1 = InstanceNorm, 0 = BatchNorm (batch statistics over B * HW, with
- * run_mean / run_var updated as torch does: momentum, unbiased variance).  Writes mean and rstd ([B * C] or [C]) for the
- * backward pass and out = (relu of) the normalised x.  ws: msam_ais_norm_workspace bytes, 256-byte aligned. */
+/* Norm of x [B, HW, C] bf16, C % 8 == 0: per_image 1 = InstanceNorm (biased variance per image and channel), 0 = BatchNorm
+ * on batch statistics (over B * HW per channel; run_mean / run_var, if given, updated as torch does: momentum, unbiased
+ * variance); optional affine gamma / beta; out = (relu of) the normalised x.  stats: the partial sums msam_op_ais_conv wrote for
+ * x (nchunk per image), or null: computed here.  The partial sums are reduced in a fixed order.  mean and rstd ([B * C] or [C],
+ * for the backward pass) are optional, both or neither.  ws: msam_ais_norm_workspace bytes, 256-byte aligned. */
 int64_t msam_ais_norm_workspace(int B, int HW, int C);
-int msam_op_ais_norm_forward(const void* x, int B, int HW, int C, int per_image, const float* gamma, const float* beta, float eps,
-                             int relu, float momentum, float* run_mean, float* run_var, void* ws, int64_t ws_bytes, float* mean,
-                             float* rstd, void* out, void* stream);
+int msam_op_ais_norm_forward(const void* x, int B, int HW, int C, int per_image, const double* stats, int nchunk, const float* gamma,
+                             const float* beta, float eps, int relu, float momentum, float* run_mean, float* run_var, void* ws,
+                             int64_t ws_bytes, float* mean, float* rstd, void* out, void* stream);
 /* Its backward pass: g = dy (bf16, or fp32 when dy_f32; row stride ldd) times [relu_out > 0] when relu_out is given;
  * dx = gamma rstd (g - mean(g) - xhat mean(g xhat)), times [x > 0] when in_mask; out_mode 0: bf16 store, 1: fp32 store,
  * 2: fp32 add, row stride ldo.  dgamma / dbeta (optional): sum g xhat, sum g per channel. */

@@ -159,10 +159,6 @@ def lib() -> ctypes.CDLL:
         L.msam_ais_conv_stats_size.argtypes = [c_int, c_int, c_int, c_int, c_int]
         L.msam_op_ais_conv.argtypes = [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
                                        c_int, c_int, c_void_p, c_void_p, c_void_p]
-        L.msam_ais_instnorm_workspace.restype = c_int64
-        L.msam_ais_instnorm_workspace.argtypes = [c_int, c_int, c_int]
-        L.msam_op_ais_instnorm.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_float, c_void_p,
-                                           c_int64, c_void_p, c_void_p]
         L.msam_op_ais_upsample2.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
         L.msam_op_ais_head.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
         L.msam_op_ais_resize.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
@@ -178,8 +174,9 @@ def lib() -> ctypes.CDLL:
                                         c_int64, c_void_p, c_void_p]
         L.msam_ais_norm_workspace.restype = c_int64
         L.msam_ais_norm_workspace.argtypes = [c_int, c_int, c_int]
-        L.msam_op_ais_norm_forward.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_float,
-                                               c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]
+        L.msam_op_ais_norm_forward.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_float,
+                                               c_int, c_float, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
+                                               c_void_p]
         L.msam_op_ais_norm_backward.argtypes = [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int,
                                                 c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int64, c_void_p, c_int, c_int,
                                                 c_void_p, c_void_p, c_void_p]

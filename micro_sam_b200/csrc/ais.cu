@@ -7,9 +7,8 @@
 //                         tensor maps, so a channel concatenation is read in place and TMA's zero fill is the padding.
 //                         Epilogue: bias (BatchNorm folded into the weights on the host), ReLU or the 2x2 / stride 2
 //                         transposed-convolution scatter, and per-(image, channel) partial sums for the InstanceNorm after it.
-//   ais_in_*            : InstanceNorm2d (biased variance, per image and channel): fp64 chunk partials (from the convolution
-//                         epilogue, or a pass of their own) reduced in a fixed order, then a scale / shift pass.  It cannot be folded into the next convolution: its zero padding
-//                         would pick up the shift.
+//   InstanceNorm2d      : the ais_nt_* norm kernels of ais_train.cu (msam_op_ais_norm_forward), fed the epilogue's partial sums.
+//                         It cannot be folded into the next convolution: its zero padding would pick up the shift.
 //   ais_up2_kernel      : bilinear x2, align_corners=False (the interpolation upsampler; its conv1x1 runs before it, at the
 //                         low resolution, because bilinear taps sum to 1).
 //   ais_head_kernel     : out_conv (1x1 to 3 channels) + sigmoid, fp32 planes.
@@ -202,73 +201,6 @@ ais_conv_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__
       }
     }
   }
-}
-
-// ------------------------------------------------------------------------------------------------ InstanceNorm2d
-constexpr int IN_CHUNK = 1024;   // pixels per partial sum
-
-__global__ void ais_in_partial_kernel(const __nv_bfloat16* __restrict__ x, int HW, int C, int nchunk, double* __restrict__ part) {
-  const int b = blockIdx.y, ch = blockIdx.x;
-  const int p0 = ch * IN_CHUNK, p1 = min(HW, p0 + IN_CHUNK);
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    double s = 0.0, ss = 0.0;
-    for (int p = p0; p < p1; ++p) {
-      const double v = (double)__bfloat162float(x[((size_t)b * HW + p) * C + c]);
-      s += v;
-      ss += v * v;
-    }
-    double* o = part + (((size_t)b * nchunk + ch) * C + c) * 2;
-    o[0] = s;
-    o[1] = ss;
-  }
-}
-
-// one block per (image, channel): thread t sums chunks t, t + 256, ... in order, then a fixed tree over the threads
-__global__ void __launch_bounds__(256) ais_in_finalize_kernel(const double* __restrict__ part, int HW, int C, int nchunk,
-                                                              const float* gamma, const float* beta, float eps,
-                                                              float* __restrict__ scale, float* __restrict__ shift) {
-  __shared__ double rs[256], rss[256];
-  const int i = blockIdx.x, b = i / C, c = i % C;
-  double s = 0.0, ss = 0.0;
-  for (int ch = threadIdx.x; ch < nchunk; ch += 256) {
-    const double* p = part + (((size_t)b * nchunk + ch) * C + c) * 2;
-    s += p[0];
-    ss += p[1];
-  }
-  rs[threadIdx.x] = s;
-  rss[threadIdx.x] = ss;
-  __syncthreads();
-  for (int o = 128; o > 0; o >>= 1) {
-    if (threadIdx.x < o) {
-      rs[threadIdx.x] += rs[threadIdx.x + o];
-      rss[threadIdx.x] += rss[threadIdx.x + o];
-    }
-    __syncthreads();
-  }
-  if (threadIdx.x) return;
-  const double mean = rs[0] / HW, var = fmax(rss[0] / HW - mean * mean, 0.0);
-  const double rstd = 1.0 / sqrt(var + (double)eps);
-  const double g = gamma ? (double)gamma[c] : 1.0, bt = beta ? (double)beta[c] : 0.0;
-  scale[i] = (float)(g * rstd);
-  shift[i] = (float)(bt - mean * g * rstd);
-}
-
-__global__ void ais_in_apply_kernel(const __nv_bfloat16* __restrict__ x, int HW, int C, long total8, const float* __restrict__ scale,
-                                    const float* __restrict__ shift, __nv_bfloat16* __restrict__ out) {
-  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= total8) return;
-  const long e = i * 8;
-  const int c = (int)(e % C);
-  const int b = (int)(e / ((long)HW * C));
-  const uint4 v = *reinterpret_cast<const uint4*>(x + e);
-  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-  uint32_t o[4];
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const int c0 = b * C + c + 2 * k;
-    o[k] = pack_bf16(bf16_lo(w[k]) * scale[c0] + shift[c0], bf16_hi(w[k]) * scale[c0 + 1] + shift[c0 + 1]);
-  }
-  *reinterpret_cast<uint4*>(out + e) = make_uint4(o[0], o[1], o[2], o[3]);
 }
 
 // ------------------------------------------------------------------------------------------------ bilinear x2, head, resize
@@ -549,10 +481,6 @@ __global__ void ais_props_init_kernel(int* props, int n_ids) {
   p[3] = p[4] = -1;
 }
 
-inline unsigned nblk(long n, int t = 256) { return (unsigned)((n + t - 1) / t); }
-inline bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
-size_t up256(size_t b) { return (b + 255) & ~size_t(255); }
-
 int gaussian_taps(const double* taps, int r, double* dev, cudaStream_t st) {
   if (r < 0 || 2 * r + 1 > MAX_TAPS) return set_error("msam_ais_postprocess: smoothing radius %d (at most %d)", r, MAX_TAPS / 2);
   if (r > 0 && !taps) return set_error("msam_ais_postprocess: null taps");
@@ -661,26 +589,6 @@ int conv_stats_count(int B, int H, int W, int Cout, int transposed) {   // doubl
   return B * (transposed ? 4 : 1) * ((W + CV_TX - 1) / CV_TX) * ((H + CV_TY - 1) / CV_TY) * Cout * 2;
 }
 
-// part: the partial sums of a convolution epilogue (nchunk per image), or null: computed here into own_part
-int launch_ais_instnorm(const __nv_bfloat16* x, int B, int HW, int C, const double* part, int nchunk, const float* gamma,
-                        const float* beta, float eps, double* own_part, float* scale, float* shift, __nv_bfloat16* out,
-                        cudaStream_t st) {
-  prof_begin(st, part ? "ais instnorm (conv statistics)" : "ais instnorm", 0.0, 4.0 * B * HW * C);
-  if (!part) {
-    nchunk = (HW + IN_CHUNK - 1) / IN_CHUNK;
-    ais_in_partial_kernel<<<dim3(nchunk, B), C < 256 ? C : 256, 0, st>>>(x, HW, C, nchunk, own_part);
-    LAUNCH_CHECK("ais instnorm partials");
-    part = own_part;
-  }
-  ais_in_finalize_kernel<<<B * C, 256, 0, st>>>(part, HW, C, nchunk, gamma, beta, eps, scale, shift);
-  LAUNCH_CHECK("ais instnorm finalize");
-  const long t8 = (long)B * HW * C / 8;
-  ais_in_apply_kernel<<<nblk(t8), 256, 0, st>>>(x, HW, C, t8, scale, shift, out);
-  prof_end(st);
-  LAUNCH_CHECK("ais instnorm apply");
-  return 0;
-}
-
 }  // namespace msam
 
 using namespace msam;
@@ -708,29 +616,6 @@ int msam_op_ais_conv(const void* x0, int C0, const void* x1, int C1, int B, int 
     return set_error("msam_op_ais_conv: misaligned pointer");
   return launch_ais_conv((const __nv_bfloat16*)x0, C0, (const __nv_bfloat16*)x1, C1, B, H, W, ks, (const __nv_bfloat16*)w_bf16,
                          bias, Cout, relu != 0, transposed != 0, (__nv_bfloat16*)out, stats, (cudaStream_t)stream);
-}
-
-int64_t msam_ais_instnorm_workspace(int B, int HW, int C) {
-  if (B <= 0 || HW <= 0 || C <= 0) return -1;
-  return (int64_t)B * ((HW + IN_CHUNK - 1) / IN_CHUNK) * C * 16 + (int64_t)B * C * 8 + 256;
-}
-
-int msam_op_ais_instnorm(const void* x, int B, int HW, int C, const double* stats, int nchunk, const float* gamma,
-                         const float* beta, float eps, void* ws, int64_t ws_bytes, void* out, void* stream) {
-  if (!x || !out || !ws) return set_error("msam_op_ais_instnorm: null argument");
-  if (B <= 0 || HW <= 0 || C <= 0 || C % 8 || (long)B * HW * C >= (1l << 40))
-    return set_error("msam_op_ais_instnorm: B=%d, HW=%d, C=%d (C a multiple of 8)", B, HW, C);
-  if (stats && nchunk <= 0) return set_error("msam_op_ais_instnorm: %d statistics chunks", nchunk);
-  if ((gamma == nullptr) != (beta == nullptr)) return set_error("msam_op_ais_instnorm: gamma and beta go together");
-  if (ws_bytes < msam_ais_instnorm_workspace(B, HW, C))
-    return set_error("msam_op_ais_instnorm: workspace of %lld bytes, %lld needed", (long long)ws_bytes,
-                     (long long)msam_ais_instnorm_workspace(B, HW, C));
-  if (!al16(x) || !al16(out) || ((uintptr_t)ws & 7) || ((uintptr_t)stats & 7))
-    return set_error("msam_op_ais_instnorm: misaligned pointer");
-  double* part = (double*)ws;
-  float* scale = (float*)(part + (size_t)B * ((HW + IN_CHUNK - 1) / IN_CHUNK) * C * 2);
-  return launch_ais_instnorm((const __nv_bfloat16*)x, B, HW, C, stats, nchunk, gamma, beta, eps, part, scale,
-                             scale + (size_t)B * C, (__nv_bfloat16*)out, (cudaStream_t)stream);
 }
 
 int msam_op_ais_upsample2(const void* x, int B, int H, int W, int C, void* out, void* stream) {

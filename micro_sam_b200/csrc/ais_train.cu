@@ -1,13 +1,14 @@
 // Training of the AIS decoder (torch_em's UNETR decoder as micro-sam trains it, DESIGN.md section 2): the backward pass of every
-// decoder layer, training-mode norms and the distance-based Dice loss.  Every reduction runs in a fixed order, so two identical
-// steps give bit-identical gradients.
+// decoder layer, the norms (of inference and training alike) and the distance-based Dice loss.  Every reduction runs in a fixed
+// order, so two identical steps give bit-identical gradients.
 //   ais_wgrad_kernel     : 3x3 / 1x1 weight gradient dW[co, tap, ci] = sum_p dY[p, co] X[p + tap, ci], an implicit GEMM on wgmma
 //                          with K over the pixels.  A k-block is one 64 x 2-pixel box of dY and of X (shifted by the tap) read
 //                          through the 4-D tensor maps of ais_conv_kernel: TMA's zero fill is the padding, the K tail and the
 //                          pixels past the image, and the channels past C0 come from the second source's map.  Split-K over
 //                          CTAs, each split writes its own fp32 partial, reduced over the splits in order.
 //   ais_nt_*             : InstanceNorm (per image and channel) and BatchNorm in training mode (per channel over the batch):
-//                          fp64 chunk partials, a finalize in a fixed order, an apply pass; the backward pass has the same shape.
+//                          fp64 chunk partials (or those of ais_conv_kernel's epilogue), a finalize in a fixed order, an apply
+//                          pass; the backward pass has the same shape.
 //   ais_up2_bwd_kernel   : adjoint of bilinear x2 (align_corners=False) as a gather: every input pixel sums the <= 4 x 4 outputs
 //                          that read it, so no atomics.
 //   ais_s2d_kernel       : space-to-depth of dY, the input of the 2x2 / stride 2 transposed convolution's backward GEMMs.
@@ -25,10 +26,6 @@
 
 namespace msam {
 namespace {
-
-inline unsigned nblk(long n, int t = 256) { return (unsigned)((n + t - 1) / t); }
-inline bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
-inline size_t up256(size_t b) { return (b + 255) & ~size_t(255); }
 
 // ------------------------------------------------------------------------------------------------ weight gradient
 // One CTA: 64 * MH output channels x 64 * NB input channels of one tap.  Each k-block is a {64 ch, 64 x, 2 y, 1 image} box
@@ -217,33 +214,49 @@ __global__ void ais_nt_partial_kernel(const __nv_bfloat16* __restrict__ x, int l
   }
 }
 
-// One thread per group (image and channel, or channel): sums the chunk partials (of every image for BatchNorm) in order.
-// mean / rstd of the biased variance; scale / shift of the affine apply; BatchNorm's running statistics as torch updates them
-// (momentum, unbiased variance).
-__global__ void ais_nt_stats_kernel(const double* __restrict__ part, int B, int HW, int C, int nchunk, int per_image, float eps,
-                                    const float* gamma, const float* beta, float momentum, float* run_mean, float* run_var,
-                                    float* __restrict__ mean, float* __restrict__ rstd, float* __restrict__ scale,
-                                    float* __restrict__ shift) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (per_image ? B * C : C)) return;
-  const int c = i % C, b0 = per_image ? i / C : 0, b1 = per_image ? b0 + 1 : B;
+// One block per group (image and channel, or channel): thread t sums the group's chunk partials t, t + 256, ... in order (for
+// BatchNorm every image's chunks, in image order), then a fixed tree over the threads.  Thread 0: mean / rstd of the biased
+// variance (when wanted), scale / shift of the affine apply, and BatchNorm's running statistics as torch updates them (momentum,
+// unbiased variance).
+__global__ void __launch_bounds__(256) ais_nt_finalize_kernel(const double* __restrict__ part, int B, int HW, int C, int nchunk,
+                                                              int per_image, float eps, const float* gamma, const float* beta,
+                                                              float momentum, float* run_mean, float* run_var,
+                                                              float* __restrict__ mean, float* __restrict__ rstd,
+                                                              float* __restrict__ scale, float* __restrict__ shift) {
+  __shared__ double rs[256], rss[256];
+  const int i = blockIdx.x, c = i % C;
+  const int n = per_image ? nchunk : B * nchunk;   // the group's chunks: part[b][chunk] with b * nchunk + chunk from k0 on
+  const size_t k0 = per_image ? (size_t)(i / C) * nchunk : 0;
   double s = 0.0, ss = 0.0;
-  for (int b = b0; b < b1; ++b)
-    for (int ch = 0; ch < nchunk; ++ch) {
-      const double* p = part + (((size_t)b * nchunk + ch) * C + c) * 2;
-      s += p[0];
-      ss += p[1];
+  for (int k = threadIdx.x; k < n; k += 256) {
+    const double* p = part + ((k0 + k) * C + c) * 2;
+    s += p[0];
+    ss += p[1];
+  }
+  rs[threadIdx.x] = s;
+  rss[threadIdx.x] = ss;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if (threadIdx.x < o) {
+      rs[threadIdx.x] += rs[threadIdx.x + o];
+      rss[threadIdx.x] += rss[threadIdx.x + o];
     }
-  const double n = (double)HW * (b1 - b0);
-  const double mu = s / n, var = fmax(ss / n - mu * mu, 0.0), r = 1.0 / sqrt(var + (double)eps);
+    __syncthreads();
+  }
+  if (threadIdx.x) return;
+  const double cnt = per_image ? (double)HW : (double)HW * B;
+  const double mu = rs[0] / cnt, var = fmax(rss[0] / cnt - mu * mu, 0.0);
+  const double r = 1.0 / sqrt(var + (double)eps);
   const double g = gamma ? (double)gamma[c] : 1.0, bt = beta ? (double)beta[c] : 0.0;
-  mean[i] = (float)mu;
-  rstd[i] = (float)r;
   scale[i] = (float)(g * r);
   shift[i] = (float)(bt - mu * g * r);
+  if (mean) {
+    mean[i] = (float)mu;
+    rstd[i] = (float)r;
+  }
   if (run_mean) {
     run_mean[c] = (float)((1.0 - momentum) * (double)run_mean[c] + momentum * mu);
-    run_var[c] = (float)((1.0 - momentum) * (double)run_var[c] + momentum * var * n / fmax(n - 1.0, 1.0));
+    run_var[c] = (float)((1.0 - momentum) * (double)run_var[c] + momentum * var * cnt / fmax(cnt - 1.0, 1.0));
   }
 }
 
@@ -599,27 +612,36 @@ static int nt_check(const char* fn, int B, int HW, int C, void* ws, int64_t ws_b
   return 0;
 }
 
-int msam_op_ais_norm_forward(const void* x, int B, int HW, int C, int per_image, const float* gamma, const float* beta, float eps,
-                             int relu, float momentum, float* run_mean, float* run_var, void* ws, int64_t ws_bytes, float* mean,
-                             float* rstd, void* out, void* stream) {
-  if (!x || !out || !mean || !rstd) return set_error("msam_op_ais_norm_forward: null argument");
+int msam_op_ais_norm_forward(const void* x, int B, int HW, int C, int per_image, const double* stats, int nchunk, const float* gamma,
+                             const float* beta, float eps, int relu, float momentum, float* run_mean, float* run_var, void* ws,
+                             int64_t ws_bytes, float* mean, float* rstd, void* out, void* stream) {
+  if (!x || !out) return set_error("msam_op_ais_norm_forward: null argument");
   RUN(nt_check("msam_op_ais_norm_forward", B, HW, C, ws, ws_bytes));
-  if ((gamma == nullptr) != (beta == nullptr) || (run_mean == nullptr) != (run_var == nullptr) || (run_mean && per_image))
-    return set_error("msam_op_ais_norm_forward: gamma / beta and the running statistics go in pairs (running ones for BatchNorm only)");
-  if (!al16(x) || !al16(out)) return set_error("msam_op_ais_norm_forward: misaligned pointer");
+  if (stats && nchunk <= 0) return set_error("msam_op_ais_norm_forward: %d statistics chunks", nchunk);
+  if ((gamma == nullptr) != (beta == nullptr) || (mean == nullptr) != (rstd == nullptr) || (run_mean == nullptr) != (run_var == nullptr) ||
+      (run_mean && per_image))
+    return set_error("msam_op_ais_norm_forward: gamma / beta, mean / rstd and the running statistics go in pairs (running ones for "
+                     "BatchNorm only)");
+  if (!al16(x) || !al16(out) || ((uintptr_t)stats & 7)) return set_error("msam_op_ais_norm_forward: misaligned pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  const int nchunk = (HW + NT_CHUNK - 1) / NT_CHUNK;
+  const int own = (HW + NT_CHUNK - 1) / NT_CHUNK;
   double* part = (double*)ws;
-  float* scale = (float*)((char*)ws + up256((size_t)B * nchunk * C * 16));
+  float* scale = (float*)((char*)ws + up256((size_t)B * own * C * 16));
   float* shift = scale + (size_t)B * C;
-  prof_begin(st, per_image ? "ais instnorm (train)" : "ais batchnorm (train)", 0.0, 6.0 * B * HW * C);
-  ais_nt_partial_kernel<float><<<dim3(nchunk, B), C < 256 ? C : 256, 0, st>>>((const __nv_bfloat16*)x, C, nullptr, 0, nullptr,
-                                                                            nullptr, nullptr, per_image, HW, C, nchunk, part);
-  LAUNCH_CHECK("ais norm partials");
-  const int groups = per_image ? B * C : C;
-  ais_nt_stats_kernel<<<nblk(groups, 128), 128, 0, st>>>(part, B, HW, C, nchunk, per_image, eps, gamma, beta, momentum, run_mean,
-                                                         run_var, mean, rstd, scale, shift);
-  LAUNCH_CHECK("ais norm statistics");
+  // the inference decoder's InstanceNorms keep no mean / rstd; their labels match its kernel tables
+  const char* label = !per_image ? "ais batchnorm (train)" : mean ? "ais instnorm (train)"
+                                 : stats ? "ais instnorm (conv statistics)" : "ais instnorm";
+  prof_begin(st, label, 0.0, (stats ? 4.0 : 6.0) * B * HW * C);
+  if (!stats) {
+    ais_nt_partial_kernel<float><<<dim3(own, B), C < 256 ? C : 256, 0, st>>>((const __nv_bfloat16*)x, C, nullptr, 0, nullptr, nullptr,
+                                                                           nullptr, per_image, HW, C, own, part);
+    LAUNCH_CHECK("ais norm partials");
+    stats = part;
+    nchunk = own;
+  }
+  ais_nt_finalize_kernel<<<per_image ? B * C : C, 256, 0, st>>>(stats, B, HW, C, nchunk, per_image, eps, gamma, beta, momentum,
+                                                                run_mean, run_var, mean, rstd, scale, shift);
+  LAUNCH_CHECK("ais norm finalize");
   const long t8 = (long)B * HW * C / 8;
   ais_nt_apply_kernel<<<nblk(t8), 256, 0, st>>>((const __nv_bfloat16*)x, HW, C, t8, scale, shift, per_image, relu, (__nv_bfloat16*)out);
   prof_end(st);

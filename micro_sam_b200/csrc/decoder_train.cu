@@ -196,8 +196,6 @@ __global__ void masks_grad_kernel(const float* __restrict__ d_low, int P, int nm
   *reinterpret_cast<uint4*>(out8 + (p * 65536 + up_row(Y, X)) * 8) = make_uint4(pack_bf16(v[0], v[1]), pack_bf16(v[2], v[3]), pack_bf16(v[4], v[5]), pack_bf16(v[6], v[7]));
 }
 
-inline unsigned nblk(long n, int per = 256) { return (unsigned)((n + per - 1) / per); }
-
 // ------------------------------------------------------------------------------------------------ mask prompts
 // PromptEncoder.mask_downscaling: conv 1->4 (k2 s2, 256^2 -> 128^2), LayerNorm2d(4), GELU, conv 4->16 (k2 s2 -> 64^2), LayerNorm2d(16),
 // GELU, conv 1x1 16->256, all fp32.  Output pixel (ty, tx) of the 64^2 grid depends on its own 4x4 input patch only.  The ten

@@ -32,6 +32,12 @@ int launch_check(const char* name);
 void prof_begin(cudaStream_t st, const char* name, double flops, double bytes);
 void prof_end(cudaStream_t st);
 
+// Launch arithmetic: blocks of `per` threads covering n items; 16-byte alignment of a vectorised operand; workspace slices
+// rounded up to 256 bytes
+inline unsigned nblk(long n, int per = 256) { return (unsigned)((n + per - 1) / per); }
+inline bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+inline size_t up256(size_t b) { return (b + 255) & ~size_t(255); }
+
 // ---- gemm.cu :  out[M,N] = act(A[M,K] * W[N,K]^T + bias) (+ residual[row % res_rows])
 struct GemmArgs {
   const __nv_bfloat16* A = nullptr;  // [M, lda]

@@ -35,9 +35,6 @@ constexpr int SL_MAX_GRID = 1056;   // 8 CTAs per SM of an H100 SXM; fixed, so t
 constexpr int SL_MAX_C = 15;
 constexpr int SL_IGNORE = -100;
 
-inline unsigned nblk(long n, int t = 256) { return (unsigned)((n + t - 1) / t); }
-inline size_t up256(size_t b) { return (b + 255) & ~size_t(255); }
-
 // The taps of one original_size pixel: the 2 x 2 stage-1 positions of the second interpolation (one position when it is the
 // identity) and, per position, the 2 x 2 low-res taps.  Values equal full_res() term by term.
 struct PixTaps {

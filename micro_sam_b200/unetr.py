@@ -18,6 +18,7 @@ import torch
 from . import _lib
 
 BN_EPS = 1e-5
+BN_MOMENTUM = 0.1
 IN_EPS = 1e-5
 IMG_SIZE = 1024
 
@@ -144,6 +145,73 @@ def _check_kernel_channels(plan):
         raise NotImplementedError(f"the AIS decoder kernels take channel counts that are multiples of 64, the plan has {bad[0]}")
 
 
+# ------------------------------------------------------------------------------------------------ kernel operands and layers
+def pack_conv3x3(w, device):
+    """Conv2d [Cout, Cin, 3, 3] -> msam_op_ais_conv's bf16 operand [Cout][9 Cin] (K-major, K index (ky * 3 + kx) * Cin + ci),
+    converted on `device`; so are the two sampler packings below"""
+    return w.permute(0, 2, 3, 1).flatten(1).to(device, torch.bfloat16).contiguous()
+
+
+def pack_conv_transpose2x2(w, device):
+    """ConvTranspose2d [Cin, Cout, 2, 2] -> [4 Cout][Cin], row (i * 2 + j) * Cout + co"""
+    return w.permute(2, 3, 1, 0).flatten(0, 2).to(device, torch.bfloat16).contiguous()
+
+
+def pack_conv1x1(w, device):
+    """Conv2d [Cout, Cin, 1, 1] -> [Cout][Cin]"""
+    return w[:, :, 0, 0].to(device, torch.bfloat16).contiguous()
+
+
+def conv(x0, x1, w, b, ks, relu, transposed=False, stats=False):
+    """msam_op_ais_conv of bf16 NHWC x0 (channel-concatenated with x1 unless it is None) with a packed weight w and fp32 bias b:
+    -> bf16 NHWC out, and with `stats` (out, (fp64 epilogue partial sums, chunks per image)) for the InstanceNorm after it."""
+    L = _lib.lib()
+    B, H, W, C0 = x0.shape
+    C1 = 0 if x1 is None else x1.shape[3]
+    cout = w.shape[0] // 4 if transposed else w.shape[0]
+    out = torch.empty((B, 2 * H, 2 * W, cout) if transposed else (B, H, W, cout), device=x0.device, dtype=torch.bfloat16)
+    st = torch.empty(int(L.msam_ais_conv_stats_size(B, H, W, cout, int(transposed))) // 8, device=x0.device,
+                     dtype=torch.float64) if stats else None
+    _lib.check(L.msam_op_ais_conv(_lib.ptr(x0), C0, _lib.ptr(x1), C1, B, H, W, ks, _lib.ptr(w), _lib.ptr(b), cout, int(relu),
+                                  int(transposed), _lib.ptr(out), _lib.ptr(st), _lib.cur_stream()))
+    return (out, (st, st.numel() // (2 * B * cout))) if stats else out
+
+
+def norm(x, per_image, gamma=None, beta=None, stats=None, relu=False, run=None, keep=False):
+    """msam_op_ais_norm_forward of bf16 NHWC x: InstanceNorm (per_image) or BatchNorm on batch statistics, updating the running
+    statistics run = (mean, var) when given; from a convolution's epilogue `stats` when given.  -> (out, mean, rstd); mean and
+    rstd (for the backward pass) only with `keep`, else None."""
+    L = _lib.lib()
+    B, H, W, C = x.shape
+    ws = torch.empty(int(L.msam_ais_norm_workspace(B, H * W, C)), device=x.device, dtype=torch.uint8)
+    out = torch.empty_like(x)
+    mean = torch.empty(B * C if per_image else C, device=x.device, dtype=torch.float32) if keep else None
+    rstd = torch.empty_like(mean) if keep else None
+    sp, nch = (None, 0) if stats is None else (_lib.ptr(stats[0]), stats[1])
+    rm, rv = (None, None) if run is None else run
+    _lib.check(L.msam_op_ais_norm_forward(_lib.ptr(x), B, H * W, C, int(per_image), sp, nch, _lib.ptr(gamma), _lib.ptr(beta),
+                                          IN_EPS if per_image else BN_EPS, int(relu), BN_MOMENTUM, _lib.ptr(rm), _lib.ptr(rv),
+                                          _lib.ptr(ws), ws.numel(), _lib.ptr(mean), _lib.ptr(rstd), _lib.ptr(out),
+                                          _lib.cur_stream()))
+    return out, mean, rstd
+
+
+def upsample2(x):
+    """msam_op_ais_upsample2: bilinear x2 of bf16 NHWC x"""
+    B, H, W, C = x.shape
+    out = torch.empty(B, 2 * H, 2 * W, C, device=x.device, dtype=torch.bfloat16)
+    _lib.check(_lib.lib().msam_op_ais_upsample2(_lib.ptr(x), B, H, W, C, _lib.ptr(out), _lib.cur_stream()))
+    return out
+
+
+def head_maps(h, w, b):
+    """msam_op_ais_head: out_conv (fp32 w [3][C], b [3]) + sigmoid of bf16 NHWC h -> fp32 maps [B, 3, H, W]"""
+    B, H, W, C = h.shape
+    out = torch.empty(B, 3, H, W, device=h.device, dtype=torch.float32)
+    _lib.check(_lib.lib().msam_op_ais_head(_lib.ptr(h), B, H * W, C, _lib.ptr(w), _lib.ptr(b), _lib.ptr(out), _lib.cur_stream()))
+    return out
+
+
 class UNETRDecoder:
     """The AIS decoder on the device: `__call__(z12, input_size, original_size)` maps a [B, 256, 64, 64] image embedding to the
     foreground / center distance / boundary distance maps, fp32 [B, 3, *original_size] (DecoderAdapter.forward)."""
@@ -164,23 +232,19 @@ class UNETRDecoder:
                 s = sd[bn + ".weight"] / torch.sqrt(sd[bn + ".running_var"] + BN_EPS)
                 w = w * s[:, None, None, None]
                 b = (b - sd[bn + ".running_mean"]) * s + sd[bn + ".bias"]
-            cout, cin = w.shape[:2]
-            return (w.permute(0, 2, 3, 1).reshape(cout, 9 * cin).to(dev, torch.bfloat16).contiguous(),   # [N][K], K-major
-                    b.to(dev, torch.float32).contiguous())
+            return pack_conv3x3(w, dev), b.to(dev, torch.float32).contiguous()
 
         def sampler(p):
             if self.transposed:
                 w, b = sd[p + ".block.weight"], sd[p + ".block.bias"]
-                cin, cout = w.shape[:2]
-                return (w.permute(2, 3, 1, 0).reshape(4 * cout, cin).to(dev, torch.bfloat16).contiguous(),
-                        b.to(dev, torch.float32).contiguous())
+                return pack_conv_transpose2x2(w, dev), b.to(dev, torch.float32).contiguous()
             w, b = sd[p + ".conv.weight"], sd[p + ".conv.bias"]
-            return (w[:, :, 0, 0].to(dev, torch.bfloat16).contiguous(), b.to(dev, torch.float32).contiguous())
+            return pack_conv1x1(w, dev), b.to(dev, torch.float32).contiguous()
 
         def block(p, affine):
-            norm = [(sd[f"{p}.block.{j}.weight"].to(dev, torch.float32).contiguous(),
-                     sd[f"{p}.block.{j}.bias"].to(dev, torch.float32).contiguous()) if affine else None for j in (0, 3)]
-            return {"norm": norm, "c1": conv3(p + ".block.1"), "c2": conv3(p + ".block.4")}
+            gb = [(sd[f"{p}.block.{j}.weight"].to(dev, torch.float32).contiguous(),
+                   sd[f"{p}.block.{j}.bias"].to(dev, torch.float32).contiguous()) if affine else None for j in (0, 3)]
+            return {"norm": gb, "c1": conv3(p + ".block.1"), "c2": conv3(p + ".block.4")}
 
         self.deconv = [{"up": sampler(f"deconv{i}.block.0"), "conv": conv3(f"deconv{i}.block.1.block", f"deconv{i}.block.2")}
                        for i in range(1, 5)]
@@ -195,42 +259,14 @@ class UNETRDecoder:
     # ---------------------------------------------------------------- layers
     # An activation is (bf16 NHWC tensor [B, H, W, C], statistics): the InstanceNorm partial sums the convolution that wrote it
     # computed in its epilogue, as (fp64 tensor, chunks per image), or None when the norm computes them itself.
-    def _conv(self, x0, x1, wb, ks, relu, transposed=False):
-        L = _lib.lib()
-        B, H, W, C0 = x0.shape
-        C1 = 0 if x1 is None else x1.shape[3]
-        w, b = wb
-        cout = b.numel()
-        shape = (B, 2 * H, 2 * W, cout) if transposed else (B, H, W, cout)
-        out = torch.empty(shape, device=x0.device, dtype=torch.bfloat16)
-        stats = torch.empty(int(L.msam_ais_conv_stats_size(B, H, W, cout, int(transposed))) // 8, device=x0.device,
-                            dtype=torch.float64)
-        _lib.check(L.msam_op_ais_conv(_lib.ptr(x0), C0, _lib.ptr(x1), C1, B, H, W, ks, _lib.ptr(w), _lib.ptr(b), cout, int(relu),
-                                      int(transposed), _lib.ptr(out), _lib.ptr(stats), _lib.cur_stream()))
-        return out, (stats, stats.numel() // (2 * B * cout))
-
-    def _norm(self, act, gb):
-        L = _lib.lib()
-        x, st = act
-        B, H, W, C = x.shape
-        ws = torch.empty(int(L.msam_ais_instnorm_workspace(B, H * W, C)), device=x.device, dtype=torch.uint8)
-        out = torch.empty_like(x)
-        g, b = gb if gb is not None else (None, None)
-        sp, nch = (None, 0) if st is None else (_lib.ptr(st[0]), st[1])
-        _lib.check(L.msam_op_ais_instnorm(_lib.ptr(x), B, H * W, C, sp, nch, _lib.ptr(g), _lib.ptr(b), IN_EPS, _lib.ptr(ws),
-                                          ws.numel(), _lib.ptr(out), _lib.cur_stream()))
-        return out
-
-    def _up2(self, x):
-        B, H, W, C = x.shape
-        out = torch.empty(B, 2 * H, 2 * W, C, device=x.device, dtype=torch.bfloat16)
-        _lib.check(_lib.lib().msam_op_ais_upsample2(_lib.ptr(x), B, H, W, C, _lib.ptr(out), _lib.cur_stream()))
-        return out, None
+    @staticmethod
+    def _norm(act, gb):
+        return norm(act[0], True, *(gb or (None, None)), stats=act[1])[0]
 
     def _sampler(self, x, wb):
         if self.transposed:
-            return self._conv(x, None, wb, 1, False, transposed=True)
-        return self._up2(self._conv(x, None, wb, 1, False)[0])   # conv1x1 commutes with bilinear x2: run it at low resolution
+            return conv(x, None, *wb, 1, False, True, stats=True)
+        return upsample2(conv(x, None, *wb, 1, False, stats=True)[0]), None   # conv1x1 commutes with bilinear x2: at low resolution
 
     def _block(self, a0, a1, blk):
         n0, n1 = blk["norm"][0], blk["norm"][1]
@@ -240,8 +276,8 @@ class UNETRDecoder:
             c0 = a0[0].shape[3]
             x0 = self._norm(a0, None if n0 is None else (n0[0][:c0].contiguous(), n0[1][:c0].contiguous()))
             x1 = self._norm(a1, None if n0 is None else (n0[0][c0:].contiguous(), n0[1][c0:].contiguous()))
-        y = self._conv(x0, x1, blk["c1"], 3, True)
-        return self._conv(self._norm(y, n1), None, blk["c2"], 3, True)
+        y = conv(x0, x1, *blk["c1"], 3, True, stats=True)
+        return conv(self._norm(y, n1), None, *blk["c2"], 3, True, stats=True)
 
     def forward_maps(self, z12: torch.Tensor) -> torch.Tensor:
         """_forward_impl + sigmoid: fp32 [B, 3, 16 h, 16 w] from the embedding [B, C, h, w]."""
@@ -251,17 +287,13 @@ class UNETRDecoder:
         zs = []
         z = x
         for d in self.deconv:
-            zs.append(self._conv(self._sampler(z, d["up"])[0], None, d["conv"], 3, True))
+            zs.append(conv(self._sampler(z, d["up"])[0], None, *d["conv"], 3, True, stats=True))
             z = zs[-1][0]
         h = self._block((x, None), None, self.base)
         for i in range(3):
             h = self._block(self._sampler(h[0], self.samplers[i]), zs[i], self.blocks[i])
         h = self._block(self._sampler(h[0], self.deconv_out), zs[3], self.head)[0]
-        B, H, W, C = h.shape
-        out = torch.empty(B, 3, H, W, device=self.device, dtype=torch.float32)
-        _lib.check(_lib.lib().msam_op_ais_head(_lib.ptr(h), B, H * W, C, _lib.ptr(self.out_w), _lib.ptr(self.out_b), _lib.ptr(out),
-                                               _lib.cur_stream()))
-        return out
+        return head_maps(h, self.out_w, self.out_b)
 
     def __call__(self, z12: torch.Tensor, input_size: Tuple[int, int], original_size: Tuple[int, int]) -> torch.Tensor:
         maps = self.forward_maps(z12)
@@ -327,9 +359,6 @@ def region_props(labels: torch.Tensor, n_ids: int) -> np.ndarray:
 
 
 # ------------------------------------------------------------------------------------------------ training
-BN_MOMENTUM = 0.1
-
-
 def default_decoder_state(emb=256, feats=(512, 256, 128, 64), deconv=(256, 128, 64, 64), head_in=64, transposed=False,
                           seed=0) -> Dict[str, torch.Tensor]:
     """A freshly initialised UNETR decoder (the production plan by default) with torch's default init, drawn from
@@ -416,35 +445,23 @@ class TrainableUNETRDecoder:
 
     # ---------------------------------------------------------------- operands
     def refresh(self):
-        """bf16 kernel operands from the fp32 masters."""
-        m, self.ops = self.masters, {}
+        """bf16 kernel operands from the fp32 masters: (forward weight, data-gradient weight) per convolution."""
+        m, self.ops, dev = self.masters, {}, self.device
         for k, w in m.items():
             if not k.endswith(".weight") or w.dim() != 4:
                 continue
             if w.shape[2:] == (3, 3):
-                cout, cin = w.shape[:2]
-                self.ops[k] = (w.permute(0, 2, 3, 1).reshape(cout, 9 * cin).to(torch.bfloat16).contiguous(),
-                               w.flip(2, 3).permute(1, 2, 3, 0).reshape(cin, 9 * cout).to(torch.bfloat16).contiguous())
+                self.ops[k] = (pack_conv3x3(w, dev), w.flip(2, 3).permute(1, 2, 3, 0).flatten(1).to(torch.bfloat16).contiguous())
             elif k.endswith(".block.weight") and w.shape[2:] == (2, 2):   # ConvTranspose2d [Cin, Cout, 2, 2]
-                cin, cout = w.shape[:2]
-                wk = w.permute(2, 3, 1, 0).reshape(4 * cout, cin)
-                self.ops[k] = (wk.to(torch.bfloat16).contiguous(), wk.t().to(torch.bfloat16).contiguous())
+                self.ops[k] = (pack_conv_transpose2x2(w, dev), w.permute(0, 2, 3, 1).flatten(1).to(torch.bfloat16).contiguous())
             elif k != "out_conv.weight":   # conv1x1 of the interpolation sampler
-                w2 = w[:, :, 0, 0]
-                self.ops[k] = (w2.to(torch.bfloat16).contiguous(), w2.t().to(torch.bfloat16).contiguous())
+                self.ops[k] = (pack_conv1x1(w, dev), w[:, :, 0, 0].t().to(torch.bfloat16).contiguous())
         self.out_w = m["out_conv.weight"][:, :, 0, 0].contiguous()
 
     # ---------------------------------------------------------------- kernels
     def _conv(self, x0, x1, w, b, ks, relu, transposed=False):
-        B, H, W, C0 = x0.shape
-        C1 = 0 if x1 is None else x1.shape[3]
-        cout = w.shape[0] // 4 if transposed else w.shape[0]
-        shape = (B, 2 * H, 2 * W, cout) if transposed else (B, H, W, cout)
-        out = torch.empty(shape, device=self.device, dtype=torch.bfloat16)
-        _lib.check(_lib.lib().msam_op_ais_conv(_lib.ptr(x0), C0, _lib.ptr(x1), C1, B, H, W, ks, _lib.ptr(w),
-                                               _lib.ptr(b if b is not None else self._zeros), cout, int(relu), int(transposed),
-                                               _lib.ptr(out), None, _lib.cur_stream()))
-        return out
+        """b None: a zero bias (the data-gradient convolutions)"""
+        return conv(x0, x1, w, b if b is not None else self._zeros, ks, relu, transposed)
 
     def _wgrad(self, dy, x0, x1, ks):
         L = _lib.lib()
@@ -466,18 +483,10 @@ class TrainableUNETRDecoder:
         _lib.check(_lib.lib().msam_op_ais_chan_sum(_lib.ptr(g), B, H * W, C, _lib.ptr(ws), ws.numel(), _lib.ptr(out), _lib.cur_stream()))
         return out
 
-    def _norm_fwd(self, x, per_image, gamma=None, beta=None, relu=False, run=None):
-        B, H, W, C = x.shape
-        ws = self._norm_ws(B, H * W, C)
-        mean = torch.empty(B * C if per_image else C, device=self.device, dtype=torch.float32)
-        rstd = torch.empty_like(mean)
-        out = torch.empty_like(x)
-        rm, rv = (None, None) if run is None else run
-        _lib.check(_lib.lib().msam_op_ais_norm_forward(_lib.ptr(x), B, H * W, C, int(per_image), _lib.ptr(gamma), _lib.ptr(beta),
-                                                       BN_EPS if not per_image else IN_EPS, int(relu), BN_MOMENTUM, _lib.ptr(rm),
-                                                       _lib.ptr(rv), _lib.ptr(ws), ws.numel(), _lib.ptr(mean), _lib.ptr(rstd),
-                                                       _lib.ptr(out), _lib.cur_stream()))
-        return out, mean, rstd
+    @staticmethod
+    def _norm_fwd(x, per_image, gamma=None, beta=None, relu=False, run=None):
+        """-> (out, mean, rstd)"""
+        return norm(x, per_image, gamma, beta, relu=relu, run=run, keep=True)
 
     def _norm_bwd(self, x, dy, dy_off, ldd, mean, rstd, per_image, gamma=None, relu_out=None, in_mask=False, dx=None, out_mode=0,
                   dgb=False):
@@ -507,11 +516,7 @@ class TrainableUNETRDecoder:
         b = self.masters[key + ".bias"]
         if self.transposed:
             return self._conv(z, None, w, b, 1, False, transposed=True), (p, z)
-        u = self._conv(z, None, w, b, 1, False)
-        B, H, W, C = u.shape
-        s = torch.empty(B, 2 * H, 2 * W, C, device=self.device, dtype=torch.bfloat16)
-        _lib.check(_lib.lib().msam_op_ais_upsample2(_lib.ptr(u), B, H, W, C, _lib.ptr(s), _lib.cur_stream()))
-        return s, (p, z)
+        return upsample2(self._conv(z, None, w, b, 1, False)), (p, z)
 
     def _sampler_bwd(self, g, saved):
         """g: bf16 d(sampler output) -> bf16 d(sampler input)"""
@@ -639,10 +644,7 @@ class TrainableUNETRDecoder:
             blocks.append(bsv)
         s, osv = self._sampler_fwd(h, "deconv_out")
         h, hsv = self._block_fwd(s, zs[3], "decoder_head")
-        B, H, W, C = h.shape
-        maps = torch.empty(B, 3, H, W, device=self.device, dtype=torch.float32)
-        _lib.check(_lib.lib().msam_op_ais_head(_lib.ptr(h), B, H * W, C, _lib.ptr(self.out_w), _lib.ptr(self.masters["out_conv.bias"]),
-                                               _lib.ptr(maps), _lib.cur_stream()))
+        maps = head_maps(h, self.out_w, self.masters["out_conv.bias"])
         self._saved = dict(x=x, zs=zs, deconv=dsaved, blocks=blocks, samplers=samplers, out=osv, head=hsv, h=h, maps=maps)
         return maps
 

@@ -95,31 +95,31 @@ def test_conv1x1_and_transposed(transposed):
 
 
 @pytest.mark.parametrize("affine", [False, True])
-def test_instance_norm_against_float64(affine):
+def test_norm_forward_instance_norm_against_float64(affine):
     g = torch.Generator().manual_seed(4)
     B, H, W, C = 2, 96, 80, 128
     x = (torch.randn(B, H, W, C, generator=g) * 3 + torch.randn(1, 1, 1, C, generator=g)).to(DEV, torch.bfloat16)
     gam, bet = (torch.rand(C, generator=g) + 0.5).to(DEV), torch.randn(C, generator=g).to(DEV)
     L = _lib.lib()
-    ws = torch.empty(int(L.msam_ais_instnorm_workspace(B, H * W, C)), device=DEV, dtype=torch.uint8)
+    ws = torch.empty(int(L.msam_ais_norm_workspace(B, H * W, C)), device=DEV, dtype=torch.uint8)
     out = torch.empty_like(x)
     gp, bp = (_lib.ptr(gam), _lib.ptr(bet)) if affine else (None, None)
-    _lib.check(L.msam_op_ais_instnorm(_lib.ptr(x), B, H * W, C, None, 0, gp, bp, 1e-5, _lib.ptr(ws), ws.numel(), _lib.ptr(out),
-                                      _lib.cur_stream()))
+    _lib.check(L.msam_op_ais_norm_forward(_lib.ptr(x), B, H * W, C, 1, None, 0, gp, bp, 1e-5, 0, 0.1, None, None, _lib.ptr(ws),
+                                          ws.numel(), None, None, _lib.ptr(out), _lib.cur_stream()))
     ref = F.instance_norm(x.double().permute(0, 3, 1, 2), weight=gam.double() if affine else None,
                           bias=bet.double() if affine else None, eps=1e-5).permute(0, 2, 3, 1)
     assert float((out.double() - ref).abs().max()) < 3e-2
     out2 = torch.empty_like(x)
-    _lib.check(L.msam_op_ais_instnorm(_lib.ptr(x), B, H * W, C, None, 0, gp, bp, 1e-5, _lib.ptr(ws), ws.numel(), _lib.ptr(out2),
-                                      _lib.cur_stream()))
+    _lib.check(L.msam_op_ais_norm_forward(_lib.ptr(x), B, H * W, C, 1, None, 0, gp, bp, 1e-5, 0, 0.1, None, None, _lib.ptr(ws),
+                                          ws.numel(), None, None, _lib.ptr(out2), _lib.cur_stream()))
     assert torch.equal(out, out2)
     # with partial sums from a convolution epilogue (the decoder's path): the same normalisation
     wk = torch.eye(C).to(DEV, torch.bfloat16).contiguous()
     y, st = _conv(x, None, wk, torch.zeros(C, device=DEV), 1, 0, stats=True)
     assert torch.equal(y, x)
     out3 = torch.empty_like(x)
-    _lib.check(L.msam_op_ais_instnorm(_lib.ptr(x), B, H * W, C, _lib.ptr(st), st.numel() // (2 * B * C), gp, bp, 1e-5,
-                                      _lib.ptr(ws), ws.numel(), _lib.ptr(out3), _lib.cur_stream()))
+    _lib.check(L.msam_op_ais_norm_forward(_lib.ptr(x), B, H * W, C, 1, _lib.ptr(st), st.numel() // (2 * B * C), gp, bp, 1e-5, 0,
+                                          0.1, None, None, _lib.ptr(ws), ws.numel(), None, None, _lib.ptr(out3), _lib.cur_stream()))
     assert float((out3.double() - ref).abs().max()) < 3e-2
 
 
@@ -269,7 +269,7 @@ def test_refusals(tmp_path):
         ps.precompute_state(str(tmp_path), str(tmp_path / "out"), model_type="vit_test", checkpoint_path=_checkpoint(tmp_path))
 
 
-def test_ops_reject_bad_arguments():
+def test_ais_ops_reject_bad_arguments():
     L = _lib.lib()
     x = torch.zeros(1, 8, 8, 64, device=DEV, dtype=torch.bfloat16)
     w = torch.zeros(64, 9 * 64, device=DEV, dtype=torch.bfloat16)
@@ -284,10 +284,13 @@ def test_ops_reject_bad_arguments():
     assert L.msam_op_ais_conv(p(x), 64, None, 32, 1, 8, 8, 3, p(w), p(b), 64, 1, 0, p(o), None, s) != 0
     assert L.msam_op_ais_conv(ctypes.c_void_p(x.data_ptr() + 2), 64, None, 0, 1, 8, 8, 3, p(w), p(b), 64, 1, 0, p(o), None, s) != 0
     ws = torch.zeros(16, device=DEV, dtype=torch.uint8)
-    assert L.msam_op_ais_instnorm(p(x), 1, 64, 64, None, 0, None, None, 1e-5, p(ws), ws.numel(), p(o), s) != 0   # workspace too small
-    assert L.msam_op_ais_instnorm(p(x), 1, 64, 60, None, 0, None, None, 1e-5, p(ws), 1 << 20, p(o), s) != 0
-    assert L.msam_op_ais_instnorm(p(x), 1, 64, 64, None, 0, p(b), None, 1e-5, p(ws), 1 << 20, p(o), s) != 0
-    assert L.msam_op_ais_instnorm(p(x), 1, 64, 64, p(ws), 0, None, None, 1e-5, p(ws), 1 << 20, p(o), s) != 0   # stats, 0 chunks
+    def norm(C, stats, nchunk, gamma, ws_bytes):
+        return L.msam_op_ais_norm_forward(p(x), 1, 64, C, 1, stats, nchunk, gamma, None, 1e-5, 0, 0.1, None, None, p(ws), ws_bytes,
+                                          None, None, p(o), s)
+    assert norm(64, None, 0, None, ws.numel()) != 0   # workspace too small
+    assert norm(60, None, 0, None, 1 << 20) != 0
+    assert norm(64, None, 0, p(b), 1 << 20) != 0
+    assert norm(64, p(ws), 0, None, 1 << 20) != 0   # stats, 0 chunks
     assert L.msam_op_ais_upsample2(p(x), 1, 8, 8, 12, p(o), s) != 0
     assert L.msam_op_ais_upsample2(None, 1, 8, 8, 64, p(o), s) != 0
     assert L.msam_op_ais_head(p(x), 1, 64, 1024, p(b), p(b), p(b), s) != 0

@@ -1,6 +1,8 @@
 """Training of the UNETR (AIS) decoder on the GPU: each csrc/ais_train.cu op against float64, the whole decoder backward against
 the float64 training-mode restatement (tests/unetr_train_ref.py), determinism, the AdamW step, a short training run with export
 and reload through get_predictor_and_decoder, and the argument checks."""
+import ctypes
+
 import numpy as np
 import pytest
 import torch
@@ -430,7 +432,7 @@ def test_joint_iteration_steps_the_right_tensors():
     assert torch.isfinite(li) and torch.isfinite(lu) and set(net.decoder.steps.values()) == {2}
 
 
-def test_ops_reject_bad_arguments():
+def test_training_ops_reject_bad_arguments():
     L = _lib.lib()
     t = torch.zeros(4096, device=DEV, dtype=torch.bfloat16)
     f = torch.zeros(4096, device=DEV)
@@ -439,10 +441,14 @@ def test_ops_reject_bad_arguments():
     assert L.msam_op_ais_wgrad(_lib.ptr(t), 64, _lib.ptr(t), 64, None, 0, 1, 8, 8, 2, _lib.ptr(f), 1 << 30, _lib.ptr(f), st) != 0
     assert L.msam_op_ais_wgrad(_lib.ptr(t), 64, _lib.ptr(t), 64, None, 0, 1, 8, 8, 3, _lib.ptr(f), 16, _lib.ptr(f), st) != 0
     assert L.msam_op_ais_wgrad(None, 64, _lib.ptr(t), 64, None, 0, 1, 8, 8, 3, _lib.ptr(f), 1 << 30, _lib.ptr(f), st) != 0
-    assert L.msam_op_ais_norm_forward(_lib.ptr(t), 1, 64, 12, 1, None, None, 1e-5, 0, 0.1, None, None, _lib.ptr(f), 1 << 20,
+    assert L.msam_op_ais_norm_forward(_lib.ptr(t), 1, 64, 12, 1, None, 0, None, None, 1e-5, 0, 0.1, None, None, _lib.ptr(f), 1 << 20,
                                       _lib.ptr(f), _lib.ptr(f), _lib.ptr(t), st) != 0
-    assert L.msam_op_ais_norm_forward(_lib.ptr(t), 1, 64, 64, 1, None, None, 1e-5, 0, 0.1, _lib.ptr(f), _lib.ptr(f), _lib.ptr(f),
-                                      1 << 20, _lib.ptr(f), _lib.ptr(f), _lib.ptr(t), st) != 0   # running statistics on an InstanceNorm
+    assert L.msam_op_ais_norm_forward(_lib.ptr(t), 1, 64, 64, 1, None, 0, None, None, 1e-5, 0, 0.1, _lib.ptr(f), _lib.ptr(f),
+                                      _lib.ptr(f), 1 << 20, _lib.ptr(f), _lib.ptr(f), _lib.ptr(t), st) != 0   # running statistics on an InstanceNorm
+    assert L.msam_op_ais_norm_forward(_lib.ptr(t), 1, 64, 64, 1, None, 0, None, None, 1e-5, 0, 0.1, None, None, _lib.ptr(f), 1 << 20,
+                                      _lib.ptr(f), None, _lib.ptr(t), st) != 0   # mean without rstd
+    assert L.msam_op_ais_norm_forward(_lib.ptr(t), 1, 64, 64, 1, ctypes.c_void_p(f.data_ptr() + 4), 1, None, None, 1e-5, 0, 0.1,
+                                      None, None, _lib.ptr(f), 1 << 20, None, None, _lib.ptr(t), st) != 0   # misaligned statistics
     assert L.msam_op_ais_norm_backward(_lib.ptr(t), 64, _lib.ptr(t), 0, 32, None, 1, 64, 64, 1, None, _lib.ptr(f), _lib.ptr(f), 0,
                                        _lib.ptr(f), 1 << 20, _lib.ptr(t), 0, 64, None, None, st) != 0   # ldd < C
     assert L.msam_op_ais_upsample2_backward(_lib.ptr(t), 1, 4, 4, 12, _lib.ptr(t), st) != 0
